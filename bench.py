@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the DEVA propagation hot path on B200 (contract: see the task statement / DESIGN.md).
+"""Benchmark of the DEVA propagation hot path on an H100 (see DESIGN.md).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c3|c2]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c3|c2] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[2], "c3"): synthetic 1080p frames (padded 1088x1920, Q = 8160 query
 positions), 16 objects, memory bank pre-filled to 10 000 slots, full encode -> read -> decode per frame
@@ -17,17 +17,22 @@ Printed JSON line: metric/value/unit/... plus
   e2e           same FPS through the public API with host frames (pinned H2D of every frame, D2H of the id mask);
   cpu_baseline  the UNMODIFIED reference (oracle/_ref, staged by oracle/build_ref.py) on this box's host cores, on a
                 bounded sample (all shared stages + `--ref-objects` of the K objects, linearly extrapolated and flagged);
-  torch_gpu_baseline  the unmodified reference on the SAME B200 (all K objects): fp32 (PyTorch's TF32 default), fp32
+  torch_gpu_baseline  the unmodified reference on the SAME GPU (all K objects): fp32 (PyTorch's TF32 default), fp32
                 with TF32 off, and --amp (fp16 autocast, evaluation/eval_vos.py:137) - the real bar;
   clocks        SM clock / throttle reasons sampled with nvidia-smi during the timed region.
 ``--impl reference`` times the reference's own ``DEVAInferenceCore.step`` on the host cores (``oracle/_ref``; the
 oracle port only when the staged copy is missing).
+``--dump-outputs DIR``: after the timed steps, the probabilities the last timed step returned are written to DIR as
+float32 .npy files (see dump_outputs), so that two builds can be compared output for output on identical seeded inputs.
 """
+import sys
+
+sys.dont_write_bytecode = True  # the tree may be read-only: nothing is cached next to the sources
+
 import argparse
 import json
 import os
 import subprocess
-import sys
 import tempfile
 import time
 
@@ -206,6 +211,7 @@ class Clip:
         p = self.core.step(self.frames_dev[self.i % 5])
         self.clamp()
         self.i += 1
+        self.last = p
         return p
 
     def step_e2e(self):
@@ -263,6 +269,28 @@ class ClipSet:
 
 HOST_MS = []  # host time (enqueue only, no sync) of every timed step of the last timed() call: a stall of the launching
               # thread (GC, scheduler, allocator) longer than the GPU's queued work shows up in the event time as well
+
+
+DUMP_CAP_BYTES = 64_000_000  # all files of --dump-outputs together
+
+
+def dump_outputs(clip, out_dir):
+    """What the last timed step returned to its caller (rank 0's clip; the first clip of a clip set): the id map (argmax
+    over the objects) at every pixel, and the probabilities [K+1, H, W] on the lattice of every s-th row and column, with
+    the smallest s that keeps both files within DUMP_CAP_BYTES (s = 2 for c3, 3 for c5).  float32."""
+    import numpy as np
+    c = clip.clips[0] if hasattr(clip, 'clips') else clip
+    prob = c.last.float()
+    ids = torch.argmax(prob, dim=0).float().cpu().numpy()
+    k1, h, w = prob.shape
+    s = 1
+    while k1 * (-(-h // s)) * (-(-w // s)) * 4 + ids.nbytes + 256 > DUMP_CAP_BYTES:
+        s += 1
+    lattice = prob[:, ::s, ::s].contiguous().cpu().numpy()
+    assert lattice.nbytes + ids.nbytes + 256 <= DUMP_CAP_BYTES, (lattice.nbytes, ids.nbytes)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, f'prob_stride{s}.npy'), lattice)
+    np.save(os.path.join(out_dir, 'ids.npy'), ids)
 
 
 def timed(fn, steps, dist_on):
@@ -356,6 +384,8 @@ def run_ours(args):
     read_ms = sum(a.elapsed_time(b) for a, b in ev) / max(len(ev), 1)
     clocks = sampler.stop() if sampler else None
     host_ms = sorted(HOST_MS)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(clip, args.dump_outputs)
 
     for _ in range(2):
         clip.step_e2e()
@@ -390,22 +420,16 @@ def run_ours(args):
             peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
         except Exception:
             pass
-        peak = peaks.get('bf16_tflops_sustained', 1400.0)
+        peak = peaks.get('bf16_tflops_sustained', 989.0)
         peak_src = 'MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)' if peaks else \
-            'fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)'
+            'H100 SXM data sheet, dense BF16 (989 TFLOP/s at 700 W; not a measured rate)'
         flops = read_flops(wl, clip.q)
         achieved = flops / (read_ms * 1e-3) / 1e12
         if wl.get('sharded'):  # every rank multiplies 1/world of the slots: per-GPU rate against one GPU's peak
             achieved /= world
-        traffic = conv_traffic = None
-        try:
-            tr = json.load(open(os.path.join(ROOT, 'profiles', 'roofline_traffic.json')))
-            traffic = tr.get(args.workload)  # readout_sparse_kernel, per launch
-            conv_traffic = tr.get(args.workload + '_conv')
-        except Exception:
-            pass
+        traffic = conv_traffic = None  # DRAM bytes of the kernels: not measured on H100
         conv_ach = conv_flops / (conv_ms * 1e-3) / 1e12 if not args.quick else 0.0
-        conv_roof = None if args.quick else {'kernel': 'conv_kernel (tcgen05 implicit GEMM), all launches of a frame', 'bound': 'tensor',
+        conv_roof = None if args.quick else {'kernel': 'conv_kernel (wgmma implicit GEMM), all launches of a frame', 'bound': 'tensor',
                      'achieved': conv_ach, 'peak': peak, 'unit': 'TFLOP/s', 'frac': conv_ach / peak,
                      'traffic': conv_traffic, 'ms_per_frame': conv_ms, 'flops_per_frame': conv_flops,
                      'what': 'algorithmic FLOPs 2*B*Ho*Wo*Cout*k*k*Cin per layer (extra split-precision passes NOT counted) / '
@@ -417,11 +441,10 @@ def run_ours(args):
             'metric': METRIC, 'value': frames_per_step * args.steps / (ms * 1e-3), 'unit': 'frames/s', 'n_gpus': world,
             'steps': args.steps, 'warmup': n_warm, 'ms_per_step': ms / args.steps,
             'higher_is_better': True, 'scaling': scaling, 'vs_baseline': None, 'dtype': 'f16 MMA operands / f32 accumulate '
-            f'(tcgen05 memory read + conv stack), precision plan {precision!r}; key path split-f16x3 (~f32)', 'data': 'synthetic',
+            f'(wgmma memory read + conv stack), precision plan {precision!r}; key path split-f16x3 (~f32)', 'data': 'synthetic',
             'config': workload_config(wl, clip.q, world), 'setup_steps': 1 + n_prime,
-            'roofline': {'kernel': 'fused affinity path: pack_query + sim_topk(tcgen05 fp16x3) + merge + bucket + readout_sparse(tcgen05, '
-                                   'affinity tiles built in smem); traffic = DRAM bytes of readout_sparse_kernel (ncu, the fp16 '
-                                   'token-major output variant the step runs)',
+            'roofline': {'kernel': 'fused affinity path: pack_query + sim_topk(wgmma fp16x3) + merge + bucket + readout_sparse(wgmma, '
+                                   'affinity tiles built in smem)',
                          'bound': 'tensor', 'achieved': achieved, 'peak': peak, 'unit': 'TFLOP/s',
                          'frac': achieved / peak, 'traffic': traffic, 'peak_source': peak_src,
                          'ms_per_launch': read_ms, 'flops_per_launch': flops},
@@ -552,18 +575,20 @@ def workload_config(wl, q, world):
     return {'workload': wl['name'], 'frame': [wl['h'], wl['w']], 'query_positions': q, 'objects': wl['k'],
             'memory_slots': wl['n'], 'mem_every': 5, 'top_k': TOP_K,
             'parallelism': f'clip-parallel x{world}' if world > 1 else 'single clip',
-            'l2': 'per-step working set (activations > 2 GB) exceeds the 126 MB L2; no explicit flush',
+            'l2': 'per-step working set (activations > 2 GB) exceeds the 50 MB L2; no explicit flush',
             'weights': 'synthetic_state_dict(seed=0), real architecture (69.2 M parameters)'}
 
 
 class RefClip:
     """The same clip as ``Clip`` driven through the UNMODIFIED reference (DEVA + DEVAInferenceCore from oracle/_ref):
-    same seeded frames, masks, checkpoint and random bank top-up; ``n_obj`` of the workload's objects."""
-    def __init__(self, wl, device, n_obj, seed):
+    same seeded frames, masks, checkpoint and random bank top-up; ``n_obj`` of the workload's objects, decoded / encoded /
+    read out ``chunk_size`` objects at a time (-1: all at once; the reference's chunking only splits the object batch)."""
+    def __init__(self, wl, device, n_obj, seed, chunk_size=-1):
         from oracle import ref_loader
         DEVA, Core, synth = ref_loader.load()
         self.wl, self.device, self.n_obj = wl, device, n_obj
         cfg = base_config()
+        cfg['chunk_size'] = chunk_size
         net = DEVA(cfg).to(device).eval()
         net.load_weights({k: v.to(device) for k, v in synth(seed=0).items()})
         self.net = net
@@ -689,13 +714,23 @@ def reference_cpu(wl, steps, warmup, n_obj, budget_s=150.0):
             'q': clip.q}
 
 
+# Objects per batch of the reference's decoder / value encoder / readout in the GPU leg.  All 16 objects of c3 at once need
+# more memory in fp32 than an 80 GB H100 has; the reference's own chunk_size option (eval_args.py) processes them in
+# batches of this many with the same result, which keeps the leg inside 80 GB.
+REF_GPU_CHUNK = 4
+
+
 def reference_gpu(wl, device, steps=5, warmup=2):
-    """SURVEY 8(d) "GPU-side comparison": the UNMODIFIED reference on the same B200, all K objects, through its public
+    """SURVEY 8(d) "GPU-side comparison": the UNMODIFIED reference on the same GPU, all K objects, through its public
     step(): fp32 under PyTorch's default TF32 policy (what a user of the reference gets), fp32 with TF32 forbidden
-    (the precision the 1e-3 parity contract is written against) and --amp (evaluation/eval_vos.py:137)."""
+    (the precision the 1e-3 parity contract is written against) and --amp (evaluation/eval_vos.py:137).  Objects are
+    processed REF_GPU_CHUNK at a time (chunk_size), so that the fp32 modes fit in 80 GB."""
     torch.set_grad_enabled(False)
     out = {'kind': 'unmodified reference (oracle/_ref) on cuda', 'objects': wl['k'], 'steps': steps, 'warmup': warmup,
-           'sample': f'{steps} frames {wl["h"]}x{wl["w"]} incl. one memory frame, N={wl["n"]}, all {wl["k"]} objects'}
+           'chunk_size': REF_GPU_CHUNK,
+           'sample': f'{steps} frames {wl["h"]}x{wl["w"]} incl. one memory frame, N={wl["n"]}, all {wl["k"]} objects, '
+                     f'chunk_size={REF_GPU_CHUNK} (objects decoded / encoded / read out {REF_GPU_CHUNK} at a time to fit 80 GB; '
+                     f'same result as all at once)'}
     torch.backends.cudnn.benchmark = True
     for mode in ('fp32_tf32_default', 'fp32_strict', 'amp_fp16'):
         torch.backends.cudnn.allow_tf32 = mode != 'fp32_strict'
@@ -704,7 +739,7 @@ def reference_gpu(wl, device, steps=5, warmup=2):
             torch.backends.cuda.matmul.allow_tf32 = False
         try:
             with torch.autocast('cuda', dtype=torch.float16, enabled=(mode == 'amp_fp16')):
-                clip = RefClip(wl, device, wl['k'], seed=100)
+                clip = RefClip(wl, device, wl['k'], seed=100, chunk_size=REF_GPU_CHUNK)
                 for _ in range(warmup):
                     clip.step()
                 torch.cuda.synchronize()
@@ -815,6 +850,8 @@ if __name__ == '__main__':
     ap.add_argument('--quick', action='store_true', help='value + e2e only (no fused-io e2e, no conv roofline pass)')
     ap.add_argument('--workload', default='c3', choices=list(WORKLOADS))
     ap.add_argument('--no-torch-baseline', action='store_true', help='skip the stock-PyTorch-on-GPU comparison pass')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step to DIR/<name>.npy (float32, at most 64 MB in all)')
     ap.add_argument('--no-c5-leg', action='store_true',
                     help='N > 1 only: skip the bank-sharded single-video leg (workload c5 on the same ranks, key bank_sharded_c5)')
     a = ap.parse_args()

@@ -1,5 +1,5 @@
 /*
- * deva_b200 - C ABI of the B200-native temporal-propagation kernels behind DEVA's
+ * deva_b200 - C ABI of the H100-native temporal-propagation kernels behind DEVA's
  * DEVAInferenceCore.step / MemoryManager API.
  *
  * The reference (hkchengrex/Tracking-Anything-with-DEVA @ 404a112) is pure Python/PyTorch and has no
@@ -45,7 +45,7 @@ DEVA_B200_API int deva_b200_abi_version(void);
 DEVA_B200_API const char* deva_b200_last_error(void);
 /* Number of kernels this library has launched in the calling process (bench.py reports it). */
 DEVA_B200_API uint64_t deva_b200_launch_count(void);
-/* 0 when the current CUDA device can run the sm_100a kernels. */
+/* 0 when the current CUDA device can run the sm_90a kernels. */
 DEVA_B200_API int deva_b200_device_check(void);
 
 /* ---- query side ------------------------------------------------------------------------------------

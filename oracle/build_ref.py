@@ -10,7 +10,7 @@ here (the build backend ``hatchling`` is absent and there is no index); outcome 
 
 What uses it (test infrastructure / reported baselines only, never the product path):
   * ``bench.py --impl reference``      - the reference's own ``DEVAInferenceCore.step`` on the host cores;
-  * ``bench.py``'s ``torch_gpu_baseline`` - the same unmodified code on the same B200 (fp32, fp32 without TF32, --amp).
+  * ``bench.py``'s ``torch_gpu_baseline`` - the same unmodified code on the same H100 (fp32, fp32 without TF32, --amp).
 ``oracle/ref_loader.py`` imports it in a process that never imports the product's ``deva`` package.
 """
 import hashlib

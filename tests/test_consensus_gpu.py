@@ -1,5 +1,5 @@
 """GPU parity of the in-clip consensus (SURVEY 8f-1) against reference-minted fixtures: spatial_alignment and the
-established-association average (floating point, through the B200 kernels) and the automatic association's voting
+established-association average (floating point, through the H100 kernels) and the automatic association's voting
 logic (integer: bit-exact ids)."""
 import importlib.util
 import json

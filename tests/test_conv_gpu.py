@@ -34,8 +34,8 @@ CASES = [
     (2, 16, 24, 256, 256, 3, 1),
     (1, 11, 19, 512, 129, 3, 1),   # key_proj-like ragged Cout (fp32 out)
     (2, 24, 40, 256, 1, 3, 1),     # pred-like single channel (fp32 out)
-    # enough tiles (>= 2 x 148) for the cluster launches: deep K -> tcgen05 CTA pairs (cta_group::2),
-    # shallow K -> weight multicast only; odd tile counts exercise the clamped "phantom" tile of a pair
+    # more tiles than SMs (132): several tiles per persistent CTA, the producer filling the ring for the next tile while
+    # the consumers run the epilogue of the current one; odd tile counts leave a partial last wave
     (2, 136, 240, 128, 256, 3, 1),
     (5, 67, 119, 192, 320, 3, 1),
     (11, 100, 150, 128, 128, 3, 2),
@@ -145,7 +145,7 @@ def test_conv_two_inputs():
     assert float((_nchw(out) - ref).abs().max()) < 2e-3
 
 
-@pytest.mark.parametrize('b,h,w', [(2, 9, 12), (16, 68, 60)])  # small: cta_group::1; large: CTA pairs
+@pytest.mark.parametrize('b,h,w', [(2, 9, 12), (16, 68, 60)])  # small: one tile per CTA; large: several
 def test_conv_gate_epilogue(b, h, w):
     """Sensory update (modules.py:145-149): h' = f*h*(1-u) + u*tanh(n) from the fp32 accumulators of the 3x3 conv
     over cat[g, h]; the 3C-channel conv output is never written."""

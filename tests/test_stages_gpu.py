@@ -1,8 +1,8 @@
 """Stage-by-stage GPU parity of the native network kernels against the reference-minted per-stage fixture
 (tests/golden/network_stages.npz: encode_image, transform_key, encode_mask, segment of the UNMODIFIED reference on one
 64x80 frame with two objects).  Every stage gets the FIXTURE's inputs, so a regression shows up in the stage that owns
-it instead of as a clip-level drift.  Bounds: ~2x what the kernels measure on B200 (printed), all tighter than what a
-single wrong layer produces (> 1e-1)."""
+it instead of as a clip-level drift.  The measured errors are printed; the bounds are all tighter than what a single wrong
+layer produces (> 1e-1)."""
 import os
 
 import numpy as np

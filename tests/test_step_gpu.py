@@ -19,7 +19,7 @@ def _core(cfg, sd, backend):
     return DEVAInferenceCore(net, cfg)
 
 
-# 'native': every layer on the hand-written sm_100a kernels (fp16 MMA operands, fp32 accumulate, the default 'parity'
+# 'native': every layer on the hand-written sm_90a kernels (fp16 MMA operands, fp32 accumulate, the default 'parity'
 # precision plan); 'torch': the same graphs through cuDNN fp32 (isolates the memory-read kernels).
 # Both are held to north_star's 1e-3 max-abs against the fp32 reference.
 @pytest.mark.parametrize('backend,tol', [('native', 1e-3), ('torch', 1e-3)])

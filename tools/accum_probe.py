@@ -1,6 +1,6 @@
 """GPU probe: how accurate is the split-precision (3-pass fp16 hi/lo) convolution, and is the residual error the tensor
 core's fp32 accumulation?  Compares one deep-K conv against fp64, whole and as a sum of K-chunks added in fp32 on the
-CUDA cores (if the chunked sum is markedly better, in-TMEM accumulation is what limits the key path)."""
+CUDA cores (if the chunked sum is markedly better, in-register accumulation is what limits the key path)."""
 import os
 import sys
 

@@ -50,7 +50,7 @@ if __name__ == '__main__':
     out = {}
     for name, backend, tf32 in (('cudnn fp32 (TF32 forbidden)', 'torch', False),
                                 ('cudnn fp32, PyTorch default (TF32 allowed)', 'torch', True),
-                                ('native sm_100a kernels (fp16 operands, fp32 accumulate)', 'native', False)):
+                                ('native sm_90a kernels (fp16 operands, fp32 accumulate)', 'native', False)):
         worst, per_frame = run(backend, tf32)
         out[name] = {'max_abs_prob_err': worst, 'per_frame': per_frame}
         print(f'{name:60s} max |prob - golden| = {worst:.3e}', flush=True)

@@ -29,7 +29,9 @@ DEVA_B200_API int deva_b200_device_check(void) {
   int dev = 0, major = 0;
   B200_CUDA(cudaGetDevice(&dev));
   B200_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  B200_REQUIRE(major == 10, "deva_b200 kernels are built for sm_100a; device has compute capability major %d", major);
+  int minor = 0;
+  B200_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+  B200_REQUIRE(major == 9 && minor == 0, "deva_b200 kernels are built for sm_90a; device has compute capability %d.%d", major, minor);
   return 0;
 }
 

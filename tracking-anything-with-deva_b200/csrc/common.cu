@@ -32,7 +32,7 @@ int sm_count() {
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       cached[dev] = n;
     else
-      cached[dev] = 148;
+      cached[dev] = 132;  // H100 SXM
   }
   return cached[dev];
 }

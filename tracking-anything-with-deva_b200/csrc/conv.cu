@@ -1,23 +1,24 @@
-// Implicit-GEMM convolution on tcgen05, NHWC fp16 activations, fp32 accumulation in TMEM.
+// Implicit-GEMM convolution on wgmma, NHWC fp16 activations, fp32 accumulation in registers.
 // Replaces the nn.Conv2d + BatchNorm(eval) + ReLU (+ residual add) call chains of the reference network
 // (deva/model/resnet.py:46-152, big_modules.py:23-212, modules.py:22-169, group_modules.py:41-67).
 //
 //   D[pixel, cout] = sum_{tap, cin} X[b, y*s + dy(tap), x*s + dx(tap), cin] * W[cout, tap, cin]
 //
-//   M = 128 output pixels = a TH x TW rectangle of one image (TMEM lanes)
-//   N = NT output channels (<= 256, TMEM columns), K = 64 input channels of one filter tap per k-iteration.
+//   M = 128 output pixels = a TH x TW rectangle of one image, N = NT output channels (<= 256),
+//   K = 64 input channels of one filter tap per k-iteration.
 //
 // A operand: the activation tensor is described to TMA as a rank-5 tiled tensor (C, W, H, B, 1); the box
 //   (64, TW, TH, 1, 1) lands in shared memory as 128 rows of 128 bytes in exactly the 128B-swizzled K-major
-//   layout tcgen05 wants.  A filter tap is just a shifted box origin; convolution padding is TMA's
+//   layout wgmma wants.  A filter tap is just a shifted box origin; convolution padding is TMA's
 //   out-of-bounds zero fill (also for negative coordinates).  Stride-2 convolutions use one tensor map per
 //   input phase (y%2, x%2) over the same memory, so every tap is again a unit-stride box.
 // B operand: weights packed [Cout_pad, taps * Cin_pad] fp16 (K-major), 2-D TMA.
-// Epilogue (TMEM -> registers): + bias (folded BatchNorm), + optional residual (own or batch-broadcast),
-//   + optional rank-1 term w1[cout] * x1[b, pixel] (the "+1" mask / logit input channel of
+// Epilogue (straight from the accumulator registers): + bias (folded BatchNorm), + optional residual (own or
+//   batch-broadcast), + optional rank-1 term w1[cout] * x1[b, pixel] (the "+1" mask / logit input channel of
 //   sensory_compress and g4_conv), then writes any of: raw fp16, ReLU'd fp16, raw fp32.
-// Warp roles: 0 = TMA producer, 1 = MMA issuer / TMEM owner, 2..9 = epilogue (two warps per TMEM lane quadrant, even /
-//   odd 32-column chunks).  Persistent CTAs, 4-stage smem ring (6-stage in CTA-pair mode), double-buffered accumulators.
+// Warp roles: warps 0..7 = two consumer warpgroups (pixels 0..63 / 64..127 of the tile: wgmma m64nNk16 + epilogue),
+//   warp 8 = TMA producer.  Persistent CTAs, 4-stage shared-memory ring; the producer fills the ring for the next
+//   tile while the consumers run the epilogue of the current one.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
@@ -34,25 +35,13 @@ constexpr int STAGES = 4;
 constexpr int A_BYTES = BM * BK * 2;
 constexpr int B_BYTES_MAX = 256 * BK * 2;
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES_MAX;
-// CTA-pair mode (tcgen05 cta_group::2): each CTA stages its own 128 pixels and HALF of the weight tile, so a stage is
-// 32 KB instead of 48 KB and the same shared memory holds a 6-deep ring.
-constexpr int PAIR_STAGES = 6;
-constexpr int PAIR_STAGE_BYTES = A_BYTES + B_BYTES_MAX / 2;
-static_assert(PAIR_STAGES * PAIR_STAGE_BYTES == STAGES * STAGE_BYTES, "both modes share one shared-memory layout");
 constexpr int RING_BYTES = STAGES * STAGE_BYTES;
-// Warp roles: 0 = TMA producer, 1 = MMA issuer, 2..9 = epilogue.  EIGHT epilogue warps: a warp may only read its own TMEM
-// lane quadrant (warp % 4), so two warps share a quadrant and take the even / odd 32-column chunks of the accumulator.
-// With one epilogue warp per scheduler every dependent instruction paid its full latency (ncu: the MMA warp spinning on
-// acc_empty, stall_wait / long_scoreboard / branch_resolving spread over the whole epilogue) and the shallow-K layers ran
-// at 2 400 cycles per chunk; two warps per scheduler overlap each other's latencies.
-constexpr int EPI_WARPS = 8;
-constexpr int EPI_THREADS = EPI_WARPS * 32;
-constexpr int THREADS = 64 + EPI_THREADS;
+constexpr int CONSUMER_THREADS = 256;  // two warpgroups; wgmma needs warpgroups aligned to warp 0, 4, ...
+constexpr int THREADS = CONSUMER_THREADS + 32;
 constexpr int HEAD_BYTES = kMaxHead * 256 * 4;
 constexpr int kMaxBias = 2048;   // bias of the whole layer staged in shared memory (Cout_pad <= kMaxBias)
 constexpr int kMaxRank1 = 1024;  // same for the rank-1 input column
-constexpr int HX_BYTES = 2 * BM * kMaxHead * 4;  // fused head: partial sums handed from the odd-chunk to the even-chunk warps
-constexpr int SMEM_BYTES = RING_BYTES + 256 + HEAD_BYTES + kMaxBias * 4 + kMaxRank1 * 4 + HX_BYTES;
+constexpr int SMEM_BYTES = RING_BYTES + 256 + HEAD_BYTES + kMaxBias * 4 + kMaxRank1 * 4;
 static_assert(SMEM_BYTES <= 232448, "conv: shared-memory budget");
 
 struct Params {
@@ -60,8 +49,6 @@ struct Params {
   int tiles_x, tiles_y, tw, th;
   int n_tiles, nt;
   int taps, cblocks;
-  int cs;        // cluster size: CTAs of a cluster work on `cs` consecutive pixel tiles of the SAME channel tile and
-                 // share the weight operand through TMA multicast (each CTA fetches 1/cs of it)
   int m_tiles;   // batch * tiles_y * tiles_x
   signed char tap_map[kMaxTaps], tap_w[kMaxTaps], tap_dx[kMaxTaps], tap_dy[kMaxTaps];  // per k-entry: activation
                                                          // map, weight tap group, input offset
@@ -83,14 +70,17 @@ struct Params {
   __half* gate_out;
   int gate_c;
   // split-K (fp32 output only): unit = (k-split, tile); split ks accumulates k-iterations [ks*k_per_split, ...) in its own
-  // TMEM accumulator and writes its partial sum to out_f32 + ks*f32_split_stride (bias in split 0).  The consumer adds
+  // accumulator and writes its partial sum to out_f32 + ks*f32_split_stride (bias in split 0).  The consumer adds
   // the partials in fp32 on the CUDA cores: the tensor core's accumulator rounds toward zero at every step, which
   // costs a split-precision conv with a deep K loop ~1e-5 relative (tools/accum_probe.py); short chains do not.
   int ksplit, k_per_split;
   long long f32_split_stride;
   // fp8 correction entries (split_mode 3): k-entries [0, taps16) are fp16 passes of `cblocks` 64-channel blocks, entries
-  // [taps16, taps) are kind::f8f6f4 (e4m3 x e4m3) passes of `cblocks8` 128-channel blocks over the 8-bit low-order
-  // activation tensor and the 8-bit weights; both feed the same accumulator, which the epilogue scales by acc_scale.
+  // [taps16, taps) are e4m3 x e4m3 passes of `cblocks8` 128-channel blocks over the 8-bit low-order activation tensor
+  // and the 8-bit weights; both feed the same accumulator, which the epilogue scales by acc_scale.  The e4m3 k-iterations
+  // run FIRST: wgmma adds e4m3 products to the accumulator with a reduced-precision adder (~14 significant bits of the
+  // running sum), which is harmless relative to the small correction term alone but would drop most of it on top of the
+  // full fp16 sum (~2e-4 relative error); the fp16 passes then accumulate on top in fp32.
   int taps16, cblocks8;
   float acc_scale;
   uint8_t* out_relu_lo8;  // optional: e4m3 of (relu - fp16(relu)) * 4096, the low-order operand of the next fp8 pass
@@ -99,9 +89,8 @@ struct Params {
 struct Maps {
   CUtensorMap act[8];
   CUtensorMap wgt;        // box {64, nt}
-  CUtensorMap wgt_slice;  // box {64, nt / cs} (cluster multicast)
   CUtensorMap act8;       // e4m3 low-order activations, box {128 B, tw, th}
-  CUtensorMap wgt8;       // e4m3 weights, box {128 B, nt / cs}
+  CUtensorMap wgt8;       // e4m3 weights, box {128 B, nt}
 };
 
 __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, const int (&c)[5]) {
@@ -111,107 +100,25 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c[0]), "r"(c[1]), "r"(c[2]), "r"(c[3]), "r"(c[4])
       : "memory");
 }
-// CTA-pair variant: the data lands in THIS CTA's shared memory, the bytes are credited to the barrier of the pair's
-// leader (even) CTA -- its address is the local one with the peer bit (bit 24 of the shared-window address) cleared.
-__device__ __forceinline__ void tma_load_5d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, const int (&c)[5]) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c[0]), "r"(c[1]), "r"(c[2]), "r"(c[3]),
-      "r"(c[4])
-      : "memory");
+
+// e4m3 pair {lo : low byte, hi : high byte}
+__device__ __forceinline__ uint16_t to_e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// (relu(v) - fp16(relu(v))) * 4096: the 8-bit low-order operand of an fp8 correction pass
+__device__ __forceinline__ float lo8_value(float v) {
+  const float a = fmaxf(v, 0.f);
+  return (a - __half2float(__float2half_rn(a))) * 4096.f;
 }
 
-// 32 fp32 values -> fp16 (and optionally the fp16 remainder value - fp16(value)).  `wide`: the destination is 32-byte
-// aligned (Cout % 16 == 0) -> 256-bit stores (full sectors, half the LSU instructions); otherwise 16-byte stores.
-template <bool WANT_LO>
-__device__ __forceinline__ void store_split_t(const float (&v)[32], __half* hi, __half* lo, long long off, bool relu, bool wide) {
-#pragma unroll
-  for (int j = 0; j < 32; j += 16) {
-    uint4 oh[2], ol[2];
-#pragma unroll
-    for (int g = 0; g < 2; ++g) {
-      __half2* h2 = reinterpret_cast<__half2*>(&oh[g]);
-      __half2* l2 = reinterpret_cast<__half2*>(&ol[g]);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float a = relu ? fmaxf(v[j + 8 * g + 2 * e], 0.f) : v[j + 8 * g + 2 * e];
-        const float b = relu ? fmaxf(v[j + 8 * g + 2 * e + 1], 0.f) : v[j + 8 * g + 2 * e + 1];
-        h2[e] = __floats2half2_rn(a, b);
-        if (WANT_LO) {
-          const float2 back = __half22float2(h2[e]);
-          l2[e] = __floats2half2_rn(a - back.x, b - back.y);
-        }
-      }
-    }
-    if (wide) {
-      stg256(hi + off + j, oh[0], oh[1]);
-      if (WANT_LO) stg256(lo + off + j, ol[0], ol[1]);
-    } else {
-      *reinterpret_cast<uint4*>(hi + off + j) = oh[0];
-      *reinterpret_cast<uint4*>(hi + off + j + 8) = oh[1];
-      if (WANT_LO) {
-        *reinterpret_cast<uint4*>(lo + off + j) = ol[0];
-        *reinterpret_cast<uint4*>(lo + off + j + 8) = ol[1];
-      }
-    }
-  }
-}
-__device__ __forceinline__ void store_split(const float (&v)[32], __half* hi, __half* lo, long long off, bool relu, bool wide) {
-  if (!hi) return;
-  if (lo) store_split_t<true>(v, hi, lo, off, relu, wide);
-  else store_split_t<false>(v, hi, lo, off, relu, wide);
-}
-
-// 32 fp32 values -> e4m3 of (relu(v) - fp16(relu(v))) * 4096: the 8-bit low-order operand of an fp8 correction pass
-__device__ __forceinline__ void store_lo8(const float (&v)[32], uint8_t* dst, bool wide) {
-  uint4 o[2];
-#pragma unroll
-  for (int j = 0; j < 32; j += 16) {
-    uint32_t* w = reinterpret_cast<uint32_t*>(&o[j / 16]);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      float l[4];
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const float a = fmaxf(v[j + 4 * e + t], 0.f);
-        l[t] = (a - __half2float(__float2half_rn(a))) * 4096.f;
-      }
-      uint16_t lo16, hi16;
-      asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo16) : "f"(l[1]), "f"(l[0]));  // {l[1] : high byte, l[0] : low byte}
-      asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi16) : "f"(l[3]), "f"(l[2]));
-      w[e] = (uint32_t)lo16 | ((uint32_t)hi16 << 16);
-    }
-  }
-  if (wide) {
-    stg256(dst, o[0], o[1]);
-  } else {
-    *reinterpret_cast<uint4*>(dst) = o[0];
-    *reinterpret_cast<uint4*>(dst + 16) = o[1];
-  }
-}
-
-// 32 consecutive halves (64 bytes) -> four 16-byte registers
-__device__ __forceinline__ void load_res32(const __half* src, uint4 (&r)[4], bool wide) {
-  if (wide) {
-    ldg256(src, r[0], r[1]);
-    ldg256(src + 16, r[2], r[3]);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) r[j] = *reinterpret_cast<const uint4*>(src + j * 8);
-  }
-}
-
-// Work unit `u` of a cluster -> this CTA's tile.  Units enumerate (channel tile, group of cs pixel tiles); CTA `rank`
-// of the cluster takes pixel tile mg*cs + rank.  A pixel tile index past the end ("phantom") is clamped so the CTA
-// still takes part in the shared weight pipeline, and flagged so its epilogue stores nothing.
-__device__ __forceinline__ bool tile_decode(int u, int rank, const Params& p, int& b, int& y0, int& x0, int& n0, int& ks) {
+// Work unit `u` -> tile.  Units enumerate (k-split, channel tile, pixel tile).
+__device__ __forceinline__ void tile_decode(int u, const Params& p, int& b, int& y0, int& x0, int& n0, int& ks) {
   ks = u % p.ksplit;
   u /= p.ksplit;
   const int nidx = u % p.n_tiles;
-  int m = (u / p.n_tiles) * p.cs + rank;
-  const bool real = m < p.m_tiles;
-  m = real ? m : p.m_tiles - 1;
+  int m = u / p.n_tiles;
   const int tx = m % p.tiles_x;
   m /= p.tiles_x;
   const int ty = m % p.tiles_y;
@@ -219,431 +126,263 @@ __device__ __forceinline__ bool tile_decode(int u, int rank, const Params& p, in
   y0 = ty * p.th;
   x0 = tx * p.tw;
   n0 = nidx * p.nt;
-  return real;
 }
 
-// PAIR = false: every CTA runs its own 128 x NT MMA (cta_group::1); clusters only share the weight tile by multicast.
-// PAIR = true : the two CTAs of a cluster form a tcgen05 CTA pair.  The leader (rank 0) issues ONE 256 x NT MMA
-//   (cta_group::2) per k-step: rows 0..127 are the leader's pixel tile and accumulate in the leader's TMEM, rows
-//   128..255 the peer's; each CTA holds half of the weight tile (NT/2 rows) and the tensor cores of both SMs read both
-//   halves.  Per SM the shared-memory operand traffic per MMA drops from 48 KB to 32 KB, which is what bounds the
-//   cta_group::1 kernel at ~80 % tensor-pipe utilisation.
 // EPI selects the epilogue: plain (bias / residual / rank-1 / ReLU / outputs), plain + fused logit head, or the gated
 // hidden-state update of the sensory updaters.
 enum { EPI_PLAIN = 0, EPI_HEAD = 1, EPI_GATES = 2 };
 
-// v[j] for a run-time j without spilling v to local memory: 5-level select tree (31 selects).
-__device__ __forceinline__ float pick32(const float (&v)[32], int j) {
-  float a[16], b[8], c[4], d[2];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) a[i] = (j & 16) ? v[i + 16] : v[i];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) b[i] = (j & 8) ? a[i + 8] : a[i];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) c[i] = (j & 4) ? b[i + 4] : b[i];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) d[i] = (j & 2) ? c[i + 2] : c[i];
-  return (j & 1) ? d[1] : d[0];
-}
-
 // Gate non-linearities of the fused hidden-state update.  ex2.approx + rcp.approx: absolute error < 1e-6 (the state is
-// stored in fp16, 5e-4), ~6 instructions each instead of ~15 (IEEE division) / ~40 (tanhf with its branchy slow path) -
-// the gate epilogue was costing the sensory update 0.4 ms per frame on top of its 192-column tiles
-// (tools/bench_conv.py gru_n192 vs gru_gates).  exp overflow -> +inf -> quotient 0 -> the correct limits 0 / 1 / -1.
+// stored in fp16, 5e-4), ~6 instructions each instead of ~15 (IEEE division) / ~40 (tanhf with its branchy slow path).
+// exp overflow -> +inf -> quotient 0 -> the correct limits 0 / 1 / -1.
 __device__ __forceinline__ float sigmoid_fast(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
 __device__ __forceinline__ float tanh_fast(float x) { return 1.f - __fdividef(2.f, 1.f + __expf(2.f * x)); }
 
-template <bool PAIR, int EPI>
+// One output element of the plain / head epilogue: bias, rank-1 term and residual added, outputs written.
+// `e`: element offset of (pixel, channel) in the [pixels, cout] outputs; `r` relative to the residual row.
+__device__ __forceinline__ float finish_scalar(const Params& p, float o, int ch, long long e, const __half* res,
+                                              const __half* res_lo, int rc, float r1x, int ks) {
+  o += ks == 0 ? p.bias[ch] : 0.f;
+  if (p.rank1_w) o = fmaf(p.rank1_w[ch], r1x, o);
+  if (res) o += __half2float(res[rc]);
+  if (res_lo) o += __half2float(res_lo[rc]);
+  if (p.out_raw) {
+    const __half hv = __float2half_rn(o);
+    p.out_raw[e] = hv;
+    if (p.out_raw_lo) p.out_raw_lo[e] = __float2half_rn(o - __half2float(hv));
+  }
+  if (p.out_relu) {
+    const float ro = fmaxf(o, 0.f);
+    const __half hv = __float2half_rn(ro);
+    p.out_relu[e] = hv;
+    if (p.out_relu_lo) p.out_relu_lo[e] = __float2half_rn(ro - __half2float(hv));
+  }
+  if (p.out_relu_lo8) p.out_relu_lo8[e] = (uint8_t)(to_e4m3x2(lo8_value(o), 0.f) & 0xffu);
+  if (p.out_f32) p.out_f32[ks * p.f32_split_stride + e] = o;
+  return o;
+}
+
+// N: wgmma width (>= p.nt; columns past p.nt are never stored).
+template <int N, int EPI>
 __global__ void __launch_bounds__(THREADS, 1)
 conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p) {
   constexpr bool HEAD = EPI == EPI_HEAD;
-  constexpr int NST = PAIR ? PAIR_STAGES : STAGES;
-  constexpr int B_STRIDE = PAIR ? B_BYTES_MAX / 2 : B_BYTES_MAX;
   // 1024-byte alignment (128B swizzle atoms) comes from the declaration: deriving an aligned pointer through an
   // integer cast would make the compiler lose the shared address space (generic LD/ST instead of LDS/STS).
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* sA = smem;
-  uint8_t* sB = smem + NST * A_BYTES;
+  uint8_t* sB = smem + STAGES * A_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RING_BYTES);
   uint64_t* full = bars;
-  uint64_t* empty = bars + NST;
-  uint64_t* acc_full = bars + 2 * NST;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  uint64_t* empty = bars + STAGES;
   float* s_head = reinterpret_cast<float*>(smem + RING_BYTES + 256);  // [kMaxHead][256] fused-head weights
   float* s_bias = s_head + kMaxHead * 256;                            // [kMaxBias] bias of every output channel
   float* s_r1w = s_bias + kMaxBias;                                   // [kMaxRank1] rank-1 column
-  float* s_hx = s_r1w + kMaxRank1;                                    // [2][BM][kMaxHead] head partial sums
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int cs = p.cs;
-  const int rank = (cs > 1) ? (int)cluster_ctarank() : 0;
-  const int cluster_id = blockIdx.x / cs, n_clusters = gridDim.x / cs;
-  const int total_units = ((p.m_tiles + cs - 1) / cs) * p.n_tiles * p.ksplit;
-  const uint16_t cmask = (uint16_t)((1u << cs) - 1u);
-  const int k16 = p.taps16 * p.cblocks;                       // fp16 k-iterations come first ...
-  const int k_iters = k16 + (p.taps - p.taps16) * p.cblocks8;  // ... then the fp8 correction k-iterations
-  // PAIR: both CTAs' loads are credited to the leader's barrier -> it expects the bytes of both
-  const uint32_t stage_tx = PAIR ? 2 * (A_BYTES + (p.nt / 2) * BK * 2) : A_BYTES + p.nt * BK * 2;
+  const int total_units = p.m_tiles * p.n_tiles * p.ksplit;
+  const int k8 = (p.taps - p.taps16) * p.cblocks8;  // fp8 correction k-iterations come first ...
+  const int k_iters = k8 + p.taps16 * p.cblocks;     // ... then the fp16 ones
+  const uint32_t stage_tx = A_BYTES + p.nt * BK * 2;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     for (int i = 0; i < 8; ++i) tma_prefetch_desc(&maps.act[i]);
     tma_prefetch_desc(&maps.wgt);
-    tma_prefetch_desc(&maps.wgt_slice);
     tma_prefetch_desc(&maps.act8);
     tma_prefetch_desc(&maps.wgt8);
-    // empty[]: one tcgen05.commit arrive per MMA-issuing CTA that reads the stage (PAIR: the single pair MMA)
-    for (int i = 0; i < NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], PAIR ? 1 : cs); }
-    // acc_empty[]: PAIR -> the leader's barrier collects the epilogue warps of both CTAs
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], PAIR ? 2 * EPI_WARPS : EPI_WARPS); }
+    // empty[]: one arrive per consumer warpgroup once its wgmma reading the stage have completed
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }
     fence_barrier_init();
   }
-  {  // bias (and the rank-1 column) of the whole layer: read once per CTA instead of once per chunk from global memory
+  {  // bias (and the rank-1 column) of the whole layer: read once per CTA instead of once per tile from global memory
     const int cout_pad = p.n_tiles * p.nt;
     for (int i = threadIdx.x; i < cout_pad; i += THREADS) s_bias[i] = p.bias[i];
     if (p.rank1_w)
       for (int i = threadIdx.x; i < cout_pad; i += THREADS) s_r1w[i] = p.rank1_w[i];
   }
-  if (warp == 1) {
-    if constexpr (PAIR) tmem_alloc_2sm<512>(tmem_slot);
-    else tmem_alloc<512>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  if (cs > 1) cluster_sync_all();  // peers' barriers are initialised before any multicast / remote arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      const int slice_rows = p.nt / cs;
-      for (int u = cluster_id; u < total_units; u += n_clusters) {
+      for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
         int b, y0, x0, n0, ks;
-        tile_decode(u, rank, p, b, y0, x0, n0, ks);
+        tile_decode(u, p, b, y0, x0, n0, ks);
         const int k_lo = ks * p.k_per_split, k_hi = min(k_iters, k_lo + p.k_per_split);
         // one k-iteration: activation box of tap t / channel block cb (+ the matching weight columns) into `stage`
         auto issue = [&](const int t, const int cb, const bool f8) {
           int c[5] = {f8 ? cb * 128 : cb * BK, x0 + p.tap_dx[t], y0 + p.tap_dy[t], b, 0};  // (channel, x, y, image, 1)
           const CUtensorMap* am = f8 ? &maps.act8 : &maps.act[p.tap_map[t]];
-          const CUtensorMap* wm = f8 ? &maps.wgt8 : &maps.wgt_slice;
           const int wcol = f8 ? (p.tap_w[t] * p.cblocks8 + cb) * 128 : (p.tap_w[t] * p.cblocks + cb) * BK;
           mbar_wait(&empty[stage], phase ^ 1);
-          if constexpr (PAIR) {
-            // own pixels + own half of the weight rows, both at the same offsets in either CTA
-            if (rank == 0) mbar_expect_tx(&full[stage], stage_tx);
-            tma_load_5d_2sm(sA + stage * A_BYTES, am, &full[stage], c);
-            tma_load_2d_2sm(sB + stage * B_STRIDE, wm, &full[stage], wcol, n0 + rank * slice_rows);
-          } else {
-            mbar_expect_tx(&full[stage], stage_tx);
-            tma_load_5d(sA + stage * A_BYTES, am, &full[stage], c);
-            if (cs == 1) {
-              tma_load_2d(sB + stage * B_STRIDE, f8 ? &maps.wgt8 : &maps.wgt, &full[stage], wcol, n0);
-            } else {  // this CTA fetches rows [rank*slice, +slice) of the weight tile for the whole cluster
-              tma_load_2d_mcast(sB + stage * B_STRIDE + rank * slice_rows * 128, wm, &full[stage], wcol,
-                                n0 + rank * slice_rows, cmask);
-            }
-          }
-          if (++stage == NST) { stage = 0; phase ^= 1; }
+          mbar_expect_tx(&full[stage], stage_tx);
+          tma_load_5d(sA + stage * A_BYTES, am, &full[stage], c);
+          tma_load_2d(sB + stage * B_BYTES_MAX, f8 ? &maps.wgt8 : &maps.wgt, &full[stage], wcol, n0);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         };
+        for (int t = p.taps16; t < p.taps; ++t)  // fp8 correction entries first (never combined with split-K)
+          for (int cb = 0; cb < p.cblocks8; ++cb) issue(t, cb, true);
         for (int t = k_lo / p.cblocks; t < p.taps16 && t * p.cblocks < k_hi; ++t)
           for (int cb = max(0, k_lo - t * p.cblocks); cb < p.cblocks && t * p.cblocks + cb < k_hi; ++cb) issue(t, cb, false);
-        for (int t = p.taps16; t < p.taps; ++t)  // fp8 correction entries (never combined with split-K)
-          for (int cb = 0; cb < p.cblocks8; ++cb) issue(t, cb, true);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && (!PAIR || rank == 0)) {
-      const uint32_t idesc = umma_idesc(0, PAIR ? 2 * BM : BM, p.nt);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int u = cluster_id; u < total_units; u += n_clusters, ++it) {
-        const int acc = it & 1;
-        mbar_wait(&acc_empty[acc], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        const int my_k = min(k_iters, (u % p.ksplit + 1) * p.k_per_split) - (u % p.ksplit) * p.k_per_split;
-        for (int ki = 0; ki < my_k; ++ki) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(sA + stage * A_BYTES);
-          const uint32_t b_addr = smem_u32(sB + stage * B_STRIDE);
-          if (ki < k16) {
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              if constexpr (PAIR)
-                umma_f16_2sm(d_tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc,
-                             (ki | k) != 0);
-              else
-                umma_f16(d_tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc,
-                         (ki | k) != 0);
-            }
-          } else {  // e4m3 x e4m3: 128 channels of this tap in four K = 32 instructions over the same 128-byte rows
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              if constexpr (PAIR)
-                umma_f8_2sm(d_tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc, 1);
-              else
-                umma_f8(d_tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc, 1);
-            }
-          }
-          if constexpr (PAIR) umma_commit_2sm(&empty[stage], cmask);  // frees the stage in both CTAs
-          else if (cs == 1) umma_commit(&empty[stage]);
-          else umma_commit_mcast(&empty[stage], cmask);  // the stage is free once EVERY CTA of the cluster has read it
-          if (++stage == NST) { stage = 0; phase ^= 1; }
-        }
-        if constexpr (PAIR) umma_commit_2sm(&acc_full[acc], cmask);  // both CTAs' epilogues drain their half
-        else umma_commit(&acc_full[acc]);
-      }
-    }
-  } else {
-    const int quad = warp & 3;          // TMEM lane quadrant this warp may read
-    const int half = (warp - 2) >> 2;   // 0: even 32-column chunks, 1: odd ones
-    const int row = quad * 32 + lane;   // pixel within the tile
-    const int ty = row / p.tw, tx = row - ty * p.tw;
-    const bool vec_ok = (p.cout % 8) == 0;
-    const bool wide = (p.cout % 16) == 0;   // 32-byte aligned channel chunks: 256-bit loads / stores
-    const bool wide8 = (p.cout % 32) == 0;  // same for the 1-byte e4m3 output
-    if constexpr (HEAD) {  // stage the head weights once per CTA (epilogue warps only), zero padded
-      for (int i = threadIdx.x - 64; i < kMaxHead * 256; i += EPI_THREADS) {
-        const int t = i / 256, ch = i - t * 256;
-        s_head[i] = (t < p.head_n && ch < p.cout) ? p.head_w[t * p.cout + ch] : 0.f;
-      }
-      named_bar_sync(1, EPI_THREADS);
-    }
-    int it = 0;
-    for (int u = cluster_id; u < total_units; u += n_clusters, ++it) {
-      int b, y0, x0, n0, ks;
-      const bool real = tile_decode(u, rank, p, b, y0, x0, n0, ks);
-      const int y = y0 + ty, x = x0 + tx;
-      const bool live = real && (y < p.ho) && (x < p.wo);
-      const long long pix = ((long long)b * p.ho + y) * p.wo + x;
-      const long long off = pix * p.cout + n0;
-      const __half* res = p.res ? p.res + (p.res_batch_stride ? off : ((long long)y * p.wo + x) * p.cout + n0)
-                                : nullptr;
-      const __half* res_lo = p.res_lo ? p.res_lo + (res - p.res) : nullptr;
-      const float r1x = (p.rank1_x && live) ? p.rank1_x[pix] : 0.f;
-      const int acc = it & 1;
-      if constexpr (EPI == EPI_GATES) {
-        // channel tile = [forget | update | new] x 64 for hidden channels hc0 .. hc0+63 (modules.py:145-149);
-        // this warp finishes hidden channels hc0 + 32*half .. +31
-        const int hc0 = (n0 / 192) * 64;
-        const long long hoff = pix * p.gate_c + hc0;
-        const int c = half;
-        uint4 hv[4];
-        if (live) load_res32(p.gate_h + hoff + c * 32, hv, true);  // gate_c % 64 == 0: always 32-byte aligned
-        mbar_wait(&acc_full[acc], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t t_addr = tmem_base + (uint32_t(quad * 32) << 16) + acc * 256;
-        {
-          uint32_t rf[32], ru[32], rn[32];
-          tmem_ld_32x32(t_addr + c * 32, rf);
-          tmem_ld_32x32(t_addr + 64 + c * 32, ru);
-          tmem_ld_32x32(t_addr + 128 + c * 32, rn);
-          tmem_ld_wait();
-          if (live) {
-            const float* bf = s_bias + n0 + c * 32;
-            uint4 ovs[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              uint4& ov = ovs[j];
-              __half2* o2 = reinterpret_cast<__half2*>(&ov);
-              const __half2* h2 = reinterpret_cast<const __half2*>(&hv[j]);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int ch = j * 8 + 2 * e;
-                const float2 hp = __half22float2(h2[e]);
-                float o[2];
-#pragma unroll
-                for (int s = 0; s < 2; ++s) {
-                  const float f = sigmoid_fast(__uint_as_float(rf[ch + s]) + bf[ch + s]);
-                  const float u = sigmoid_fast(__uint_as_float(ru[ch + s]) + bf[64 + ch + s]);
-                  const float n = tanh_fast(__uint_as_float(rn[ch + s]) + bf[128 + ch + s]);
-                  o[s] = f * (s ? hp.y : hp.x) * (1.f - u) + u * n;
-                }
-                o2[e] = __floats2half2_rn(o[0], o[1]);
-              }
-            }
-            stg256(p.gate_out + hoff + c * 32, ovs[0], ovs[1]);
-            stg256(p.gate_out + hoff + c * 32 + 16, ovs[2], ovs[3]);
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if constexpr (PAIR) mbar_arrive_cluster_relaxed(&acc_empty[acc], 0);
-          else mbar_arrive(&acc_empty[acc]);
-        }
-      } else {
-      float hacc[kMaxHead];
-#pragma unroll
-      for (int t = 0; t < kMaxHead; ++t) hacc[t] = 0.f;
-      // Software pipeline over this warp's 32-channel chunks (c = half, half + 2, ...): the TMEM load and the residual
-      // loads of its next chunk are in flight while the current one is finished (the residual comes from L2/HBM: ~1 us
-      // if waited for in place); the first chunk's residual is requested before the accumulator is even complete.
-      const int n_chunks = p.nt / 32;
-      const float acc_scale = p.acc_scale;
-      const bool res_pf = res && live && vec_ok && (p.cout % 32 == 0);
-      uint32_t r[32];
-      uint4 res_cur[4], res_nxt[4];
-      if (res_pf && half < n_chunks && n0 + (half + 1) * 32 <= p.cout) load_res32(res + half * 32, res_cur, wide);
-      mbar_wait(&acc_full[acc], (it >> 1) & 1);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + (uint32_t(quad * 32) << 16) + acc * 256;
-      if (half < n_chunks) tmem_ld_32x32(t_addr + half * 32, r);
-      auto chunk = [&](const int c) {
-        tmem_ld_wait();
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * acc_scale;  // 1 unless the operands were pre-scaled (fp8 mode)
-        if (c + 2 < n_chunks) {
-          tmem_ld_32x32(t_addr + (c + 2) * 32, r);
-          if (res_pf && n0 + (c + 3) * 32 <= p.cout) load_res32(res + (c + 2) * 32, res_nxt, wide);
-        }
-        const int ch0 = n0 + c * 32;
-        if (live && ch0 < p.cout) {
-          if (ch0 + 32 <= p.cout && vec_ok) {
-            if (ks == 0) {  // partial sums of the later k-splits carry no bias
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 bv = *reinterpret_cast<const float4*>(s_bias + ch0 + j);
-                v[j] += bv.x; v[j + 1] += bv.y; v[j + 2] += bv.z; v[j + 3] += bv.w;
-              }
-            }
-            if (p.rank1_w) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 wv = *reinterpret_cast<const float4*>(s_r1w + ch0 + j);
-                v[j] = fmaf(wv.x, r1x, v[j]); v[j + 1] = fmaf(wv.y, r1x, v[j + 1]);
-                v[j + 2] = fmaf(wv.z, r1x, v[j + 2]); v[j + 3] = fmaf(wv.w, r1x, v[j + 3]);
-              }
-            }
-            if (res) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) {
-                const uint4 rv = res_pf ? res_cur[j / 8] : *reinterpret_cast<const uint4*>(res + c * 32 + j);
-                const __half2* h2 = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 f = __half22float2(h2[e]);
-                  v[j + 2 * e] += f.x;
-                  v[j + 2 * e + 1] += f.y;
-                }
-              }
-            }
-            if (res_lo) {
-              uint4 rl[4];
-              load_res32(res_lo + c * 32, rl, wide);
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) {
-                const uint4 rv = rl[j / 8];
-                const __half2* h2 = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 f = __half22float2(h2[e]);
-                  v[j + 2 * e] += f.x;
-                  v[j + 2 * e + 1] += f.y;
-                }
-              }
-            }
-            store_split(v, p.out_raw, p.out_raw_lo, off + c * 32, false, wide);
-            store_split(v, p.out_relu, p.out_relu_lo, off + c * 32, true, wide);
-            if (p.out_relu_lo8) store_lo8(v, p.out_relu_lo8 + off + c * 32, wide8);
-            if constexpr (HEAD) {  // logit head: 9 taps x 32 channels of this chunk, fp32, weights from shared memory
-              float rv[32];
-#pragma unroll
-              for (int j = 0; j < 32; ++j) rv[j] = fmaxf(v[j], 0.f);
-#pragma unroll
-              for (int t = 0; t < kMaxHead; ++t) {
-                const float4* w4 = reinterpret_cast<const float4*>(s_head + t * 256 + c * 32);
-                float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;  // four independent chains per tap
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float4 wv = w4[j];
-                  a0 = fmaf(rv[4 * j], wv.x, a0);
-                  a1 = fmaf(rv[4 * j + 1], wv.y, a1);
-                  a2 = fmaf(rv[4 * j + 2], wv.z, a2);
-                  a3 = fmaf(rv[4 * j + 3], wv.w, a3);
-                }
-                hacc[t] += (a0 + a1) + (a2 + a3);
-              }
-            }
-            if (p.out_f32) {
-              float* o32 = p.out_f32 + ks * p.f32_split_stride + off + c * 32;
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) {  // Cout % 8 == 0 on this path: the fp32 rows are 32-byte aligned
-                uint4 a, b;
-                a.x = __float_as_uint(v[j]); a.y = __float_as_uint(v[j + 1]); a.z = __float_as_uint(v[j + 2]); a.w = __float_as_uint(v[j + 3]);
-                b.x = __float_as_uint(v[j + 4]); b.y = __float_as_uint(v[j + 5]); b.z = __float_as_uint(v[j + 6]); b.w = __float_as_uint(v[j + 7]);
-                stg256(o32 + j, a, b);
-              }
-            }
-          } else {  // ragged channel tail (e.g. Cout = 1, 129): scalar path, rolled (the value comes out of the
-            // register array through a select tree, so the 32 copies of this body do not sit in the instruction stream)
-#pragma unroll 1
-            for (int j = 0; j < 32; ++j) {
-              const int ch = ch0 + j;
-              if (ch >= p.cout) break;
-              float o = pick32(v, j) + (ks == 0 ? p.bias[ch] : 0.f);
-              if (p.rank1_w) o = fmaf(p.rank1_w[ch], r1x, o);
-              if (res) o += __half2float(res[c * 32 + j]);
-              if (res_lo) o += __half2float(res_lo[c * 32 + j]);
-              if (p.out_raw) {
-                const __half hv = __float2half_rn(o);
-                p.out_raw[off + c * 32 + j] = hv;
-                if (p.out_raw_lo) p.out_raw_lo[off + c * 32 + j] = __float2half_rn(o - __half2float(hv));
-              }
-              if (p.out_relu) {
-                const float ro = fmaxf(o, 0.f);
-                const __half hv = __float2half_rn(ro);
-                p.out_relu[off + c * 32 + j] = hv;
-                if (p.out_relu_lo) p.out_relu_lo[off + c * 32 + j] = __float2half_rn(ro - __half2float(hv));
-              }
-              if (p.out_f32) p.out_f32[ks * p.f32_split_stride + off + c * 32 + j] = o;
-            }
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) res_cur[j] = res_nxt[j];
-      };
-#pragma unroll 1
-      for (int c = half; c < n_chunks; c += 2) chunk(c);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_cluster_relaxed(&acc_empty[acc], 0);  // tcgen05.ld are complete; no stores to publish
-        else mbar_arrive(&acc_empty[acc]);
-      }
-      if constexpr (HEAD) {
-        // the two warps of a quadrant hold the head sums of the even / odd chunks of the same pixels: the odd-chunk warp
-        // hands its sums over through shared memory (double-buffered by tile, one named barrier per tile)
-        float* hx = s_hx + (it & 1) * (BM * kMaxHead) + row * kMaxHead;
-        if (half == 1) {
-#pragma unroll
-          for (int t = 0; t < kMaxHead; ++t) hx[t] = hacc[t];
-        }
-        named_bar_sync(2, EPI_THREADS);
-        if (half == 0 && live) {
-#pragma unroll
-          for (int t = 0; t < kMaxHead; ++t)
-            if (t < p.head_n) p.head_out[pix * p.head_n + t] = hacc[t] + hx[t];
-        }
-      }
-      }  // plain / head epilogue
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (cs > 1) cluster_sync_all();  // nobody leaves while a peer may still multicast into this CTA
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc_2sm<512>(tmem_base);
-    else tmem_dealloc<512>(tmem_base);
+  // ---------------------------------------------------------------- consumers: warpgroup wg owns pixels wg*64 .. +63
+  const int wg = warp >> 2;
+  const int qd = lane & 3;  // column pair within each 8-column block of the fragment
+  if constexpr (HEAD) {  // stage the head weights once per CTA, zero padded
+    for (int i = threadIdx.x; i < kMaxHead * 256; i += CONSUMER_THREADS) {
+      const int t = i / 256, ch = i - t * 256;
+      s_head[i] = (t < p.head_n && ch < p.cout) ? p.head_w[t * p.cout + ch] : 0.f;
+    }
+    named_bar_sync(1, CONSUMER_THREADS);
+  }
+  const uint32_t a_off = wg * 64 * 128;  // this warpgroup's 64 rows of the A tile (8 swizzle atoms)
+  const bool even = (p.cout % 2) == 0;   // (channel, channel + 1) pairs are 4-byte aligned in the fp16 outputs
+  float d[N / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
+    int b, y0, x0, n0, ks;
+    tile_decode(u, p, b, y0, x0, n0, ks);
+    const int my_k = min(k_iters, (ks + 1) * p.k_per_split) - ks * p.k_per_split;
+    int prev_stage = -1;
+    for (int ki = 0; ki < my_k; ++ki) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t a_addr = smem_u32(sA + stage * A_BYTES) + a_off;
+      const uint32_t b_addr = smem_u32(sB + stage * B_BYTES_MAX);
+      wgmma_fence();
+      if (ki >= k8) {
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_f16<N>(d, wgmma_desc_sw128(a_addr + k * 32), wgmma_desc_sw128(b_addr + k * 32), (ki | k) != 0);
+      } else {  // e4m3 x e4m3: 128 channels of this tap in four K = 32 instructions over the same 128-byte rows
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_e4m3<N>(d, wgmma_desc_sw128(a_addr + k * 32), wgmma_desc_sw128(b_addr + k * 32), (ki | k) != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-iteration's group has finished reading its stage
+      if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev_stage]);
+      prev_stage = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(d);
+    if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev_stage]);
+
+    // thread holds rows r_i = wg*64 + (warp%4)*16 + lane/4 + 8i, columns 8j + 2*qd + {0, 1}
+    const float acc_scale = p.acc_scale;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+      const int ty = row / p.tw, tx = row - ty * p.tw;
+      const int y = y0 + ty, x = x0 + tx;
+      const bool live = (y < p.ho) && (x < p.wo);
+      const long long pix = ((long long)b * p.ho + y) * p.wo + x;
+      const long long off = pix * p.cout + n0;
+      if constexpr (EPI == EPI_GATES) {
+        // channel tile = [forget | update | new] x 64 for hidden channels hc0 .. hc0+63 (modules.py:145-149): the three
+        // gates of hidden channel c sit in columns c, 64 + c, 128 + c, i.e. in the same thread
+        if (live) {
+          const int hc0 = (n0 / 192) * 64;
+          const long long hoff = pix * p.gate_c + hc0;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int c = 8 * j + 2 * qd;
+            const float2 hp = __half22float2(*reinterpret_cast<const __half2*>(p.gate_h + hoff + c));
+            float o[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float f = sigmoid_fast(d[4 * j + 2 * i + e] + s_bias[n0 + c + e]);
+              const float uu = sigmoid_fast(d[4 * (j + 8) + 2 * i + e] + s_bias[n0 + 64 + c + e]);
+              const float n = tanh_fast(d[4 * (j + 16) + 2 * i + e] + s_bias[n0 + 128 + c + e]);
+              o[e] = f * (e ? hp.y : hp.x) * (1.f - uu) + uu * n;
+            }
+            *reinterpret_cast<__half2*>(p.gate_out + hoff + c) = __floats2half2_rn(o[0], o[1]);
+          }
+        }
+      } else {
+        const __half* res = p.res ? p.res + (p.res_batch_stride ? off : ((long long)y * p.wo + x) * p.cout + n0)
+                                  : nullptr;
+        const __half* res_lo = p.res_lo ? p.res_lo + (res - p.res) : nullptr;
+        const float r1x = (p.rank1_x && live) ? p.rank1_x[pix] : 0.f;
+        float hacc[kMaxHead];
+#pragma unroll
+        for (int t = 0; t < kMaxHead; ++t) hacc[t] = 0.f;
+        if (live) {
+#pragma unroll
+          for (int j = 0; j < N / 8; ++j) {
+            const int col = 8 * j + 2 * qd;
+            const int ch = n0 + col;
+            if (col >= p.nt || ch >= p.cout) continue;
+            float v0 = d[4 * j + 2 * i] * acc_scale, v1 = d[4 * j + 2 * i + 1] * acc_scale;  // acc_scale: fp8 mode
+            if (even) {  // both channels exist (cout even, ch even): 4-byte fp16 pairs, 8-byte fp32 pairs
+              if (ks == 0) { v0 += s_bias[ch]; v1 += s_bias[ch + 1]; }
+              if (p.rank1_w) { v0 = fmaf(s_r1w[ch], r1x, v0); v1 = fmaf(s_r1w[ch + 1], r1x, v1); }
+              if (res) {
+                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res + col));
+                v0 += f.x; v1 += f.y;
+              }
+              if (res_lo) {
+                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res_lo + col));
+                v0 += f.x; v1 += f.y;
+              }
+              const long long e = off + col;
+              if (p.out_raw) {
+                const __half2 h = __floats2half2_rn(v0, v1);
+                *reinterpret_cast<__half2*>(p.out_raw + e) = h;
+                if (p.out_raw_lo) {
+                  const float2 back = __half22float2(h);
+                  *reinterpret_cast<__half2*>(p.out_raw_lo + e) = __floats2half2_rn(v0 - back.x, v1 - back.y);
+                }
+              }
+              if (p.out_relu) {
+                const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
+                const __half2 h = __floats2half2_rn(a0, a1);
+                *reinterpret_cast<__half2*>(p.out_relu + e) = h;
+                if (p.out_relu_lo) {
+                  const float2 back = __half22float2(h);
+                  *reinterpret_cast<__half2*>(p.out_relu_lo + e) = __floats2half2_rn(a0 - back.x, a1 - back.y);
+                }
+              }
+              if (p.out_relu_lo8)
+                *reinterpret_cast<uint16_t*>(p.out_relu_lo8 + e) = to_e4m3x2(lo8_value(v0), lo8_value(v1));
+              if (p.out_f32)
+                *reinterpret_cast<float2*>(p.out_f32 + ks * p.f32_split_stride + e) = make_float2(v0, v1);
+            } else {  // ragged channel count (e.g. Cout = 1, 129): element by element
+              v0 = finish_scalar(p, v0, ch, off + col, res, res_lo, col, r1x, ks);
+              if (ch + 1 < p.cout) v1 = finish_scalar(p, v1, ch + 1, off + col + 1, res, res_lo, col + 1, r1x, ks);
+            }
+            if constexpr (HEAD) {  // logit head: 9 taps over the ReLU'd channels, fp32, weights from shared memory
+              const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
+#pragma unroll
+              for (int t = 0; t < kMaxHead; ++t) {
+                const float2 w2 = *reinterpret_cast<const float2*>(s_head + t * 256 + col);
+                hacc[t] = fmaf(a0, w2.x, fmaf(a1, w2.y, hacc[t]));
+              }
+            }
+          }
+        }
+        if constexpr (HEAD) {  // the four threads of a quad hold the same pixel's partial sums over disjoint channels
+#pragma unroll
+          for (int t = 0; t < kMaxHead; ++t) {
+            hacc[t] += __shfl_xor_sync(0xffffffffu, hacc[t], 1);
+            hacc[t] += __shfl_xor_sync(0xffffffffu, hacc[t], 2);
+          }
+          if (live && qd == 0) {
+#pragma unroll
+            for (int t = 0; t < kMaxHead; ++t)
+              if (t < p.head_n) p.head_out[pix * p.head_n + t] = hacc[t];
+          }
+        }
+      }
+    }
   }
 }
 
@@ -764,112 +503,54 @@ int launch_conv(const ConvDesc& d, cudaStream_t stream) {
                  "conv: fused head needs the whole Cout (%d) in one channel tile and head_n <= %d", d.cout, kMaxHead);
     p.head_w = d.head_w; p.head_out = d.head_out; p.head_n = d.head_n;
   }
+  // wgmma width: the channel tile rounded up to one of four instantiations.  TMA fills only nt weight rows of a stage;
+  // rows nt .. N-1 hold whatever an earlier stage left there, so columns nt .. N-1 of the accumulator are garbage and the
+  // epilogue never stores them (col < p.nt).  The cost is up to half the MMA work of layers with a ragged tile
+  // (Cout 1 -> N 64, Cout 129 -> nt 160 -> N 192); those layers are small.
+  const int n_mma = d.nt <= 64 ? 64 : (d.nt <= 128 ? 128 : (d.nt <= 192 ? 192 : 256));
+  const int epi = p.gate_out ? EPI_GATES : (p.head_w ? EPI_HEAD : EPI_PLAIN);
+  void (*kern)(const Maps, const Params) = nullptr;
+  if (epi == EPI_GATES) kern = conv_kernel<192, EPI_GATES>;
+  else if (epi == EPI_HEAD)
+    kern = n_mma == 64 ? conv_kernel<64, EPI_HEAD> : n_mma == 128 ? conv_kernel<128, EPI_HEAD>
+         : n_mma == 192 ? conv_kernel<192, EPI_HEAD> : conv_kernel<256, EPI_HEAD>;
+  else
+    kern = n_mma == 64 ? conv_kernel<64, EPI_PLAIN> : n_mma == 128 ? conv_kernel<128, EPI_PLAIN>
+         : n_mma == 192 ? conv_kernel<192, EPI_PLAIN> : conv_kernel<256, EPI_PLAIN>;
   static bool configured_dev[kMaxDevices] = {false};  // function attributes are per device
   bool& configured = configured_dev[device_slot()];
   if (!configured) {
-    B200_CUDA(cudaFuncSetAttribute(conv_kernel<false, EPI_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    B200_CUDA(cudaFuncSetAttribute(conv_kernel<true, EPI_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    B200_CUDA(cudaFuncSetAttribute(conv_kernel<false, EPI_HEAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    B200_CUDA(cudaFuncSetAttribute(conv_kernel<true, EPI_HEAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    B200_CUDA(cudaFuncSetAttribute(conv_kernel<false, EPI_GATES>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    B200_CUDA(cudaFuncSetAttribute(conv_kernel<true, EPI_GATES>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    for (auto k : {conv_kernel<64, EPI_PLAIN>, conv_kernel<128, EPI_PLAIN>, conv_kernel<192, EPI_PLAIN>, conv_kernel<256, EPI_PLAIN>,
+                   conv_kernel<64, EPI_HEAD>, conv_kernel<128, EPI_HEAD>, conv_kernel<192, EPI_HEAD>, conv_kernel<256, EPI_HEAD>,
+                   conv_kernel<192, EPI_GATES>})
+      B200_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     configured = true;
   }
-  // Clusters: with enough work to keep every SM busy, two CTAs either form a tcgen05 CTA pair (default) or only share
-  // the weight tile by TMA multicast (DEVA_B200_CONV_PAIR=0; DEVA_B200_CONV_CLUSTER=1/2/4 sets the multicast width).
-  static const int max_cs = [] { const char* e = getenv("DEVA_B200_CONV_CLUSTER"); return e ? atoi(e) : 2; }();
-  static const bool want_pair = [] { const char* e = getenv("DEVA_B200_CONV_PAIR"); return e ? atoi(e) != 0 : true; }();
-  int cs = 1;
-  for (int c = max_cs; c >= 2; c >>= 1)
-    if ((c == 2 || c == 4) && (d.nt / c) % 8 == 0 && (long long)p.m_tiles * p.n_tiles >= 2ll * sm_count() && sm_count() % c == 0) {
-      cs = c;
-      break;
-    }
-  // the pair's cross-CTA handshakes only pay off with a deep K loop (short ones are latency/epilogue bound)
-  static const bool pair_head = [] { const char* e = getenv("DEVA_B200_CONV_PAIR_HEAD"); return e ? atoi(e) != 0 : true; }();
-  const bool pair = want_pair && cs >= 2 && (d.nt / 2) % 16 == 0 && p.taps * (d.cin_pad / 64) >= 16 &&
-                    (!d.head_w || pair_head);
-  if (pair) cs = 2;
-  p.cs = cs;
-  if (cs > 1 && make_tmap_2d(&maps.wgt_slice, TmapType::F16, d.w_packed, (uint64_t)w_groups * ktaps * d.cin_pad,
-                             d.cout_pad, (uint64_t)w_groups * ktaps * d.cin_pad * 2, 64, d.nt / cs, &err)) {
-    set_error("conv: %s", err ? err : "weight slice tensor map");
-    return 3;
-  }
-  if (cs == 1) maps.wgt_slice = maps.wgt;
   maps.act8 = maps.act[0];
   maps.wgt8 = maps.wgt;
   if (d.split_mode == 3) {
     const uint64_t k8 = (uint64_t)ktaps * d.cin_pad;  // bytes per weight row (cin_pad is a multiple of 128)
     if (make_tmap_act5_u8(&maps.act8, d.x_lo8, d.cin_pad, d.w, d.h, d.batch, (long long)d.cin_pad, (long long)d.w * d.cin_pad,
                           (long long)d.h * d.w * d.cin_pad, d.tw, d.th, &err) ||
-        make_tmap_2d(&maps.wgt8, TmapType::U8, d.w8_packed, k8, d.cout_pad, k8, 128, d.nt / cs, &err)) {
+        make_tmap_2d(&maps.wgt8, TmapType::U8, d.w8_packed, k8, d.cout_pad, k8, 128, d.nt, &err)) {
       set_error("conv: %s", err ? err : "fp8 tensor maps");
       return 3;
     }
   }
-  // split-K: fp32 output only, one CTA per unit (no clusters)
+  // split-K: fp32 output only
   p.ksplit = d.ksplit > 1 ? d.ksplit : 1;
   const int k_iters_total = p.taps16 * p.cblocks + (p.taps - p.taps16) * p.cblocks8;
   if (p.ksplit > 1) {
     B200_REQUIRE(d.out_f32 && !d.out_raw && !d.out_relu && !d.res && !d.rank1_w && !d.head_w && !d.gate_out,
                  "conv: split-K writes fp32 partial sums only (no residual / rank-1 / head / gates / fp16 outputs)");
     B200_REQUIRE(p.ksplit <= k_iters_total, "conv: ksplit %d exceeds the %d k-iterations", p.ksplit, k_iters_total);
-    cs = 1;
-    p.cs = 1;
-    maps.wgt_slice = maps.wgt;
   }
   p.k_per_split = (k_iters_total + p.ksplit - 1) / p.ksplit;
   p.ksplit = (k_iters_total + p.k_per_split - 1) / p.k_per_split;  // no empty trailing split
   p.f32_split_stride = (long long)d.batch * ho * wo * d.cout;
-  const long long units = (long long)((p.m_tiles + cs - 1) / cs) * p.n_tiles * p.ksplit;
-  // co-resident clusters (a GPC with a leftover odd SM count strands SMs for cs = 4): ask the runtime once
-  static int max_clusters_dev[kMaxDevices][5] = {{0}};
-  int* max_clusters = max_clusters_dev[device_slot()];
-  if (cs > 1 && max_clusters[cs] == 0) {
-    cudaLaunchConfig_t q{};
-    q.gridDim = dim3(sm_count() / cs * cs);
-    q.blockDim = dim3(THREADS);
-    q.dynamicSmemBytes = SMEM_BYTES;
-    cudaLaunchAttribute a[1];
-    a[0].id = cudaLaunchAttributeClusterDimension;
-    a[0].val.clusterDim.x = cs; a[0].val.clusterDim.y = 1; a[0].val.clusterDim.z = 1;
-    q.attrs = a; q.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, conv_kernel<false, EPI_PLAIN>, &q) != cudaSuccess || n <= 0) { (void)cudaGetLastError(); n = sm_count() / cs; }
-    max_clusters[cs] = n;
-  }
-  long long clusters = cs > 1 ? max_clusters[cs] : sm_count();
-  if (units < clusters) clusters = units;
-  const int grid = (int)(clusters * cs);
-  const int epi = p.gate_out ? EPI_GATES : (p.head_w ? EPI_HEAD : EPI_PLAIN);
-  if (cs == 1) {
-    if (epi == EPI_GATES) conv_kernel<false, EPI_GATES><<<grid, THREADS, SMEM_BYTES, stream>>>(maps, p);
-    else if (epi == EPI_HEAD) conv_kernel<false, EPI_HEAD><<<grid, THREADS, SMEM_BYTES, stream>>>(maps, p);
-    else conv_kernel<false, EPI_PLAIN><<<grid, THREADS, SMEM_BYTES, stream>>>(maps, p);
-  } else {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = SMEM_BYTES;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cs;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (pair) {
-      if (epi == EPI_GATES) B200_CUDA(cudaLaunchKernelEx(&cfg, conv_kernel<true, EPI_GATES>, maps, p));
-      else if (epi == EPI_HEAD) B200_CUDA(cudaLaunchKernelEx(&cfg, conv_kernel<true, EPI_HEAD>, maps, p));
-      else B200_CUDA(cudaLaunchKernelEx(&cfg, conv_kernel<true, EPI_PLAIN>, maps, p));
-    } else {
-      if (epi == EPI_GATES) B200_CUDA(cudaLaunchKernelEx(&cfg, conv_kernel<false, EPI_GATES>, maps, p));
-      else if (epi == EPI_HEAD) B200_CUDA(cudaLaunchKernelEx(&cfg, conv_kernel<false, EPI_HEAD>, maps, p));
-      else B200_CUDA(cudaLaunchKernelEx(&cfg, conv_kernel<false, EPI_PLAIN>, maps, p));
-    }
-  }
+  const long long units = (long long)p.m_tiles * p.n_tiles * p.ksplit;
+  const int grid = (int)(units < sm_count() ? units : sm_count());
+  kern<<<grid, THREADS, SMEM_BYTES, stream>>>(maps, p);
   B200_LAUNCH_CHECK();
   return 0;
 }

@@ -106,7 +106,7 @@ stem_im2col_kernel(const float* __restrict__ src, __half* __restrict__ dst, __ha
 // or without the fp16 remainders).  The generic kernel spends ~120 instructions of index arithmetic per 16-byte store
 // and ran at 16-28 % of the HBM peak; here a thread owns one output pixel, reads its 49*C taps from a patch staged in
 // shared memory (even / odd input columns de-interleaved so consecutive pixels read consecutive words) with compile-time
-// tap offsets, and writes its whole im2col row with 256-bit stores.  Same values as the generic kernel.
+// tap offsets, and writes its whole im2col row with 16-byte stores.  Same values as the generic kernel.
 constexpr int IM1_XT = 128;
 template <int C, int ROWS, bool LO>
 __global__ void __launch_bounds__(IM1_XT)
@@ -137,7 +137,7 @@ stem_im2col_px_kernel(const float* __restrict__ src, __half* __restrict__ dst, _
     if (yo >= Ho) break;
     const long long out = (((long long)b * Ho + yo) * Wo + xo) * KP;
 #pragma unroll
-    for (int k0 = 0; k0 < KP; k0 += 16) {  // 16 columns = one 32-byte store (and one for the remainders)
+    for (int k0 = 0; k0 < KP; k0 += 16) {  // 16 columns = two 16-byte stores (and two for the remainders)
       uint4 oh[2], ol[2];
       __half2* h2 = reinterpret_cast<__half2*>(oh);
       __half2* l2 = reinterpret_cast<__half2*>(ol);
@@ -160,13 +160,14 @@ stem_im2col_px_kernel(const float* __restrict__ src, __half* __restrict__ dst, _
           l2[k2] = __floats2half2_rn(v[0] - back.x, v[1] - back.y);
         }
       }
-      asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst + out + k0), "r"(oh[0].x), "r"(oh[0].y),
-                   "r"(oh[0].z), "r"(oh[0].w), "r"(oh[1].x), "r"(oh[1].y), "r"(oh[1].z), "r"(oh[1].w)
-                   : "memory");
-      if (LO)
-        asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst_lo + out + k0), "r"(ol[0].x),
-                     "r"(ol[0].y), "r"(ol[0].z), "r"(ol[0].w), "r"(ol[1].x), "r"(ol[1].y), "r"(ol[1].z), "r"(ol[1].w)
-                     : "memory");
+      uint4* dh = reinterpret_cast<uint4*>(dst + out + k0);
+      dh[0] = oh[0];
+      dh[1] = oh[1];
+      if (LO) {
+        uint4* dl = reinterpret_cast<uint4*>(dst_lo + out + k0);
+        dl[0] = ol[0];
+        dl[1] = ol[1];
+      }
     }
   }
 }
@@ -796,7 +797,7 @@ int ew_stem_im2col(const float* src, __half* dst, __half* dst_lo, int B, int C, 
   B200_REQUIRE(H % 2 == 0 && W % 2 == 0 && Kp % 64 == 0 && Kp >= 49 * C, "stem_im2col: bad shape");
   B200_REQUIRE(C >= 1 && C <= 8, "stem_im2col: at most 8 input planes");
   const size_t smem = (size_t)C * 7 * (2 * ew::IM_XT + 5) * sizeof(float);
-  // the network's shapes: one thread per output pixel, whole im2col rows written with 256-bit stores
+  // the network's shapes: one thread per output pixel, whole im2col rows written with 16-byte stores
   const dim3 gx(ceil_div(W / 2, ew::IM1_XT));
   if (C == 1 && Kp == 64 && !dst_lo) {
     ew::stem_im2col_px_kernel<1, 4, false><<<dim3(gx.x, B * ceil_div(H / 2, 4)), ew::IM1_XT, 0, s>>>(src, dst, nullptr, B, H, W);

@@ -1,12 +1,12 @@
 // Memory readout  out[K*CV, Q] = V[K*CV, N] . P[N, Q]   (reference: MemoryManager._readout,
 // deva/inference/memory_manager.py:64-75; training twin memory_utils.py:87-94).
 //
-// tcgen05 GEMM, fp16 operands / fp32 accumulation in TMEM.
+// wgmma GEMM, fp16 operands / fp32 accumulation in registers.
 //   A operand = value bank rows (M = value channels of the active objects), K-major: the bank
 //               keeps every value row contiguous along the memory-slot axis N.
 //   B operand = dense affinity P stored [Q, N] (K-major), produced by the top-k/softmax stage.
-//   D         = 128 x 256 fp32 tile per CTA, double-buffered in TMEM (2 x 256 columns).
-// Warp roles: warp 0 TMA producer, warp 1 MMA issuer (+TMEM owner), warps 2-5 epilogue.
+//   D         = 128 x 256 fp32 tile per CTA: two consumer warpgroups, 64 rows each (m64n256k16).
+// Warp roles: warps 0-7 consumers (MMA + epilogue), warp 8 TMA producer.
 // Persistent CTAs (one per SM) walk a grouped raster of the tile grid so that CTAs running
 // together share value panels and affinity panels in L2.
 #include <cuda_fp16.h>
@@ -26,7 +26,8 @@ constexpr int STAGES = 4;
 constexpr int A_BYTES = BM * BK * 2;
 constexpr int B_BYTES = BN * BK * 2;
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int THREADS = 192;
+constexpr int CONSUMER_THREADS = 256;
+constexpr int THREADS = CONSUMER_THREADS + 32;
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 constexpr int GROUP_M = 16;
 constexpr int kListCapR = 32;  // row pitch of the top-k index / weight lists (== simtopk's kListCap)
@@ -52,6 +53,57 @@ __device__ __forceinline__ void tile_coords(int tile, int m_tiles, int n_tiles, 
   n = r / rows;
 }
 
+// Consumer side of one tile: the k-loop over the shared-memory ring (a stage is released once the wgmma that read it
+// have completed), leaving this warpgroup's 64 x BN accumulator in d.
+__device__ __forceinline__ void mma_tile(float (&d)[BN / 2], const uint8_t* sA, const uint8_t* sB, uint64_t* full,
+                                         uint64_t* empty, int k_blocks, int& stage, uint32_t& phase) {
+  const uint32_t a_off = (threadIdx.x >> 7) * 64 * 128;  // this warpgroup's 64 rows of the A tile
+  int prev = -1;
+  for (int kb = 0; kb < k_blocks; ++kb) {
+    mbar_wait(&full[stage], phase);
+    const uint32_t a_addr = smem_u32(sA + stage * A_BYTES) + a_off;
+    const uint32_t b_addr = smem_u32(sB + stage * B_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)
+      wgmma_f16<BN>(d, wgmma_desc_sw128(a_addr + k * 32), wgmma_desc_sw128(b_addr + k * 32), (kb | k) != 0);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(d);
+  if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+}
+
+// Row i (0: lane/4, 1: lane/4 + 8) of this thread's accumulator fragment -> fp32 row `dst` (columns q0 + 8j, +1), or
+// the fp16 token-major output `dt` when given.
+template <int W>
+__device__ __forceinline__ void store_rows(const float (&d)[W / 2], int i, int q0, int q, float* dst, __half* dt,
+                                           int rows_per_group, bool vec_ok) {
+  if (dt) {
+#pragma unroll
+    for (int j = 0; j < W / 8; ++j) {
+      const int c = q0 + 8 * j;
+      if (c < q) dt[(long long)c * rows_per_group] = __float2half_rn(d[4 * j + 2 * i]);
+      if (c + 1 < q) dt[(long long)(c + 1) * rows_per_group] = __float2half_rn(d[4 * j + 2 * i + 1]);
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < W / 8; ++j) {
+      const int c = q0 + 8 * j;
+      if (vec_ok && c + 1 < q) {
+        *reinterpret_cast<float2*>(dst + c) = make_float2(d[4 * j + 2 * i], d[4 * j + 2 * i + 1]);
+      } else {
+        if (c < q) dst[c] = d[4 * j + 2 * i];
+        if (c + 1 < q) dst[c + 1] = d[4 * j + 2 * i + 1];
+      }
+    }
+  }
+}
+
 __global__ void __launch_bounds__(THREADS, 1)
 readout_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_p,
                const __grid_constant__ Params p) {
@@ -64,34 +116,23 @@ readout_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_constant_
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* full = bars;                 // [STAGES]
   uint64_t* empty = bars + STAGES;       // [STAGES]
-  uint64_t* acc_full = bars + 2 * STAGES;   // [2]
-  uint64_t* acc_empty = acc_full + 2;       // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int total_tiles = p.m_tiles * p.n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&map_v);
     tma_prefetch_desc(&map_p);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], 4);
+      mbar_init(&empty[i], 2);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -109,85 +150,31 @@ readout_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc(0, BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        mbar_wait(&acc_empty[acc], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(sA + stage * A_BYTES);
-          const uint32_t b_addr = smem_u32(sB + stage * B_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            umma_f16(d_tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc,
-                     (kb | k) != 0);
-          }
-          umma_commit(&empty[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&acc_full[acc]);
-      }
-    }
-  } else {
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may read
-    const int row = quad * 32 + lane;
-    const bool vec_ok = (p.ldo % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 15) == 0);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      int m, n;
-      tile_coords(tile, p.m_tiles, p.n_tiles, m, n);
-      const int g = m / p.tiles_per_group;
-      const long long o_row = p.out_row[g] + (long long)(m - g * p.tiles_per_group) * BM + row;
-      float* dst = p.out + o_row * p.ldo;
-      const int acc = it & 1;
-      mbar_wait(&acc_full[acc], (it >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_base + (uint32_t(quad * 32) << 16) + acc * BN + c * 32, r);
-        tmem_ld_wait();
-        const int q0 = n * BN + c * 32;
-        if (p.out_tok) {
-          const long long R = p.out_row[g] + (long long)(m - g * p.tiles_per_group) * BM + row;
-          const long long obj = R / p.rows_per_group;
-          const int ch = (int)(R - obj * p.rows_per_group);
-          __half* dt = p.out_tok + (obj * p.q) * p.rows_per_group + ch;
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (q0 + j < p.q) dt[(long long)(q0 + j) * p.rows_per_group] = __float2half_rn(__uint_as_float(r[j]));
-        } else if (q0 + 32 <= p.q && vec_ok) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float4 v = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                                   __uint_as_float(r[j + 3]));
-            *reinterpret_cast<float4*>(dst + q0 + j) = v;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (q0 + j < p.q) dst[q0 + j] = __uint_as_float(r[j]);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[acc]);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+  const bool vec_ok = (p.ldo % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 7) == 0);
+  const int qd = lane & 3;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    int m, n;
+    tile_coords(tile, p.m_tiles, p.n_tiles, m, n);
+    float d[BN / 2];
+    mma_tile(d, sA, sB, full, empty, p.k_blocks, stage, phase);
+    const int g = m / p.tiles_per_group;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int row = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+      const long long R = p.out_row[g] + (long long)(m - g * p.tiles_per_group) * BM + row;
+      float* dst = p.out + R * p.ldo;
+      __half* dt = nullptr;
+      if (p.out_tok) {
+        const long long obj = R / p.rows_per_group;
+        dt = p.out_tok + (obj * p.q) * p.rows_per_group + (R - obj * p.rows_per_group);
+      }
+      store_rows<BN>(d, i, n * BN + 2 * qd, p.q, dst, dt, p.rows_per_group, vec_ok);
+    }
   }
 }
 
@@ -200,7 +187,7 @@ readout_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_constant_
 // operand streams through TMA (16 KB instead of 48 KB per k-iteration), and no dense affinity is ever written.
 // The lists are pre-bucketed per (256-query tile, 64-slot k-block) by bucket_kernel.
 // ======================================================================================================
-constexpr int SP_THREADS = 320;   // warps: 0 TMA, 1 MMA, 2-5 epilogue, 6-9 affinity generators (one per stage)
+constexpr int SP_THREADS = CONSUMER_THREADS + 128;  // warps: 0-7 consumers, 8-11 value TMA + affinity generators (one per stage)
 constexpr int SP_REC = 1024;      // per-stage record of scattered offsets (falls back to a full clear beyond)
 constexpr int SP_SMEM = STAGES * STAGE_BYTES + 1024 + 256 + STAGES * SP_REC * 2;
 
@@ -257,9 +244,13 @@ struct SpParams {
   int reduce;
 };
 
-__device__ __forceinline__ void red_add_v4_sys(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
-               : "memory");
+// Raise the stage's expected transaction bytes without arriving (the arrive follows once the affinity tile is built).
+__device__ __forceinline__ void mbar_expect_tx_only(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+
+__device__ __forceinline__ void red_add_v2_sys(float* addr, float a, float b) {
+  asm volatile("red.relaxed.sys.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 __global__ void __launch_bounds__(SP_THREADS, 1)
@@ -271,9 +262,6 @@ readout_sparse_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_co
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  uint64_t* acc_full = bars + 2 * STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
   uint16_t* rec = reinterpret_cast<uint16_t*>(smem + STAGES * STAGE_BYTES + 256);   // [STAGES][SP_REC] byte offsets / 2
 
   const int warp = threadIdx.x >> 5;
@@ -283,46 +271,22 @@ readout_sparse_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_co
   // zero the affinity stage buffers once
   for (int i = threadIdx.x; i < STAGES * B_BYTES / 16; i += SP_THREADS)
     reinterpret_cast<uint4*>(sB)[i] = make_uint4(0, 0, 0, 0);
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&map_v);
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 2);   // TMA producer (expect_tx) + affinity generator
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], 4);
+      mbar_init(&full[i], 1);   // the stage's generator, after its scatter (the value tile completes as tx bytes)
+      mbar_init(&empty[i], 2);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        int m, n;
-        tile_coords(tile, p.m_tiles, p.n_tiles, m, n);
-        const int g = m / p.tiles_per_group;
-        const int a_row = p.val_row[g] + (m - g * p.tiles_per_group) * BM;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          mbar_expect_tx(&full[stage], A_BYTES);
-          tma_load_2d(sA + stage * A_BYTES, &map_v, &full[stage], kb * BK, a_row);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp >= 6) {
-    // ---- affinity generators: warp 6+s owns pipeline stage s (k-iterations f = s, s+4, ...), so the ~2 dependent
-    // global loads per k-block (bucket offsets, entries) have four MMA periods to complete ----
-    const int stage = warp - 6;
+  if (warp >= 8) {
+    // ---- warp 8+s owns pipeline stage s (k-iterations f = s, s+4, ...): it loads the value tile by TMA and builds the
+    // affinity tile, so the ~2 dependent global loads per k-block (bucket offsets, entries) have four MMA periods to
+    // complete ----
+    const int stage = warp - 8;
     uint8_t* tileB = sB + stage * B_BYTES;
     uint16_t* r = rec + stage * SP_REC;
     const int my_tiles = (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
@@ -340,6 +304,11 @@ readout_sparse_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_co
       if (lane < cnt) e_a = ent[e0 + lane];
       if (lane + 32 < cnt) e_b = ent[e0 + 32 + lane];
       mbar_wait(&empty[stage], (uint32_t)((f / STAGES) & 1) ^ 1u);
+      if (lane == 0) {
+        const int g = m / p.tiles_per_group;
+        mbar_expect_tx_only(&full[stage], A_BYTES);
+        tma_load_2d(sA + stage * A_BYTES, &map_v, &full[stage], kb * BK, p.val_row[g] + (m - g * p.tiles_per_group) * BM);
+      }
       // clear what the previous use of this stage scattered
       if (prev > SP_REC) {
         for (int i = lane; i < B_BYTES / 16; i += 32) reinterpret_cast<uint4*>(tileB)[i] = make_uint4(0, 0, 0, 0);
@@ -360,91 +329,41 @@ readout_sparse_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_co
       __syncwarp();
       if (lane == 0) mbar_arrive(&full[stage]);
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc(0, BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        mbar_wait(&acc_empty[acc], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(sA + stage * A_BYTES);
-          const uint32_t b_addr = smem_u32(sB + stage * B_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_f16(d_tmem, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc, (kb | k) != 0);
-          umma_commit(&empty[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&acc_full[acc]);
-      }
-    }
-  } else if (warp >= 2 && warp <= 5) {
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const bool vec_ok = (p.ldo % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 15) == 0);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
+  } else {
+    const bool vec_ok = (p.ldo % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 7) == 0);
+    const int qd = lane & 3;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int m, n;
       tile_coords(tile, p.m_tiles, p.n_tiles, m, n);
+      float d[BN / 2];
+      mma_tile(d, sA, sB, full, empty, p.k_blocks, stage, phase);
       const int g = m / p.tiles_per_group;
-      const long long R = p.out_row[g] + (long long)(m - g * p.tiles_per_group) * BM + row;
-      float* dst = (p.reduce ? p.rank_dst[p.owner[g]] : p.out) + R * p.ldo;
-      const long long obj = R / p.rows_per_group;
-      const int ch = (int)(R - obj * p.rows_per_group);
-      __half* dt = p.out_tok ? p.out_tok + (obj * p.q) * p.rows_per_group + ch : nullptr;
-      const int acc = it & 1;
-      mbar_wait(&acc_full[acc], (it >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_base + (uint32_t(quad * 32) << 16) + acc * BN + c * 32, r);
-        tmem_ld_wait();
-        const int q0 = n * BN + c * 32;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int row = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+        const long long R = p.out_row[g] + (long long)(m - g * p.tiles_per_group) * BM + row;
+        float* dst = (p.reduce ? p.rank_dst[p.owner[g]] : p.out) + R * p.ldo;
+        const long long obj = R / p.rows_per_group;
+        __half* dt = p.out_tok ? p.out_tok + (obj * p.q) * p.rows_per_group + (R - obj * p.rows_per_group) : nullptr;
         if (p.reduce) {  // partial sums of this rank's slots -> the owner's buffer (peer memory or local)
-          if (p.reduce == 1 && q0 + 32 <= p.q && p.ldo % 4 == 0) {  // 16-byte vector reductions
+          const bool vec = p.reduce == 1 && p.ldo % 2 == 0;  // 8-byte vector reductions
 #pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              red_add_v4_sys(dst + q0 + j, __uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                             __uint_as_float(r[j + 3]));
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (q0 + j < p.q) atomicAdd_system(dst + q0 + j, __uint_as_float(r[j]));
+          for (int j = 0; j < BN / 8; ++j) {
+            const int q = n * BN + 8 * j + 2 * qd;
+            if (vec && q + 1 < p.q) {
+              red_add_v2_sys(dst + q, d[4 * j + 2 * i], d[4 * j + 2 * i + 1]);
+            } else {
+              if (q < p.q) atomicAdd_system(dst + q, d[4 * j + 2 * i]);
+              if (q + 1 < p.q) atomicAdd_system(dst + q + 1, d[4 * j + 2 * i + 1]);
+            }
           }
-        } else if (dt) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (q0 + j < p.q) dt[(long long)(q0 + j) * p.rows_per_group] = __float2half_rn(__uint_as_float(r[j]));
-        } else if (q0 + 32 <= p.q && vec_ok) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(dst + q0 + j) = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                                                   __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
         } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (q0 + j < p.q) dst[q0 + j] = __uint_as_float(r[j]);
+          store_rows<BN>(d, i, n * BN + 2 * qd, p.q, dst, dt, p.rows_per_group, vec_ok);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[acc]);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -530,7 +449,7 @@ int launch_readout_sparse(const __half* values, long long values_ld, long long v
   uint32_t* entries = reinterpret_cast<uint32_t*>(offsets + (size_t)p.n_tiles * (p.k_blocks + 1));
   p.offsets = offsets; p.entries = entries;
   for (int i = 0; i < n_groups; ++i) { p.val_row[i] = val_row[i]; p.out_row[i] = out_row[i]; }
-  // DEVA_B200_SCATTER_RED=scalar: one 4-byte reduction per element instead of red.add.v4 (debugging aid)
+  // DEVA_B200_SCATTER_RED=scalar: one 4-byte reduction per element instead of red.add.v2 (debugging aid)
   static const bool scalar_red = [] { const char* e = getenv("DEVA_B200_SCATTER_RED"); return e && e[0] == 's'; }();
   p.reduce = rank_dst ? (scalar_red ? 2 : 1) : 0;
   if (rank_dst) {

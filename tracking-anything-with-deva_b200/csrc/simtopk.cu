@@ -2,17 +2,18 @@
 // (reference: get_similarity + do_softmax, deva/model/memory_utils.py:6-76).
 //
 // sim[n,q] = s_n * ( sum_c mk_cn^2 * (-qe_cq) + sum_c mk_cn * (2 qk_cq qe_cq) - bsq_q ),  s_n = shrinkage_n / sqrt(CK)
-// runs as ONE tcgen05 GEMM with K = 2*CK:   key row n = [ s*mk^2 | s*mk ],  query row q = [ -qe | 2*qk*qe ],
+// runs as ONE wgmma GEMM with K = 2*CK:   key row n = [ s*mk^2 | s*mk ],  query row q = [ -qe | 2*qk*qe ],
 // and the  - s_n * bsq_q  term is applied in the epilogue.  fp32-equivalent accuracy comes from a
-// three-term split of both operands into fp16 (hi, lo) pairs: D = Qh.Kh + Ql.Kh + Qh.Kl, fp32 accumulate in TMEM
+// three-term split of both operands into fp16 (hi, lo) pairs: D = Qh.Kh + Ql.Kh + Qh.Kl, fp32 accumulate
 // (11+11 significand bits; the dropped Ql.Kl term is ~2^-22 relative).
 //
-// CTA = 128 queries (TMEM lanes) x a contiguous range of 128-slot memory tiles; the query operand is TMA-loaded
-// once and stays resident, key tiles stream through a 2-stage ring.  Each epilogue thread owns one query: it scans
-// the accumulator row with a running threshold (current k-th best) and keeps its k best (value, slot) pairs in a
-// bank-conflict-free shared-memory column.  The memory axis can be split over several CTAs (grid.y); a small merge
-// kernel picks the global top-k, applies the softmax, accumulates per-slot usage and scatters the dense fp16
-// affinity rows consumed by the readout GEMM.
+// CTA = 64 queries x a contiguous range of 64-slot memory tiles; the query operand is TMA-loaded once and stays
+// resident, key tiles stream through a 2-stage ring.  Two consumer warpgroups take alternating tiles: each runs the
+// 64 x 64 wgmma of its tile, stages the accumulator in shared memory, and then two threads per query scan one half of
+// the tile each with a running threshold (current k-th best), keeping their k best (value, slot) pairs in a
+// bank-conflict-free shared-memory column: four candidate lists per query.  The memory axis can be split over several
+// CTAs (grid.y); a small merge kernel picks the global top-k, applies the softmax, accumulates per-slot usage and
+// scatters the dense fp16 affinity rows consumed by the readout GEMM.
 #include <cuda_fp16.h>
 #include <math_constants.h>
 
@@ -24,21 +25,23 @@
 namespace b200 {
 namespace simtopk {
 
-constexpr int BQ = 128, BNK = 64, BK = 64;
-constexpr int QTILE_BYTES = BQ * 128;   // 128 query rows x 64 halves
+constexpr int BQ = 64, BNK = 64, BK = 64;
+constexpr int QTILE_BYTES = BQ * 128;   // 64 query rows x 64 halves
 constexpr int KTILE_BYTES = BNK * 128;  // 64 key rows x 64 halves
 constexpr int MAX_KB = 2;               // 2*CK/64 with CK <= 64
-constexpr int KSTAGES = 3;
-constexpr int ACC_STAGES = 4;           // 4 x 64 TMEM columns; epilogue group g owns stages g, g+2
-constexpr int GROUPS = 2;               // epilogue warp groups working on alternating tiles
-constexpr int THREADS = 64 + GROUPS * 128;
+constexpr int KSTAGES = 2;
+constexpr int GROUPS = 2;               // consumer warpgroups working on alternating tiles
+constexpr int LISTS = 2 * GROUPS;       // candidate lists per query: (group, column half)
+static_assert(kMaxSplit * LISTS <= kMaxMergeLists, "merge: candidate lists per query");
+constexpr int THREADS = GROUPS * 128 + 32;  // warps 0..7 consumers, warp 8 TMA producer
 constexpr int Q_BYTES = 2 * MAX_KB * QTILE_BYTES;  // hi/lo x k-blocks
 constexpr int KSTAGE_BYTES = 2 * MAX_KB * KTILE_BYTES;
-constexpr int LIST_BYTES = GROUPS * 2 * kListCap * BQ * 4;
-constexpr int NS_BYTES = ACC_STAGES * BNK * 4;
-static_assert(GROUPS == 2, "the threshold exchange pairs group g with group g ^ 1");
-constexpr int THR_BYTES = GROUPS * BQ * 4;  // each epilogue group publishes its running k-th best per query
-constexpr int SMEM_BYTES = Q_BYTES + KSTAGES * KSTAGE_BYTES + LIST_BYTES + NS_BYTES + 256 + THR_BYTES;
+constexpr int LIST_BYTES = LISTS * 2 * kListCap * BQ * 4;
+constexpr int STG_PITCH = BNK + 4;      // fp32 accumulator staging row pitch (conflict-free float4 row reads)
+constexpr int STG_BYTES = GROUPS * BQ * STG_PITCH * 4;
+constexpr int NS_BYTES = GROUPS * BNK * 4;
+constexpr int THR_BYTES = LISTS * BQ * 4;  // each list publishes its running k-th best per query
+constexpr int SMEM_BYTES = Q_BYTES + KSTAGES * KSTAGE_BYTES + LIST_BYTES + STG_BYTES + NS_BYTES + 256 + THR_BYTES;
 static_assert(SMEM_BYTES <= 232448, "simtopk: shared-memory budget");
 
 struct Params {
@@ -47,7 +50,7 @@ struct Params {
   int qpad;
   const float* neg_s;   // [n_window]  -shrinkage/sqrt(CK)
   const float* bsq;     // [q]
-  float* part_val;      // [nsplit*GROUPS][kListCap][qpad]
+  float* part_val;      // [nsplit*LISTS][kListCap][qpad]
   int* part_idx;
   float* dense_out;     // DENSE mode: [q][ld_dense]
   long long ld_dense;
@@ -116,17 +119,15 @@ simtopk_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* sQ = smem;                                   // [hi/lo][kb] query tiles, resident
   uint8_t* sK = smem + Q_BYTES;                         // [stage][hi/lo][kb] key tiles
-  float* list_val = reinterpret_cast<float*>(sK + KSTAGES * KSTAGE_BYTES);   // [group][kListCap][BQ]
-  int* list_idx = reinterpret_cast<int*>(list_val + GROUPS * kListCap * BQ);
-  float* ns = reinterpret_cast<float*>(list_idx + GROUPS * kListCap * BQ);   // [ACC_STAGES][BNK]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ns + ACC_STAGES * BNK);
+  float* list_val = reinterpret_cast<float*>(sK + KSTAGES * KSTAGE_BYTES);   // [list][kListCap][BQ]
+  int* list_idx = reinterpret_cast<int*>(list_val + LISTS * kListCap * BQ);
+  float* stg = reinterpret_cast<float*>(list_idx + LISTS * kListCap * BQ);   // [group][BQ][STG_PITCH]
+  float* ns = stg + GROUPS * BQ * STG_PITCH;                                 // [group][BNK]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ns + GROUPS * BNK);
   uint64_t* q_full = bars;
   uint64_t* full = bars + 1;                    // [KSTAGES]
   uint64_t* empty = full + KSTAGES;             // [KSTAGES]
-  uint64_t* acc_full = empty + KSTAGES;         // [ACC_STAGES]
-  uint64_t* acc_empty = acc_full + ACC_STAGES;  // [ACC_STAGES]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + ACC_STAGES);
-  volatile float* thr_pub = reinterpret_cast<volatile float*>(reinterpret_cast<uint8_t*>(bars) + 256);  // [GROUPS][BQ]
+  volatile float* thr_pub = reinterpret_cast<volatile float*>(reinterpret_cast<uint8_t*>(bars) + 256);  // [LISTS][BQ]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -134,21 +135,16 @@ simtopk_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
   const int t_begin = blockIdx.y * p.tiles_per_split;
   const int t_end = min(p.tiles_total, t_begin + p.tiles_per_split);
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&map_qh); tma_prefetch_desc(&map_ql);
     tma_prefetch_desc(&map_kh); tma_prefetch_desc(&map_kl);
     mbar_init(q_full, 1);
     for (int i = 0; i < KSTAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < ACC_STAGES; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 4); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<256>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(q_full, 2u * p.kblocks * QTILE_BYTES);
       for (int kb = 0; kb < p.kblocks; ++kb) {
@@ -168,139 +164,128 @@ simtopk_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
         if (++stage == KSTAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc(0, BQ, BNK);
-      mbar_wait(q_full, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int t = t_begin; t < t_end; ++t, ++it) {
-        const int acc = it & (ACC_STAGES - 1);
-        mbar_wait(&acc_empty[acc], ((it / ACC_STAGES) & 1) ^ 1);
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BNK;
-        const uint32_t k_base = smem_u32(sK + stage * KSTAGE_BYTES);
-        const uint32_t q_base = smem_u32(sQ);
-        for (int kb = 0; kb < p.kblocks; ++kb) {
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t qh = umma_desc_sw128(q_base + (0 * MAX_KB + kb) * QTILE_BYTES + k * 32);
-            const uint64_t ql = umma_desc_sw128(q_base + (1 * MAX_KB + kb) * QTILE_BYTES + k * 32);
-            const uint64_t kh = umma_desc_sw128(k_base + (0 * MAX_KB + kb) * KTILE_BYTES + k * 32);
-            const uint64_t kl = umma_desc_sw128(k_base + (1 * MAX_KB + kb) * KTILE_BYTES + k * 32);
-            umma_f16(d_tmem, ql, kh, idesc, (kb | k) != 0);
-            umma_f16(d_tmem, qh, kl, idesc, 1);
-            umma_f16(d_tmem, qh, kh, idesc, 1);
-          }
-        }
-        umma_commit(&empty[stage]);
-        umma_commit(&acc_full[acc]);
-        if (++stage == KSTAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else {
-    const int group = (warp - 2) >> 2;  // 0: even local tiles, 1: odd local tiles
-    const int quad = warp & 3;          // TMEM lane quadrant this warp may read
-    const int row = quad * 32 + lane;   // query within the tile == TMEM lane
-    const int qg = q0 + row;
-    const float bsq = (qg < p.q) ? p.bsq[qg] : 0.f;
-    const int top_k = p.top_k;
-    // Nothing at or below a valid lower bound of the k-th best similarity can be in the top-k: with the bound taken from
-    // the slots the previous frame selected, only a handful of candidates per query ever reach the insertion path.
-    const float floor_thr = (!DENSE && p.thr_floor && qg < p.q) ? p.thr_floor[qg] : -CUDART_INF_F;
-    float* lv = list_val + group * kListCap * BQ;
-    int* li = list_idx + group * kListCap * BQ;
-    TopK tk;
-    if (!DENSE) {
-      for (int j = 0; j < kListCap; ++j) {
-        lv[j * BQ + row] = (j < top_k) ? -CUDART_INF_F : CUDART_INF_F;
-        li[j * BQ + row] = -1;
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        tk.gmin[i] = (i * 8 < top_k) ? -CUDART_INF_F : CUDART_INF_F;
-        tk.gpos[i] = i * 8;
-      }
-      tk.refresh();
-      // The two groups scan alternating tiles of the SAME queries into separate lists.  Each publishes its running k-th
-      // best; the other group's value is a valid lower bound of the query's global k-th best (its list holds k real
-      // candidates at least that large), so gating on it keeps every global top-k member while cutting the insertions
-      // of two half-length lists to about those of one full-length list.  Stale reads are fine: the bound only grows.
-      thr_pub[group * BQ + row] = -CUDART_INF_F;
-      named_bar_sync(3, GROUPS * 128);
-    }
-    volatile const float* thr_other = thr_pub + (group ^ 1) * BQ + row;
-    for (int it = group; t_begin + it < t_end; it += GROUPS) {
-      const int acc = it & (ACC_STAGES - 1);
-      const int n0 = (t_begin + it) * BNK;
-      if (row < BNK) {
-        const int n = n0 + row;
-        ns[acc * BNK + row] = (n >= p.n_lead && n < p.n_window) ? p.neg_s[n] : -CUDART_INF_F;
-      }
-      named_bar_sync(1 + group, 128);
-      mbar_wait(&acc_full[acc], (it / ACC_STAGES) & 1);
-      tc_fence_after();
-      const float4* ns4 = reinterpret_cast<const float4*>(ns + acc * BNK);
-#pragma unroll 1
-      for (int c = 0; c < BNK / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_base + (uint32_t(quad * 32) << 16) + acc * BNK + c * 32, r);
-        tmem_ld_wait();
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 s4 = ns4[c * 8 + j];
-          v[4 * j + 0] = fmaf(s4.x, bsq, __uint_as_float(r[4 * j + 0]));
-          v[4 * j + 1] = fmaf(s4.y, bsq, __uint_as_float(r[4 * j + 1]));
-          v[4 * j + 2] = fmaf(s4.z, bsq, __uint_as_float(r[4 * j + 2]));
-          v[4 * j + 3] = fmaf(s4.w, bsq, __uint_as_float(r[4 * j + 3]));
-        }
-        if (DENSE) {
-          if (qg < p.q) {
-            float* dst = p.dense_out + (long long)qg * p.ld_dense + n0 + c * 32;
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (n0 + c * 32 + j < p.n_window) dst[j] = (v[j] == v[j]) ? v[j] : -CUDART_INF_F;
-          }
-        } else {
-          // Bit j of `pending` = column j beats this query's current k-th best.  Lanes then retire their
-          // pending candidates in lock-step (1st of every lane, 2nd of every lane, ...): the warp pays for
-          // max-per-lane insertions per chunk, not for every distinct column position.
-          uint32_t pending = 0;
-          const float gate = fmaxf(fmaxf(tk.thr, floor_thr), *thr_other);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) pending |= (v[j] > gate) ? (1u << j) : 0u;
-          while (__any_sync(0xffffffffu, pending != 0)) {
-            if (pending) {
-              const int j = __ffs(pending) - 1;
-              pending &= pending - 1;
-              const float x = pick32(v, j);
-              if (x > tk.thr) tk.insert(lv, li, row, x, n0 + c * 32 + j);
-            }
-          }
-          thr_pub[group * BQ + row] = tk.thr;
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[acc]);
-    }
-    if (!DENSE) {
-      const long long base = ((long long)blockIdx.y * GROUPS + group) * kListCap;
-      for (int j = 0; j < top_k; ++j) {
-        p.part_val[(base + j) * p.qpad + qg] = lv[j * BQ + row];
-        p.part_idx[(base + j) * p.qpad + qg] = li[j * BQ + row];
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<256>(tmem_base);
+  const int group = warp >> 2;        // 0: even local tiles, 1: odd local tiles
+  const int tid = threadIdx.x & 127;  // thread within the group's warpgroup
+  const int row = tid & (BQ - 1);     // query within the tile
+  const int half = tid >> 6;          // 32-column half of the tile this thread scans
+  const int list = group * 2 + half;
+  const int qg = q0 + row;
+  const float bsq = (qg < p.q) ? p.bsq[qg] : 0.f;
+  const int top_k = p.top_k;
+  // Nothing at or below a valid lower bound of the k-th best similarity can be in the top-k: with the bound taken from
+  // the slots the previous frame selected, only a handful of candidates per query ever reach the insertion path.
+  const float floor_thr = (!DENSE && p.thr_floor && qg < p.q) ? p.thr_floor[qg] : -CUDART_INF_F;
+  float* lv = list_val + list * kListCap * BQ;
+  int* li = list_idx + list * kListCap * BQ;
+  float* my_stg = stg + group * BQ * STG_PITCH;
+  float* my_ns = ns + group * BNK;
+  TopK tk;
+  if (!DENSE) {
+    for (int j = 0; j < kListCap; ++j) {
+      lv[j * BQ + row] = (j < top_k) ? -CUDART_INF_F : CUDART_INF_F;
+      li[j * BQ + row] = -1;
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      tk.gmin[i] = (i * 8 < top_k) ? -CUDART_INF_F : CUDART_INF_F;
+      tk.gpos[i] = i * 8;
+    }
+    tk.refresh();
+    // The two halves scan disjoint columns of the SAME queries into separate lists.  Each publishes its running k-th
+    // best; the other's value is a valid lower bound of the query's global k-th best (its list holds k real candidates
+    // at least that large), so gating on it keeps every global top-k member while cutting the insertions of two
+    // half-length lists to about those of one full-length list.  Stale reads are fine: the bound only grows.
+    thr_pub[list * BQ + row] = -CUDART_INF_F;
+    named_bar_sync(3, GROUPS * 128);
+  }
+  volatile const float* thr_other = thr_pub + (list ^ 1) * BQ + row;
+  mbar_wait(q_full, 0);
+  const uint32_t q_base = smem_u32(sQ);
+  for (int it = group; t_begin + it < t_end; it += GROUPS) {
+    const int stage = it % KSTAGES;
+    const int n0 = (t_begin + it) * BNK;
+    float d[BNK / 2];
+    mbar_wait(&full[stage], (it / KSTAGES) & 1);
+    const uint32_t k_base = smem_u32(sK + stage * KSTAGE_BYTES);
+    wgmma_fence();
+    for (int kb = 0; kb < p.kblocks; ++kb) {
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t qh = wgmma_desc_sw128(q_base + (0 * MAX_KB + kb) * QTILE_BYTES + k * 32);
+        const uint64_t ql = wgmma_desc_sw128(q_base + (1 * MAX_KB + kb) * QTILE_BYTES + k * 32);
+        const uint64_t kh = wgmma_desc_sw128(k_base + (0 * MAX_KB + kb) * KTILE_BYTES + k * 32);
+        const uint64_t kl = wgmma_desc_sw128(k_base + (1 * MAX_KB + kb) * KTILE_BYTES + k * 32);
+        wgmma_f16<BNK>(d, ql, kh, (kb | k) != 0);
+        wgmma_f16<BNK>(d, qh, kl, 1);
+        wgmma_f16<BNK>(d, qh, kh, 1);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(d);
+    if (tid == 0) mbar_arrive(&empty[stage]);
+    named_bar_sync(1 + group, 128);  // the previous tile's staging / ns reads are done
+    if (tid < BNK) {
+      const int n = n0 + tid;
+      my_ns[tid] = (n >= p.n_lead && n < p.n_window) ? p.neg_s[n] : -CUDART_INF_F;
+    }
+#pragma unroll
+    for (int j = 0; j < BNK / 8; ++j)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int r = (warp & 3) * 16 + (lane >> 2) + 8 * i;
+        *reinterpret_cast<float2*>(my_stg + r * STG_PITCH + 8 * j + 2 * (lane & 3)) =
+            make_float2(d[4 * j + 2 * i], d[4 * j + 2 * i + 1]);
+      }
+    named_bar_sync(1 + group, 128);
+    const float4* ns4 = reinterpret_cast<const float4*>(my_ns + half * 32);
+    const float4* acc4 = reinterpret_cast<const float4*>(my_stg + row * STG_PITCH + half * 32);
+    float v[32];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float4 s4 = ns4[j];
+      const float4 a4 = acc4[j];
+      v[4 * j + 0] = fmaf(s4.x, bsq, a4.x);
+      v[4 * j + 1] = fmaf(s4.y, bsq, a4.y);
+      v[4 * j + 2] = fmaf(s4.z, bsq, a4.z);
+      v[4 * j + 3] = fmaf(s4.w, bsq, a4.w);
+    }
+    const int c0 = n0 + half * 32;
+    if (DENSE) {
+      if (qg < p.q) {
+        float* dst = p.dense_out + (long long)qg * p.ld_dense + c0;
+#pragma unroll
+        for (int j = 0; j < 32; ++j)
+          if (c0 + j < p.n_window) dst[j] = (v[j] == v[j]) ? v[j] : -CUDART_INF_F;
+      }
+    } else {
+      // Bit j of `pending` = column j beats this query's current k-th best.  Lanes then retire their
+      // pending candidates in lock-step (1st of every lane, 2nd of every lane, ...): the warp pays for
+      // max-per-lane insertions per tile, not for every distinct column position.
+      uint32_t pending = 0;
+      const float gate = fmaxf(fmaxf(tk.thr, floor_thr), *thr_other);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) pending |= (v[j] > gate) ? (1u << j) : 0u;
+      while (__any_sync(0xffffffffu, pending != 0)) {
+        if (pending) {
+          const int j = __ffs(pending) - 1;
+          pending &= pending - 1;
+          const float x = pick32(v, j);
+          if (x > tk.thr) tk.insert(lv, li, row, x, c0 + j);
+        }
+      }
+      thr_pub[list * BQ + row] = tk.thr;
+    }
+  }
+  if (!DENSE) {
+    const long long base = ((long long)blockIdx.y * LISTS + list) * kListCap;
+    for (int j = 0; j < top_k; ++j) {
+      p.part_val[(base + j) * p.qpad + qg] = lv[j * BQ + row];
+      p.part_idx[(base + j) * p.qpad + qg] = li[j * BQ + row];
+    }
   }
 }
 
@@ -311,8 +296,8 @@ merge_kernel(const float* __restrict__ part_val, const int* __restrict__ part_id
              int qpad, int* __restrict__ out_idx, float* __restrict__ out_w, __half* __restrict__ P, long long ldP,
              float* __restrict__ use_cnt, int n_long, int add_long, int add_work, float* __restrict__ out_sim) {
   // row pitch = 4 mod 32: the staging writes of a warp (4 candidates x 8 queries) and the per-warp scans are conflict-free
-  __shared__ float cv[MERGE_WARPS][kMaxSplit * GROUPS * kListCap + 4];
-  __shared__ int ci[MERGE_WARPS][kMaxSplit * GROUPS * kListCap + 4];
+  __shared__ float cv[MERGE_WARPS][kMaxMergeLists * kListCap + 4];
+  __shared__ int ci[MERGE_WARPS][kMaxMergeLists * kListCap + 4];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qb = blockIdx.x * MERGE_WARPS;
   const int C = nsplit * top_k;
@@ -467,8 +452,8 @@ static int make_maps(CUtensorMap* m, const __half* q_hi, const __half* q_lo, int
                      const __half* k_lo, int n_window, int ck) {
   const char* err = nullptr;
   const uint64_t kdim = 2ull * ck;
-  if (make_tmap_2d(&m[0], TmapType::F16, q_hi, kdim, q, kdim * 2, 64, 128, &err) ||
-      make_tmap_2d(&m[1], TmapType::F16, q_lo, kdim, q, kdim * 2, 64, 128, &err) ||
+  if (make_tmap_2d(&m[0], TmapType::F16, q_hi, kdim, q, kdim * 2, 64, simtopk::BQ, &err) ||
+      make_tmap_2d(&m[1], TmapType::F16, q_lo, kdim, q, kdim * 2, 64, simtopk::BQ, &err) ||
       make_tmap_2d(&m[2], TmapType::F16, k_hi, kdim, n_window, kdim * 2, 64, 64, &err) ||
       make_tmap_2d(&m[3], TmapType::F16, k_lo, kdim, n_window, kdim * 2, 64, 64, &err)) {
     set_error("simtopk: %s", err ? err : "tensor map");
@@ -493,8 +478,8 @@ static int choose_split(int q_tiles, int tiles, int max_split) {
 }
 
 size_t simtopk_workspace_bytes(int q) {
-  const size_t qpad = (size_t)ceil_div(q, 128) * 128;
-  return (size_t)kMaxSplit * simtopk::GROUPS * kListCap * qpad * 8;
+  const size_t qpad = (size_t)ceil_div(q, simtopk::BQ) * simtopk::BQ;
+  return (size_t)kMaxSplit * simtopk::LISTS * kListCap * qpad * 8;
 }
 
 int launch_sim_topk(const __half* k_hi, const __half* k_lo, const float* neg_s, int n_window, int n_lead,
@@ -520,7 +505,7 @@ int launch_sim_topk(const __half* k_hi, const __half* k_lo, const float* neg_s, 
   p.qpad = q_tiles * BQ;
   p.neg_s = neg_s; p.bsq = bsq;
   p.part_val = reinterpret_cast<float*>(workspace);
-  p.part_idx = reinterpret_cast<int*>(p.part_val + (size_t)kMaxSplit * GROUPS * kListCap * p.qpad);
+  p.part_idx = reinterpret_cast<int*>(p.part_val + (size_t)kMaxSplit * LISTS * kListCap * p.qpad);
   static bool configured_dev[kMaxDevices] = {false};  // function attributes are per device
   bool& configured = configured_dev[device_slot()];
   if (!configured) {
@@ -539,7 +524,7 @@ int launch_sim_topk(const __half* k_hi, const __half* k_lo, const float* neg_s, 
   simtopk_kernel<false><<<dim3(q_tiles, nsplit), THREADS, SMEM_BYTES, stream>>>(maps[0], maps[1], maps[2], maps[3], p);
   B200_LAUNCH_CHECK();
   merge_kernel<<<ceil_div(q, MERGE_WARPS), MERGE_WARPS * 32, 0, stream>>>(
-      p.part_val, p.part_idx, nsplit * GROUPS, top_k, q, p.qpad, out_idx, out_w, P, ldP, use_cnt, n_long, count_long,
+      p.part_val, p.part_idx, nsplit * LISTS, top_k, q, p.qpad, out_idx, out_w, P, ldP, use_cnt, n_long, count_long,
       count_work, out_sim);
   B200_LAUNCH_CHECK();
   if (life_cnt) {
@@ -559,7 +544,7 @@ int launch_sim_topk(const __half* k_hi, const __half* k_lo, const float* neg_s, 
 int launch_merge_lists(const float* part_val, const int* part_idx, int n_lists, int top_k, int q, int qpad, int* out_idx,
                        float* out_w, float* out_sim, cudaStream_t stream) {
   using namespace simtopk;
-  B200_REQUIRE(n_lists >= 1 && n_lists <= kMaxSplit * GROUPS, "merge: n_lists %d out of range [1,%d]", n_lists, kMaxSplit * GROUPS);
+  B200_REQUIRE(n_lists >= 1 && n_lists <= kMaxMergeLists, "merge: n_lists %d out of range [1,%d]", n_lists, kMaxMergeLists);
   B200_REQUIRE(top_k >= 1 && top_k <= kListCap && q >= 1 && qpad >= q, "merge: bad shape");
   merge_kernel<<<ceil_div(q, MERGE_WARPS), MERGE_WARPS * 32, 0, stream>>>(part_val, part_idx, n_lists, top_k, q, qpad, out_idx,
                                                                          out_w, nullptr, 0, nullptr, 0, 0, 0, out_sim);

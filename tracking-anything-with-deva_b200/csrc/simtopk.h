@@ -5,7 +5,7 @@
 
 namespace b200 {
 constexpr int kListCap = 32;  // max top_k; also the row pitch of the idx / weight outputs
-constexpr int kMaxSplit = 8;  // max CTAs sharing one 128-query tile along the memory axis
+constexpr int kMaxSplit = 4;  // max CTAs sharing one 64-query tile along the memory axis
 
 size_t simtopk_workspace_bytes(int q);
 

@@ -1,4 +1,4 @@
-"""Drop-in ``deva`` package: DEVA's propagation API on B200-native kernels.
+"""Drop-in ``deva`` package: DEVA's propagation API on H100-native kernels.
 
 Same import surface as the reference (deva/__init__.py:1-2): ``deva.DEVAInferenceCore`` and
 ``deva.DEVA``.  Imports are lazy so that pure-host modules (checkpoint spec, object bookkeeping)

@@ -1,6 +1,6 @@
 """ctypes binding of libdeva_b200.so (C ABI declared in include/deva_b200.h).
 
-This is the only door between the Python host code and the sm_100a kernels.  There is no
+This is the only door between the Python host code and the sm_90a kernels.  There is no
 fallback: if the library is missing, was built for another ABI version, or a kernel reports an
 error, a RuntimeError is raised.  PyTorch is used for device memory and streams only.
 """
@@ -138,7 +138,7 @@ def launch_count() -> int:
 
 def require_device():
     if not torch.cuda.is_available():
-        raise RuntimeError('deva_b200: no CUDA device; the sm_100a kernels have no CPU fallback')
+        raise RuntimeError('deva_b200: no CUDA device; the sm_90a kernels have no CPU fallback')
     _check(lib().deva_b200_device_check(), 'device_check')
 
 

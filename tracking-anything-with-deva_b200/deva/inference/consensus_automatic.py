@@ -2,7 +2,7 @@
 (API of the reference's deva/inference/consensus_automatic.py:82-272).
 
 Every buffered frame's detections are projected onto a keyframe (``spatial_alignment``: one frame of the propagation
-hot path, on the B200 kernels), segments of different frames that overlap with IoU > 0.5 support each other, and the
+hot path, on the H100 kernels), segments of different frames that overlap with IoU > 0.5 support each other, and the
 subset of segments that maximises ``sum_i x_i * (2 * support_i - 1)`` with no two overlapping segments selected is
 kept.  The reference states that selection as an integer program and hands it to gurobi / pulp
 (consensus_automatic.py:28-79); the constraint graph is the IoU > 0.5 match graph, so the program is a maximum-weight

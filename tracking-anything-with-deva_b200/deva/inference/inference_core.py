@@ -2,7 +2,7 @@
 
 ``DEVAInferenceCore`` keeps the reference's constructor, methods, attributes and side effects so that
 ``evaluation/eval_vos.py`` and the ``deva/ext`` detector hooks can drive it unchanged; the work it
-schedules runs on the B200 kernels (memory read / bank) and the engine (conv stack).
+schedules runs on the H100 kernels (memory read / bank) and the engine (conv stack).
 """
 import warnings
 from typing import Dict, Iterable, List, Literal, Optional

@@ -16,7 +16,7 @@ no stacking of per-object values (:83-89).  Slot order inside the long-term regi
 the reference's; top-k, softmax and readout are order independent, so only fp summation order
 differs.
 
-Per token: packed fp16 key rows (hi, lo) for the tcgen05 similarity GEMM, -shrinkage/sqrt(CK),
+Per token: packed fp16 key rows (hi, lo) for the wgmma similarity GEMM, -shrinkage/sqrt(CK),
 fp32 copies of key / selection / shrinkage (API views, consolidation), usage counters.
 Per object: a [CV, cap] fp16 value matrix (memory-slot axis contiguous = K-major GEMM operand).
 """

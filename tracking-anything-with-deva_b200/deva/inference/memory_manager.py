@@ -1,7 +1,7 @@
-"""Working / long-term / sensory memory on B200 (API of deva/inference/memory_manager.py:14-292).
+"""Working / long-term / sensory memory on H100 (API of deva/inference/memory_manager.py:14-292).
 
 Same class, method names, argument meaning and error behaviour as the reference's ``MemoryManager``;
-the math runs in the sm_100a kernels behind ``deva._native``:
+the math runs in the sm_90a kernels behind ``deva._native``:
 
 * ``match_memory``  = pack_query -> per bucket [sim_topk (fused similarity / top-k / softmax / usage)
   -> readout GEMM] writing straight into one [K, CV, h, w] buffer in temporary-id order;

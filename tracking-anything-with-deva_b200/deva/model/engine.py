@@ -13,9 +13,9 @@ call.  The engine instead
 * expresses the forward passes against a small op set implemented by a backend.
 
 Backends: ``TorchOps`` (cuDNN/cuBLAS through ATen, fp32 NCHW) is the interim implementation of the conv
-stack while the hand-written NHWC tcgen05 implicit-GEMM kernels land layer by layer; it is library code
+stack while the hand-written NHWC wgmma implicit-GEMM kernels land layer by layer; it is library code
 on the device, never a CPU path.  The memory read never goes through a backend - it is always the
-sm_100a kernels in deva/inference/memory_manager.py.
+sm_90a kernels in deva/inference/memory_manager.py.
 """
 from typing import Dict, Optional, Tuple
 

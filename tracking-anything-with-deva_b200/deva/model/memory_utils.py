@@ -1,4 +1,4 @@
-"""Functional memory-read API (names of deva/model/memory_utils.py:6-94) on the sm_100a kernels.
+"""Functional memory-read API (names of deva/model/memory_utils.py:6-94) on the sm_90a kernels.
 
 ``get_similarity`` / ``do_softmax`` / ``readout`` are what ``consensus_associated.spatial_alignment`` and user
 code call directly.  The fused production path is ``MemoryManager.match_memory``; these helpers expose

@@ -1,4 +1,4 @@
-"""The DEVA propagation network on the hand-written sm_100a kernels (NHWC fp16, tcgen05 implicit GEMM).
+"""The DEVA propagation network on the hand-written sm_90a kernels (NHWC fp16, wgmma implicit GEMM).
 
 Same forward graphs as ``deva.model.engine.Engine`` (which restates the reference's network.py /
 big_modules.py / modules.py / group_modules.py / cbam.py / resnet.py with BatchNorm folded and the
@@ -150,8 +150,8 @@ class NativeEngine:
         _, h, w, _ = x.shape
         pc = self.P['key_proj.all']
         # split-K: the projection's 3 x 9 x Cin/64 k-iterations run as KSPLIT short accumulation chains whose fp32 partial
-        # sums key_tail adds on the CUDA cores.  One TMEM accumulator over the whole loop (round-toward-zero at every
-        # step) left the keys 7.5e-5 off - enough to flip near-tied top-k members (profiles/r02_keypath_accumulation.md).
+        # sums key_tail adds on the CUDA cores.  One accumulator over the whole loop (round-toward-zero at every
+        # step) leaves a systematic error in the keys that can flip near-tied top-k members (tools/accum_probe.py).
         y = ops.conv_ex(x, pc, x_lo=lo, want_f32=True, ksplit=self.key_ksplit).f32  # [parts,1,h,w,2*CK+1] fp32
         q, ck = h * w, self.key_dim
         key = torch.empty(q, ck, dtype=torch.float32, device=x.device)

@@ -1,4 +1,4 @@
-"""Host-side wrappers of the sm_100a network kernels: weight packing, tile choice, op calls.
+"""Host-side wrappers of the sm_90a network kernels: weight packing, tile choice, op calls.
 
 Activations are fp16 NHWC torch tensors [B, H, W, C]; weights are packed once per checkpoint into the
 layout the implicit-GEMM kernel streams with TMA ([Cout_pad, taps * Cin_pad] fp16, BN folded bias fp32).
@@ -161,10 +161,10 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
     def new(dtype=torch.float16):
         return torch.empty(b, ho, wo, pc.cout, dtype=dtype, device=dev)
 
-    # Split-precision layers keep at most MAX_CHAIN k-iterations in one TMEM accumulator: the tensor core rounds toward
+    # Split-precision layers keep at most MAX_CHAIN k-iterations in one accumulator: the tensor core rounds toward
     # zero at every accumulation step, and a deep K loop (3x3 x 256 channels x 3 passes = 108 k-iterations) leaves a
-    # systematic ~1e-5 relative error that the top-k read downstream of the key path does not tolerate
-    # (tools/accum_probe.py, profiles/r02_keypath_accumulation.md).  Longer loops run as chains of <= CHAIN k-iterations
+    # systematic relative error that the top-k read downstream of the key path does not tolerate
+    # (tools/accum_probe.py measures it).  Longer loops run as chains of <= CHAIN k-iterations
     # whose fp32 partial sums are added - with the bias, the residual and the output conversions - by sum_parts.
     k_iters = pc.k * pc.k * (pc.cin_pad // 64) * (3 if pc.precise else (2 if (pc.act_lo or pc.w_lo or pc.two_inputs) else 1))
     if (pc.precise and ksplit == 0 and k_iters > MAX_CHAIN and not (want_f32 or head_w is not None or pc.rank1_w is not None)

@@ -43,7 +43,7 @@ class DEVA(nn.Module):
                 node.register_parameter(leaf, nn.Parameter(init[name].clone(), requires_grad=False))
         self._engine = None
         self._engine_key = None
-        # 'native' = hand-written sm_100a conv stack (default); 'torch' = cuDNN/ATen fp32 (debug / comparison only)
+        # 'native' = hand-written sm_90a conv stack (default); 'torch' = cuDNN/ATen fp32 (debug / comparison only)
         self.conv_backend = os.environ.get('DEVA_B200_CONV', 'native')
         self.return_full_logits = True  # segment() also returns the up-sampled logits like the reference
 
