@@ -9,7 +9,10 @@ from deva.model import native_ops as ops  # noqa: E402
 CASES = {
     # name: (batch, h, w, cin, cout, k, mode)
     'up84_c1': (16, 272, 480, 256, 256, 3, 'relu'),
-    'up84_c1_actlo': (16, 272, 480, 256, 256, 3, 'actlo'),   # parity plan: activations as (hi, lo), two MMA passes
+    'up84_c1_actlo': (16, 272, 480, 256, 256, 3, 'actlo'),   # activations as (hi, lo), two fp16 MMA passes
+    # what up_8_4.out_conv.c1 runs in the parity plan: an e4m3 correction pass over the low-order activations, then the
+    # fp16 pass, writing the ReLU'd output and its e4m3 low-order part for the next layer
+    'up84_c1_lo8': (16, 272, 480, 256, 256, 3, 'actlo8'),
     'up84_c2_res': (16, 272, 480, 256, 256, 3, 'raw+res'),
     'up84_c2_head': (16, 272, 480, 256, 256, 3, 'raw+res+head'),
     'gru': (16, 68, 120, 512, 1536, 3, 'two'),
@@ -36,7 +39,7 @@ def run(name, iters=8):
     wgt = torch.randn(cout, cin * (2 if two else 1), k, k, device=dev, generator=g) / (cin * k * k)**0.5
     bias = torch.randn(cout, device=dev, generator=g)
     pc = ops.PackedConv(wgt, bias, 1, two_inputs=two, precise=(mode == 'precise'), act_lo=(mode == 'actlo'),
-                        gates=(mode == 'gates'), nt_override=192 if mode == 'two192' else None)
+                        act_lo8=(mode == 'actlo8'), gates=(mode == 'gates'), nt_override=192 if mode == 'two192' else None)
     kw = {}
     if two:
         kw['x2'] = torch.randn_like(x)
@@ -44,6 +47,8 @@ def run(name, iters=8):
         kw['gate_h'] = kw['x2']
     if mode in ('precise', 'actlo'):
         kw['x_lo'] = (torch.randn_like(x) * 1e-3)
+    if mode == 'actlo8':  # e4m3 of (x - fp16(x)) * 4096
+        kw['x_lo8'] = (torch.randn_like(x, dtype=torch.float32) * 4).to(torch.float8_e4m3fn).view(torch.uint8)
     if 'res' in mode:
         kw['res'] = torch.randn(b, h, w, cout, device=dev, generator=g).half()
     if 'head' in mode:
@@ -51,7 +56,10 @@ def run(name, iters=8):
     want = dict(want_relu=True) if mode in ('relu', ) else (dict() if mode == 'gates' else dict(want_raw=True))
     if mode in ('precise', 'actlo'):
         want = dict(want_relu=True, want_lo=True)
-    passes = 3 if mode == 'precise' else (2 if (two or mode == 'actlo') else 1)
+    if mode == 'actlo8':
+        want = dict(want_relu=True, want_relu_lo8=True)
+    # fp16-equivalent MMA passes; the e4m3 pass does the same MACs at twice the rate, so it counts as half a pass
+    passes = 3 if mode == 'precise' else (2 if (two or mode == 'actlo') else (1.5 if mode == 'actlo8' else 1))
     flops = 2.0 * b * h * w * cout * k * k * pc.cin_pad * passes
     for _ in range(3):
         ops.conv_ex(x, pc, **kw, **want)
@@ -66,10 +74,37 @@ def run(name, iters=8):
     return dict(case=name, ms=ms, tflops=flops / ms / 1e9, gflop=flops / 1e9)
 
 
+# The measured fp16 tensor-core ceiling on the card at hand: cuBLAS on one GEMM with the N and K of up84_c1 (Cout 256,
+# 3x3 x 256 channels) and M = 8 waves of 128-row tiles on 132 SMs.
+MATMULS = {'cublas_up84': (132 * 128 * 8, 256, 9 * 256)}
+
+
+def run_matmul(name, iters=8, reps=10):
+    m, n, k = MATMULS[name]
+    g = torch.Generator(device='cuda').manual_seed(0)
+    a = torch.randn(m, k, device='cuda', generator=g).half()
+    b = torch.randn(k, n, device='cuda', generator=g).half()
+    for _ in range(3):
+        torch.matmul(a, b)
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(iters):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            torch.matmul(a, b)
+        e1.record(); torch.cuda.synchronize()
+        ts.append(e0.elapsed_time(e1) / reps)
+    ts.sort()
+    ms = ts[len(ts) // 2]
+    flops = 2.0 * m * n * k
+    return dict(case=name, ms=ms, tflops=flops / ms / 1e9, gflop=flops / 1e9)
+
+
 if __name__ == '__main__':
     ap = argparse.ArgumentParser()
-    ap.add_argument('--cases', default=','.join(CASES))
+    ap.add_argument('--cases', default=','.join([*CASES, *MATMULS]))
     a = ap.parse_args()
     nat.require_device()
     for c in a.cases.split(','):
-        print(json.dumps(run(c)))
+        print(json.dumps(run_matmul(c) if c in MATMULS else run(c)))

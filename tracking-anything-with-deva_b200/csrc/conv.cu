@@ -17,10 +17,14 @@
 //   batch-broadcast), + optional rank-1 term w1[cout] * x1[b, pixel] (the "+1" mask / logit input channel of
 //   sensory_compress and g4_conv), then writes any of: raw fp16, ReLU'd fp16, raw fp32.
 // Warp roles: warps 0..7 = two consumer warpgroups (pixels 0..63 / 64..127 of the tile: wgmma m64nNk16 + epilogue),
-//   warp 8 = TMA producer.  Persistent CTAs, 4-stage shared-memory ring; the producer fills the ring for the next
-//   tile while the consumers run the epilogue of the current one.
+//   warps 8..11 = producer warpgroup, of which one thread issues the TMA loads.  The producer warpgroup exists so
+//   that setmaxnreg can hand its registers to the consumers (a 64 x 256 fp32 accumulator is 128 registers per
+//   thread).  Persistent CTAs, 4-stage shared-memory ring; the producer fills the ring for the next tile while the
+//   consumers run the epilogue of the current one.
 #include <cuda_fp16.h>
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "common.h"
 #include "conv.h"
@@ -37,7 +41,11 @@ constexpr int B_BYTES_MAX = 256 * BK * 2;
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES_MAX;
 constexpr int RING_BYTES = STAGES * STAGE_BYTES;
 constexpr int CONSUMER_THREADS = 256;  // two warpgroups; wgmma needs warpgroups aligned to warp 0, 4, ...
-constexpr int THREADS = CONSUMER_THREADS + 32;
+constexpr int THREADS = CONSUMER_THREADS + 128;
+// Per-thread registers after setmaxnreg.  The launch gives every thread 65536 / 384 -> 168; the producer warpgroup
+// returns 128 each, which is exactly the 64 more each consumer takes.
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+static_assert(128 * PRODUCER_REGS + CONSUMER_THREADS * CONSUMER_REGS <= THREADS * 168, "conv: register budget");
 constexpr int HEAD_BYTES = kMaxHead * 256 * 4;
 constexpr int kMaxBias = 2048;   // bias of the whole layer staged in shared memory (Cout_pad <= kMaxBias)
 constexpr int kMaxRank1 = 1024;  // same for the rank-1 input column
@@ -192,8 +200,9 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
     tma_prefetch_desc(&maps.wgt);
     tma_prefetch_desc(&maps.act8);
     tma_prefetch_desc(&maps.wgt8);
-    // empty[]: one arrive per consumer warpgroup once its wgmma reading the stage have completed
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }
+    // empty[]: every consumer thread arrives once the wgmma reading the stage have completed (a release by one thread
+    // per warpgroup behind a branch puts the wgmma next to a divergent path, which makes ptxas serialize them)
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONSUMER_THREADS); }
     fence_barrier_init();
   }
   {  // bias (and the rank-1 column) of the whole layer: read once per CTA instead of once per tile from global memory
@@ -204,8 +213,9 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
   }
   __syncthreads();
 
-  if (warp == 8) {
-    if (lane == 0) {
+  if (warp >= 8) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x == CONSUMER_THREADS) {
       int stage = 0;
       uint32_t phase = 0;
       for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
@@ -233,6 +243,7 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
   }
 
   // ---------------------------------------------------------------- consumers: warpgroup wg owns pixels wg*64 .. +63
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = warp >> 2;
   const int qd = lane & 3;  // column pair within each 8-column block of the fragment
   if constexpr (HEAD) {  // stage the head weights once per CTA, zero padded
@@ -250,31 +261,36 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
   for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
     int b, y0, x0, n0, ks;
     tile_decode(u, p, b, y0, x0, n0, ks);
-    const int my_k = min(k_iters, (ks + 1) * p.k_per_split) - ks * p.k_per_split;
-    int prev_stage = -1;
-    for (int ki = 0; ki < my_k; ++ki) {
-      mbar_wait(&full[stage], phase);
-      const uint32_t a_addr = smem_u32(sA + stage * A_BYTES) + a_off;
-      const uint32_t b_addr = smem_u32(sB + stage * B_BYTES_MAX);
-      wgmma_fence();
-      if (ki >= k8) {
+    const int k_lo = ks * p.k_per_split;
+    const int my_k = min(k_iters, k_lo + p.k_per_split) - k_lo;
+    const int my_k8 = min(my_k, max(0, k8 - k_lo));  // the e4m3 k-iterations of this unit come first
+    // k-iterations [ki0, ki1), all of one operand kind.  The kind is a template argument so that no wgmma sits in a
+    // branch: ptxas then keeps one wgmma group in flight instead of draining each before the next.  A stage is
+    // released once wgmma_wait<1> shows the group that read it has completed.
+    auto k_loop = [&](auto f8, const int ki0, const int ki1) {
+      for (int ki = ki0; ki < ki1; ++ki) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t a_addr = smem_u32(sA + stage * A_BYTES) + a_off;
+        const uint32_t b_addr = smem_u32(sB + stage * B_BYTES_MAX);
+        wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          wgmma_f16<N>(d, wgmma_desc_sw128(a_addr + k * 32), wgmma_desc_sw128(b_addr + k * 32), (ki | k) != 0);
-      } else {  // e4m3 x e4m3: 128 channels of this tap in four K = 32 instructions over the same 128-byte rows
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          wgmma_e4m3<N>(d, wgmma_desc_sw128(a_addr + k * 32), wgmma_desc_sw128(b_addr + k * 32), (ki | k) != 0);
+        for (int k = 0; k < 4; ++k) {  // 32 bytes of the 128-byte rows each: fp16 K = 16, e4m3 K = 32
+          if constexpr (decltype(f8)::value)
+            wgmma_e4m3<N>(d, wgmma_desc_sw128(a_addr + k * 32), wgmma_desc_sw128(b_addr + k * 32), (ki | k) != 0);
+          else
+            wgmma_f16<N>(d, wgmma_desc_sw128(a_addr + k * 32), wgmma_desc_sw128(b_addr + k * 32), (ki | k) != 0);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (ki > 0) mbar_arrive(&empty[stage == 0 ? STAGES - 1 : stage - 1]);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      wgmma_commit();
-      wgmma_wait<1>();  // the previous k-iteration's group has finished reading its stage
-      if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev_stage]);
-      prev_stage = stage;
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-    }
+    };
+    k_loop(std::true_type{}, 0, my_k8);
+    k_loop(std::false_type{}, my_k8, my_k);
     wgmma_wait<0>();
     wgmma_fence_regs(d);
-    if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev_stage]);
+    mbar_arrive(&empty[stage == 0 ? STAGES - 1 : stage - 1]);  // the stage of the last k-iteration (my_k >= 1)
 
     // thread holds rows r_i = wg*64 + (warp%4)*16 + lane/4 + 8i, columns 8j + 2*qd + {0, 1}
     const float acc_scale = p.acc_scale;

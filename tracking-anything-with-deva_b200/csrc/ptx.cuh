@@ -161,6 +161,18 @@ __device__ __forceinline__ void wgmma_e4m3<256>(float (&d)[128], uint64_t a, uin
 }
 
 // ------------------------------------------------------------------- misc
+// Move registers between the warpgroups of a CTA: every thread of the executing warpgroup must run the same call.
+// `dec` returns registers to the CTA's pool; `inc` waits until the pool holds enough of them.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  static_assert(R >= 24 && R <= 256 && R % 8 == 0, "setmaxnreg: 24..256 registers in steps of 8");
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  static_assert(R >= 24 && R <= 256 && R % 8 == 0, "setmaxnreg: 24..256 registers in steps of 8");
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
