@@ -27,9 +27,10 @@
 extern "C" {
 #endif
 
-/* v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
+/* v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
+ * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 11
+#define DEVA_B200_ABI_VERSION 12
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 
@@ -281,6 +282,21 @@ DEVA_B200_API int deva_b200_transpose_append(const void* src, void* dst, int64_t
  * PCIe bytes).  Bit-exact with the torch ops (IEEE divisions in the same order). */
 DEVA_B200_API int deva_b200_ingest_rgb8(const uint8_t* src, float* dst, int h, int w, const float mean[3],
                                         const float std[3], deva_stream_t stream);
+/* Decoded frame u8 [h, w, 3] -> fp32 [3, out_h, out_w]: ToTensor + Normalize of every source pixel exactly as
+ * deva_b200_ingest_rgb8, then a separable resample - horizontal into scratch fp32 [3, h, out_w], then vertical - and an
+ * optional horizontal flip of the result.  Output pixel o of an axis is sum_{j < taps} w[o * taps + j] * in[idx[o * taps
+ * + j]] (fused multiply-adds in ascending j); the int32 idx / fp32 w tables of each axis come from the caller (the
+ * package builds them from torch's CPU bilinear and antialiased-bilinear arithmetic: video_reader.py:151's
+ * Resize(BILINEAR, antialias=True) and demo_utils.py:18's F.interpolate(mode='bilinear')). */
+DEVA_B200_API int deva_b200_ingest_rgb8_resize(const uint8_t* src, int h, int w, int out_h, int out_w,
+                                               const int32_t* x_idx, const float* x_w, int x_taps, const int32_t* y_idx,
+                                               const float* y_w, int y_taps, float* scratch, float* dst, int flip,
+                                               const float mean[3], const float std[3], deva_stream_t stream);
+/* Index mask u8 [h, w] -> int64 [out_h, out_w]: dst[y, x] = src[y_idx[y], x_idx[x']], x' = out_w - 1 - x when flip,
+ * else x.  With PIL's NEAREST index maps this is the reader's Resize(NEAREST) of a first-frame mask
+ * (video_reader.py:159-161), then eval_vos.py:162-164's flip. */
+DEVA_B200_API int deva_b200_mask_nearest(const uint8_t* src, int h, int w, int out_h, int out_w, const int32_t* x_idx,
+                                         const int32_t* y_idx, int flip, int64_t* dst, deva_stream_t stream);
 /* Driver post-step (evaluation/eval_vos.py:169-181) in one pass: optional bilinear resize (align_corners=False) of
  * prob fp32 [c, h, w] to [out_h, out_w], optional horizontal flip, argmax over channels (first maximum wins),
  * temporary-id -> object-id remap through lut int32 [c] (lut[0] = 0).  Writes out_u8 [out_h, out_w] and/or

@@ -246,6 +246,17 @@ DEVA_B200_API int deva_b200_ingest_rgb8(const uint8_t* src, float* dst, int h, i
                                         const float std[3], deva_stream_t stream) {
   return ew_ingest_rgb8(src, dst, h, w, mean, std, S(stream));
 }
+DEVA_B200_API int deva_b200_ingest_rgb8_resize(const uint8_t* src, int h, int w, int out_h, int out_w,
+                                               const int32_t* x_idx, const float* x_w, int x_taps, const int32_t* y_idx,
+                                               const float* y_w, int y_taps, float* scratch, float* dst, int flip,
+                                               const float mean[3], const float std[3], deva_stream_t stream) {
+  return ew_ingest_rgb8_resize(src, h, w, out_h, out_w, x_idx, x_w, x_taps, y_idx, y_w, y_taps, scratch, dst, flip, mean,
+                               std, S(stream));
+}
+DEVA_B200_API int deva_b200_mask_nearest(const uint8_t* src, int h, int w, int out_h, int out_w, const int32_t* x_idx,
+                                         const int32_t* y_idx, int flip, int64_t* dst, deva_stream_t stream) {
+  return ew_mask_nearest(src, h, w, out_h, out_w, x_idx, y_idx, flip, reinterpret_cast<long long*>(dst), S(stream));
+}
 DEVA_B200_API int deva_b200_prob_to_ids(const float* prob, int c, int h, int w, int out_h, int out_w, int flip,
                                         const int32_t* lut, uint8_t* out_u8, int64_t* out_i64, deva_stream_t stream) {
   return ew_prob_to_ids(prob, c, h, w, out_h, out_w, flip, lut, out_u8, reinterpret_cast<long long*>(out_i64), S(stream));

@@ -979,6 +979,64 @@ prob_to_ids_kernel(const float* __restrict__ prob, int c, int h, int w, int out_
   if (out_u8) out_u8[i] = (unsigned char)id;
   if (out_i64) out_i64[i] = id;
 }
+
+// Resized ingest, pass 1 (horizontal, the order torch's CPU separable resampler uses): u8 [h, w, 3] -> fp32 tmp
+// [3, h, out_w].  Every source tap is normalised exactly like ingest_rgb8_kernel (through a 256-entry table per channel,
+// same divisions), then tmp = sum_j x_w[ox, j] * v[y, x_idx[ox, j]] accumulated in ascending j with FMAs.
+__global__ void __launch_bounds__(256)
+resize_rows_rgb8_kernel(const unsigned char* __restrict__ src, int h, int w, int out_w, const int* __restrict__ x_idx,
+                        const float* __restrict__ x_w, int taps, float* __restrict__ tmp, float m0, float m1, float m2,
+                        float s0, float s1, float s2) {
+  __shared__ float norm[3][256];
+  for (int i = threadIdx.x; i < 768; i += 256) {
+    const int c = i >> 8;
+    const float m = c == 0 ? m0 : (c == 1 ? m1 : m2), sd = c == 0 ? s0 : (c == 1 ? s1 : s2);
+    norm[c][i & 255] = __fdiv_rn(__fdiv_rn((float)(i & 255), 255.f) - m, sd);
+  }
+  __syncthreads();
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= (long long)h * out_w) return;
+  const int y = (int)(i / out_w), ox = (int)(i - (long long)y * out_w);
+  const unsigned char* row = src + (long long)y * w * 3;
+  float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+  for (int j = 0; j < taps; ++j) {
+    const unsigned char* p = row + 3 * x_idx[ox * taps + j];
+    const float wt = x_w[ox * taps + j];
+    a0 = __fmaf_rn(norm[0][p[0]], wt, a0);
+    a1 = __fmaf_rn(norm[1][p[1]], wt, a1);
+    a2 = __fmaf_rn(norm[2][p[2]], wt, a2);
+  }
+  const long long plane = (long long)h * out_w;
+  tmp[i] = a0;
+  tmp[plane + i] = a1;
+  tmp[2 * plane + i] = a2;
+}
+
+// Resized ingest, pass 2 (vertical): tmp [3, h, out_w] -> dst [3, out_h, out_w], optionally flipped horizontally.
+__global__ void __launch_bounds__(256)
+resize_cols_kernel(const float* __restrict__ tmp, int h, int out_h, int out_w, const int* __restrict__ y_idx,
+                   const float* __restrict__ y_w, int taps, int flip, float* __restrict__ dst) {
+  const long long plane = (long long)out_h * out_w;
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= 3 * plane) return;
+  const int c = (int)(i / plane);
+  const long long r = i - c * plane;
+  const int oy = (int)(r / out_w), ox = (int)(r - (long long)oy * out_w);
+  const float* col = tmp + (long long)c * h * out_w + ox;
+  float a = 0.f;
+  for (int j = 0; j < taps; ++j) a = __fmaf_rn(col[(long long)y_idx[oy * taps + j] * out_w], y_w[oy * taps + j], a);
+  dst[c * plane + (long long)oy * out_w + (flip ? out_w - 1 - ox : ox)] = a;
+}
+
+// Index mask u8 [h, w] -> int64 [out_h, out_w] by row / column gather (nearest), optionally flipped after the resize.
+__global__ void __launch_bounds__(256)
+mask_gather_kernel(const unsigned char* __restrict__ src, int w, int out_h, int out_w, const int* __restrict__ x_idx,
+                   const int* __restrict__ y_idx, int flip, long long* __restrict__ dst) {
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= (long long)out_h * out_w) return;
+  const int oy = (int)(i / out_w), ox = (int)(i - (long long)oy * out_w);
+  dst[i] = src[(long long)y_idx[oy] * w + x_idx[flip ? out_w - 1 - ox : ox]];
+}
 }  // namespace ew
 
 int ew_ingest_rgb8(const unsigned char* src, float* dst, int h, int w, const float* mean, const float* stdv, cudaStream_t s) {
@@ -986,6 +1044,28 @@ int ew_ingest_rgb8(const unsigned char* src, float* dst, int h, int w, const flo
   const long long hw = (long long)h * w;
   ew::ingest_rgb8_kernel<<<(unsigned)ceil_div(hw, 256ll), 256, 0, s>>>(src, dst, hw, mean[0], mean[1], mean[2], stdv[0],
                                                                       stdv[1], stdv[2]);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+int ew_ingest_rgb8_resize(const unsigned char* src, int h, int w, int out_h, int out_w, const int* x_idx,
+                          const float* x_w, int x_taps, const int* y_idx, const float* y_w, int y_taps, float* tmp,
+                          float* dst, int flip, const float* mean, const float* stdv, cudaStream_t s) {
+  B200_REQUIRE(h > 0 && w > 0 && out_h > 0 && out_w > 0 && x_taps > 0 && y_taps > 0 && x_idx && x_w && y_idx && y_w &&
+               tmp && mean && stdv, "ingest_rgb8_resize: bad arguments");
+  const long long n1 = (long long)h * out_w, n2 = 3ll * out_h * out_w;
+  ew::resize_rows_rgb8_kernel<<<(unsigned)ceil_div(n1, 256ll), 256, 0, s>>>(src, h, w, out_w, x_idx, x_w, x_taps, tmp,
+                                                                            mean[0], mean[1], mean[2], stdv[0], stdv[1],
+                                                                            stdv[2]);
+  B200_LAUNCH_CHECK();
+  ew::resize_cols_kernel<<<(unsigned)ceil_div(n2, 256ll), 256, 0, s>>>(tmp, h, out_h, out_w, y_idx, y_w, y_taps, flip, dst);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+int ew_mask_nearest(const unsigned char* src, int h, int w, int out_h, int out_w, const int* x_idx, const int* y_idx,
+                    int flip, long long* dst, cudaStream_t s) {
+  B200_REQUIRE(h > 0 && w > 0 && out_h > 0 && out_w > 0 && x_idx && y_idx, "mask_nearest: bad arguments");
+  const long long n = (long long)out_h * out_w;
+  ew::mask_gather_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, s>>>(src, w, out_h, out_w, x_idx, y_idx, flip, dst);
   B200_LAUNCH_CHECK();
   return 0;
 }

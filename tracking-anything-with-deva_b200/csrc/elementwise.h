@@ -28,6 +28,11 @@ int ew_output_tail(const float* logits, float* agg, float* prob, float* logits_o
 int ew_head_gather3x3(const float* z, float* out, float bias, int B, int H, int W, cudaStream_t s);
 int ew_transpose_append(const __half* src, __half* dst, long long ld_dst, int n, int C, cudaStream_t s);
 int ew_ingest_rgb8(const unsigned char* src, float* dst, int h, int w, const float* mean, const float* stdv, cudaStream_t s);
+int ew_ingest_rgb8_resize(const unsigned char* src, int h, int w, int out_h, int out_w, const int* x_idx,
+                          const float* x_w, int x_taps, const int* y_idx, const float* y_w, int y_taps, float* tmp,
+                          float* dst, int flip, const float* mean, const float* stdv, cudaStream_t s);
+int ew_mask_nearest(const unsigned char* src, int h, int w, int out_h, int out_w, const int* x_idx, const int* y_idx,
+                    int flip, long long* dst, cudaStream_t s);
 int ew_prob_to_ids(const float* prob, int c, int h, int w, int out_h, int out_w, int flip, const int* lut,
                    unsigned char* out_u8, long long* out_i64, cudaStream_t s);
 }  // namespace b200

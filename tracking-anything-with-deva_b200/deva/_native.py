@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 11
+ABI_VERSION = 12
 LIST_PITCH = 32
 MAX_GROUPS = 256
 
@@ -94,6 +94,11 @@ _SIGNATURES = {
     'deva_b200_transpose_append': (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
     'deva_b200_ingest_rgb8': (c_int, [c_void_p, c_void_p, c_int, c_int, ctypes.POINTER(ctypes.c_float),
                                       ctypes.POINTER(ctypes.c_float), c_void_p]),
+    'deva_b200_ingest_rgb8_resize': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                             c_void_p, c_int, c_void_p, c_void_p, c_int, ctypes.POINTER(ctypes.c_float),
+                                             ctypes.POINTER(ctypes.c_float), c_void_p]),
+    'deva_b200_mask_nearest': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                       c_void_p]),
     'deva_b200_prob_to_ids': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                       c_void_p]),
 }
@@ -354,6 +359,19 @@ def ingest_rgb8(src, dst, h, w, mean, std):
     m = (ctypes.c_float * 3)(*[float(v) for v in mean])
     s = (ctypes.c_float * 3)(*[float(v) for v in std])
     _check(lib().deva_b200_ingest_rgb8(_ptr(src), _ptr(dst), h, w, m, s, _stream()), 'ingest_rgb8')
+
+
+def ingest_rgb8_resize(src, h, w, out_h, out_w, x_idx, x_w, y_idx, y_w, scratch, dst, flip, mean, std):
+    m = (ctypes.c_float * 3)(*[float(v) for v in mean])
+    s = (ctypes.c_float * 3)(*[float(v) for v in std])
+    _check(lib().deva_b200_ingest_rgb8_resize(_ptr(src), h, w, out_h, out_w, _ptr(x_idx), _ptr(_f32(x_w)), x_w.shape[1],
+                                              _ptr(y_idx), _ptr(_f32(y_w)), y_w.shape[1], _ptr(_f32(scratch)),
+                                              _ptr(_f32(dst)), int(flip), m, s, _stream()), 'ingest_rgb8_resize')
+
+
+def mask_nearest(src, h, w, out_h, out_w, x_idx, y_idx, flip, dst):
+    _check(lib().deva_b200_mask_nearest(_ptr(src), h, w, out_h, out_w, _ptr(x_idx), _ptr(y_idx), int(flip), _ptr(dst),
+                                        _stream()), 'mask_nearest')
 
 
 def prob_to_ids(prob, c, h, w, out_h, out_w, flip, lut, out_u8, out_i64):

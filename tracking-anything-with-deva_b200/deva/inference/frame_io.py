@@ -2,12 +2,18 @@
 real pipeline, each as one kernel.
 
 * ``frame_from_rgb8``: the decoded uint8 frame is uploaded as is (3 bytes / pixel instead of 12) and ToTensor +
-  Normalize (deva/inference/data/video_reader.py:146-150, IMAGENET mean/std) run on the device - bit-exact.
+  Normalize (deva/inference/data/video_reader.py:146-150, IMAGENET mean/std) run on the device - bit-exact.  With
+  ``size`` it also resizes to the working resolution the way the reference's drivers do, on the device: the readers'
+  ``Resize(size, BILINEAR, antialias=True)`` (video_reader.py:151, detection_video_reader.py:67-70) or demo_utils'
+  plain bilinear ``F.interpolate`` (demo_utils.py:10-19), optionally followed by eval_vos.py:162-164's flip.
+* ``mask_from_index8``: the first-frame / detection index mask through the readers' ``Resize(size, NEAREST)`` (PIL's
+  nearest, not torch's) and the same optional flip.
 * ``prob_to_ids``: the driver's post-step (evaluation/eval_vos.py:169-181) - bilinear resize to the original size,
   optional flip, argmax, ``ObjectManager.tmp_to_obj_cls`` - fused into a single pass that writes the id map.
 """
-from typing import Optional, Sequence, Tuple
+from typing import Dict, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from deva import _native as nat
@@ -16,16 +22,129 @@ IMAGENET_MEAN = (0.485, 0.456, 0.406)
 IMAGENET_STD = (0.229, 0.224, 0.225)
 
 
+def reader_size(h: int, w: int, size: int) -> Tuple[int, int]:
+    """Output (h, w) of torchvision's ``Resize(size)`` (the readers' convention): short side = size, long side =
+    int(size * long / short)."""
+    short, long = (w, h) if w <= h else (h, w)
+    new_short, new_long = size, int(size * long / short)
+    return (new_long, new_short) if w <= h else (new_short, new_long)
+
+
+def demo_size(h: int, w: int, size: int) -> Tuple[int, int]:
+    """Output (h, w) of demo_utils.get_input_frame_for_deva: scale = size / min(h, w), (int(h * scale), int(w * scale))."""
+    scale = size / min(h, w)
+    return int(h * scale), int(w * scale)
+
+
+def antialias_taps(n_in: int, n_out: int) -> Tuple[np.ndarray, np.ndarray]:
+    """int32 / float32 [n_out, taps] source indices and weights of torch's CPU ``_upsample_bilinear2d_aa`` along one
+    axis (align_corners=False): a triangle filter whose support is scaled by the downscale factor, weights normalised
+    per output pixel.  Float32 where torch's kernel keeps float, double where its expressions promote to double.
+    Unused taps have weight 0 and repeat the last index."""
+    f32, f64 = np.float32, np.float64
+    scale = f32(n_in) / f32(n_out)
+    support = scale if scale >= 1 else f32(1.0)
+    taps = int(np.ceil(support)) * 2 + 1
+    invscale = f32(1.0 / f64(scale)) if scale >= 1 else f32(1.0)
+    center = (f64(scale) * (np.arange(n_out, dtype=f64) + 0.5)).astype(f32)
+    xmin = np.maximum((f64(center - support) + 0.5).astype(np.int64), 0)
+    xsize = np.clip(np.minimum((f64(center + support) + 0.5).astype(np.int64), n_in) - xmin, 0, taps)
+    j = np.arange(taps)
+    x = np.abs(((f64((xmin[:, None] + j).astype(f32) - center[:, None]) + 0.5) * f64(invscale)).astype(f32))
+    wt = np.where(x < 1, f32(1) - x, f32(0)).astype(f32)
+    wt[j >= xsize[:, None]] = 0
+    total = np.zeros(n_out, f32)
+    for k in range(taps):  # torch sums the weights in tap order
+        total = total + wt[:, k]
+    wt = np.where(total[:, None] != 0, wt / np.where(total == 0, f32(1), total)[:, None], wt).astype(f32)
+    idx = np.minimum(xmin[:, None] + np.minimum(j, np.maximum(xsize[:, None] - 1, 0)), n_in - 1)
+    return idx.astype(np.int32), wt
+
+
+def bilinear_taps(n_in: int, n_out: int) -> Tuple[np.ndarray, np.ndarray]:
+    """int32 / float32 [n_out, 2] source indices and weights of torch's CPU ``upsample_bilinear2d``
+    (align_corners=False) along one axis.  The source coordinate scale * (o + 0.5) - 0.5 is one fused multiply-add in
+    float32, as torch's kernel computes it."""
+    f32, f64 = np.float32, np.float64
+    scale = f32(n_in) / f32(n_out)
+    real = np.maximum((f64(scale) * (np.arange(n_out) + 0.5) - 0.5).astype(f32), f32(0))
+    i0 = np.minimum(np.floor(real).astype(np.int64), n_in - 1)
+    lam = np.clip(real - i0.astype(f32), f32(0), f32(1)).astype(f32)
+    i1 = i0 + (i0 < n_in - 1)
+    return np.stack([i0, i1], 1).astype(np.int32), np.stack([f32(1) - lam, lam], 1)
+
+
+def pil_nearest_map(n_in: int, n_out: int) -> np.ndarray:
+    """int32 [n_out] source index of PIL's NEAREST resize along one axis: PIL steps a double coordinate from
+    0.5 * n_in / n_out by n_in / n_out and truncates it (ImagingScaleAffine), which is not torch's 'nearest'."""
+    a = n_in / n_out
+    out, xo = np.empty(n_out, np.int32), a * 0.5
+    for o in range(n_out):
+        out[o] = min(int(xo), n_in - 1)
+        xo += a
+    return out
+
+
+_TABLES: Dict[tuple, Tuple[torch.Tensor, ...]] = {}
+
+
+def _axis_table(kind: str, n_in: int, n_out: int, device) -> Tuple[torch.Tensor, ...]:
+    """Device copy of one axis' resampling table, built on the host once per (kind, n_in, n_out, device)."""
+    key = (kind, n_in, n_out, torch.device(device))
+    if key not in _TABLES:
+        if kind == 'nearest':
+            arrays = (pil_nearest_map(n_in, n_out),)
+        else:
+            arrays = (antialias_taps if kind == 'antialias' else bilinear_taps)(n_in, n_out)
+        _TABLES[key] = tuple(torch.from_numpy(a).to(device) for a in arrays)
+    return _TABLES[key]
+
+
+def _to_device(t: torch.Tensor, device) -> torch.Tensor:
+    if not t.is_cuda:
+        t = t.to(device or torch.device('cuda', torch.cuda.current_device()), non_blocking=True)
+    return t.contiguous()
+
+
 def frame_from_rgb8(frame: torch.Tensor, mean: Sequence[float] = IMAGENET_MEAN, std: Sequence[float] = IMAGENET_STD,
-                    device: Optional[torch.device] = None) -> torch.Tensor:
-    """uint8 [H, W, 3] RGB (host - ideally pinned - or device) -> normalised float32 [3, H, W] on the device."""
+                    device: Optional[torch.device] = None, *, size: Optional[int] = None, resize: str = 'reader',
+                    flip: bool = False) -> torch.Tensor:
+    """uint8 [H, W, 3] RGB (host - ideally pinned - or device) -> normalised float32 [3, H', W'] on the device.
+
+    ``size`` (None: keep H, W) is the working resolution's short side.  ``resize='reader'`` sizes the output like
+    torchvision's ``Resize(size)`` and filters like the readers (antialiased bilinear); ``resize='demo'`` sizes and
+    filters like demo_utils (plain bilinear).  ``flip`` mirrors the resized frame horizontally.  An output the size of
+    the input is the plain normalised frame, bit for bit, as the reference's resize returns its input unchanged."""
     assert frame.dtype == torch.uint8 and frame.dim() == 3 and frame.shape[2] == 3
-    if not frame.is_cuda:
-        frame = frame.to(device or torch.device('cuda', torch.cuda.current_device()), non_blocking=True)
-    frame = frame.contiguous()
+    assert resize in ('reader', 'demo'), resize
+    assert size is None or size > 0, size
+    frame = _to_device(frame, device)
     h, w = frame.shape[:2]
-    out = torch.empty(3, h, w, dtype=torch.float32, device=frame.device)
-    nat.ingest_rgb8(frame, out, h, w, mean, std)
+    oh, ow = (h, w) if size is None else (reader_size if resize == 'reader' else demo_size)(h, w, size)
+    out = torch.empty(3, oh, ow, dtype=torch.float32, device=frame.device)
+    if (oh, ow) == (h, w) and not flip:
+        nat.ingest_rgb8(frame, out, h, w, mean, std)
+        return out
+    kind = 'antialias' if resize == 'reader' else 'bilinear'
+    x_idx, x_w = _axis_table(kind, w, ow, frame.device)
+    y_idx, y_w = _axis_table(kind, h, oh, frame.device)
+    scratch = torch.empty(3, h, ow, dtype=torch.float32, device=frame.device)
+    nat.ingest_rgb8_resize(frame, h, w, oh, ow, x_idx, x_w, y_idx, y_w, scratch, out, flip, mean, std)
+    return out
+
+
+def mask_from_index8(mask: torch.Tensor, size: Optional[int] = None, *, flip: bool = False,
+                     device: Optional[torch.device] = None) -> torch.Tensor:
+    """uint8 [H, W] index mask (host or device) -> int64 [H', W'] on the device: the readers' ``Resize(size, NEAREST)``
+    on the PIL mask (output size as torchvision's ``Resize(size)``), then an optional horizontal flip."""
+    assert mask.dtype == torch.uint8 and mask.dim() == 2
+    assert size is None or size > 0, size
+    mask = _to_device(mask, device)
+    h, w = mask.shape
+    oh, ow = (h, w) if size is None else reader_size(h, w, size)
+    (x_idx,), (y_idx,) = _axis_table('nearest', w, ow, mask.device), _axis_table('nearest', h, oh, mask.device)
+    out = torch.empty(oh, ow, dtype=torch.long, device=mask.device)
+    nat.mask_nearest(mask, h, w, oh, ow, x_idx, y_idx, flip, out)
     return out
 
 
