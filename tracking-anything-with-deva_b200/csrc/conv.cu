@@ -331,58 +331,68 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
         float hacc[kMaxHead];
 #pragma unroll
         for (int t = 0; t < kMaxHead; ++t) hacc[t] = 0.f;
-        if (live) {
-#pragma unroll
-          for (int j = 0; j < N / 8; ++j) {
-            const int col = 8 * j + 2 * qd;
-            const int ch = n0 + col;
-            if (col >= p.nt || ch >= p.cout) continue;
-            float v0 = d[4 * j + 2 * i] * acc_scale, v1 = d[4 * j + 2 * i + 1] * acc_scale;  // acc_scale: fp8 mode
-            if (even) {  // both channels exist (cout even, ch even): 4-byte fp16 pairs, 8-byte fp32 pairs
-              if (ks == 0) { v0 += s_bias[ch]; v1 += s_bias[ch + 1]; }
-              if (p.rank1_w) { v0 = fmaf(s_r1w[ch], r1x, v0); v1 = fmaf(s_r1w[ch + 1], r1x, v1); }
-              if (res) {
-                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res + col));
-                v0 += f.x; v1 += f.y;
-              }
-              if (res_lo) {
-                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res_lo + col));
-                v0 += f.x; v1 += f.y;
-              }
-              const long long e = off + col;
-              if (p.out_raw) {
-                const __half2 h = __floats2half2_rn(v0, v1);
-                *reinterpret_cast<__half2*>(p.out_raw + e) = h;
-                if (p.out_raw_lo) {
-                  const float2 back = __half22float2(h);
-                  *reinterpret_cast<__half2*>(p.out_raw_lo + e) = __floats2half2_rn(v0 - back.x, v1 - back.y);
-                }
-              }
-              if (p.out_relu) {
-                const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
-                const __half2 h = __floats2half2_rn(a0, a1);
-                *reinterpret_cast<__half2*>(p.out_relu + e) = h;
-                if (p.out_relu_lo) {
-                  const float2 back = __half22float2(h);
-                  *reinterpret_cast<__half2*>(p.out_relu_lo + e) = __floats2half2_rn(a0 - back.x, a1 - back.y);
-                }
-              }
-              if (p.out_relu_lo8)
-                *reinterpret_cast<uint16_t*>(p.out_relu_lo8 + e) = to_e4m3x2(lo8_value(v0), lo8_value(v1));
-              if (p.out_f32)
-                *reinterpret_cast<float2*>(p.out_f32 + ks * p.f32_split_stride + e) = make_float2(v0, v1);
-            } else {  // ragged channel count (e.g. Cout = 1, 129): element by element
-              v0 = finish_scalar(p, v0, ch, off + col, res, res_lo, col, r1x, ks);
-              if (ch + 1 < p.cout) v1 = finish_scalar(p, v1, ch + 1, off + col + 1, res, res_lo, col + 1, r1x, ks);
+        // One column pair (8j + 2qd, +1) of row i.  `full`: the tile spans N existing channels of an even Cout, so the
+        // per-column bounds check and the element-by-element path drop out of the unrolled loop at compile time.
+        auto pair = [&](auto full_t, const int j) {
+          constexpr bool full = decltype(full_t)::value;
+          const int col = 8 * j + 2 * qd;
+          const int ch = n0 + col;
+          if (!full && (col >= p.nt || ch >= p.cout)) return;
+          float v0 = d[4 * j + 2 * i] * acc_scale, v1 = d[4 * j + 2 * i + 1] * acc_scale;  // acc_scale: fp8 mode
+          if (full || even) {  // both channels exist (cout even, ch even): 4-byte fp16 pairs, 8-byte fp32 pairs
+            if (ks == 0) { v0 += s_bias[ch]; v1 += s_bias[ch + 1]; }
+            if (p.rank1_w) { v0 = fmaf(s_r1w[ch], r1x, v0); v1 = fmaf(s_r1w[ch + 1], r1x, v1); }
+            if (res) {
+              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res + col));
+              v0 += f.x; v1 += f.y;
             }
-            if constexpr (HEAD) {  // logit head: 9 taps over the ReLU'd channels, fp32, weights from shared memory
+            if (res_lo) {
+              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res_lo + col));
+              v0 += f.x; v1 += f.y;
+            }
+            const long long e = off + col;
+            if (p.out_raw) {
+              const __half2 h = __floats2half2_rn(v0, v1);
+              *reinterpret_cast<__half2*>(p.out_raw + e) = h;
+              if (p.out_raw_lo) {
+                const float2 back = __half22float2(h);
+                *reinterpret_cast<__half2*>(p.out_raw_lo + e) = __floats2half2_rn(v0 - back.x, v1 - back.y);
+              }
+            }
+            if (p.out_relu) {
               const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
-#pragma unroll
-              for (int t = 0; t < kMaxHead; ++t) {
-                const float2 w2 = *reinterpret_cast<const float2*>(s_head + t * 256 + col);
-                hacc[t] = fmaf(a0, w2.x, fmaf(a1, w2.y, hacc[t]));
+              const __half2 h = __floats2half2_rn(a0, a1);
+              *reinterpret_cast<__half2*>(p.out_relu + e) = h;
+              if (p.out_relu_lo) {
+                const float2 back = __half22float2(h);
+                *reinterpret_cast<__half2*>(p.out_relu_lo + e) = __floats2half2_rn(a0 - back.x, a1 - back.y);
               }
             }
+            if (p.out_relu_lo8)
+              *reinterpret_cast<uint16_t*>(p.out_relu_lo8 + e) = to_e4m3x2(lo8_value(v0), lo8_value(v1));
+            if (p.out_f32)
+              *reinterpret_cast<float2*>(p.out_f32 + ks * p.f32_split_stride + e) = make_float2(v0, v1);
+          } else {  // ragged channel count (e.g. Cout = 1, 129): element by element
+            v0 = finish_scalar(p, v0, ch, off + col, res, res_lo, col, r1x, ks);
+            if (ch + 1 < p.cout) v1 = finish_scalar(p, v1, ch + 1, off + col + 1, res, res_lo, col + 1, r1x, ks);
+          }
+          if constexpr (HEAD) {  // logit head: 9 taps over the ReLU'd channels, fp32, weights from shared memory
+            const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
+#pragma unroll
+            for (int t = 0; t < kMaxHead; ++t) {
+              const float2 w2 = *reinterpret_cast<const float2*>(s_head + t * 256 + col);
+              hacc[t] = fmaf(a0, w2.x, fmaf(a1, w2.y, hacc[t]));
+            }
+          }
+        };
+        if (live) {
+          // (not with the fused head: its nine running sums leave no registers for a second copy of the loop)
+          if (!HEAD && even && p.nt == N && n0 + N <= p.cout) {  // every tile of the wide layers
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) pair(std::integral_constant<bool, !HEAD>{}, j);
+          } else {
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) pair(std::false_type{}, j);
           }
         }
         if constexpr (HEAD) {  // the four threads of a quad hold the same pixel's partial sums over disjoint channels
