@@ -27,12 +27,14 @@
 extern "C" {
 #endif
 
-/* v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
+/* v13: deva_b200_prob_to_segments (the result savers' id map, id image, overlay, areas and boxes in one pass).
+ * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 12
+#define DEVA_B200_ABI_VERSION 13
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
+#define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
 
 typedef void* deva_stream_t; /* cudaStream_t */
 
@@ -303,6 +305,22 @@ DEVA_B200_API int deva_b200_mask_nearest(const uint8_t* src, int h, int w, int o
  * out_i64 [out_h, out_w] (either may be NULL). */
 DEVA_B200_API int deva_b200_prob_to_ids(const float* prob, int c, int h, int w, int out_h, int out_w, int flip,
                                         const int32_t* lut, uint8_t* out_u8, int64_t* out_i64, deva_stream_t stream);
+/* Result-saver egress (deva/inference/result_utils.py:98-102 and the per-frame work of save_result, :158-257) in one
+ * pass: the resize and argmax of deva_b200_prob_to_ids without flip (its id map, bit for bit), then per output pixel of
+ * argmax channel k, each output optional (NULL = not written):
+ *  - out_u8 [out_h, out_w] = (uint8)lut[k]: the remapped index mask (:159-163, :217);
+ *  - out_rgb [out_h, out_w, 3] = bytes (v & 255, v >> 8 & 255, v >> 16 & 255) of v = rgb[k]: the long-id RGB image
+ *    (:208-215; the caller packs ID2RGBConverter._id_to_rgb(id) for the ids it colours, 0 for the others);
+ *  - out_overlay [out_h, out_w, 3] = frame where lut[k] == 0, else (frame + id image) >> 1: the visualisation blend
+ *    (:240-242; frame u8 [out_h, out_w, 3]);
+ *  - counts int64 [c] (pixels per channel) and boxes int32 [c, 4] (x_min, y_min, x_max, y_max; (INT32_MAX, INT32_MAX,
+ *    -1, -1) for an empty channel), written together: the segment areas (:166-171, :198-204) and masks_to_boxes
+ *    (:244-257).  The call initialises them.
+ * lut int32 [c] is required; rgb uint32 [c] with out_rgb or out_overlay.  c <= DEVA_B200_MAX_SEGMENT_CHANNELS. */
+DEVA_B200_API int deva_b200_prob_to_segments(const float* prob, int c, int h, int w, int out_h, int out_w,
+                                             const int32_t* lut, const uint32_t* rgb, const uint8_t* frame,
+                                             uint8_t* out_u8, uint8_t* out_rgb, uint8_t* out_overlay, int64_t* counts,
+                                             int32_t* boxes, deva_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -261,5 +261,13 @@ DEVA_B200_API int deva_b200_prob_to_ids(const float* prob, int c, int h, int w, 
                                         const int32_t* lut, uint8_t* out_u8, int64_t* out_i64, deva_stream_t stream) {
   return ew_prob_to_ids(prob, c, h, w, out_h, out_w, flip, lut, out_u8, reinterpret_cast<long long*>(out_i64), S(stream));
 }
+static_assert(DEVA_B200_MAX_SEGMENT_CHANNELS == kMaxSegmentChannels, "header and kernel disagree on the channel limit");
+DEVA_B200_API int deva_b200_prob_to_segments(const float* prob, int c, int h, int w, int out_h, int out_w,
+                                             const int32_t* lut, const uint32_t* rgb, const uint8_t* frame,
+                                             uint8_t* out_u8, uint8_t* out_rgb, uint8_t* out_overlay, int64_t* counts,
+                                             int32_t* boxes, deva_stream_t stream) {
+  return ew_prob_to_segments(prob, c, h, w, out_h, out_w, lut, rgb, frame, out_u8, out_rgb, out_overlay,
+                             reinterpret_cast<unsigned long long*>(counts), boxes, S(stream));
+}
 
 }  // extern "C"

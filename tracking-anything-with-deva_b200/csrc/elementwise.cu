@@ -3,6 +3,8 @@
 // non-standard sensory GRU (modules.py:145-149), and the soft-aggregation / x4 upsampling / softmax tail
 // (network.py:33-40,144-168).  One thread per output element (or per pixel x channel-vector); all accesses
 // are coalesced along the channel axis.
+#include <algorithm>
+#include <climits>
 #include <cuda_fp16.h>
 #include <math_constants.h>
 #include <stdint.h>
@@ -942,16 +944,11 @@ ingest_rgb8_kernel(const unsigned char* __restrict__ src, float* __restrict__ ds
   dst[2 * hw + i] = __fdiv_rn(__fdiv_rn((float)p[2], 255.f) - m2, s2);
 }
 
-// prob [c, h, w] -> ids [out_h, out_w]: bilinear (align_corners = False, PyTorch's upsample_bilinear2d arithmetic),
-// flip, argmax (first maximum), id remap.  One thread per output pixel, channels streamed.
-__global__ void __launch_bounds__(256)
-prob_to_ids_kernel(const float* __restrict__ prob, int c, int h, int w, int out_h, int out_w, int flip, float rh,
-                   float rw, const int* __restrict__ lut, unsigned char* __restrict__ out_u8,
-                   long long* __restrict__ out_i64) {
-  const long long i = blockIdx.x * 256ll + threadIdx.x;
-  if (i >= (long long)out_h * out_w) return;
-  const int oy = (int)(i / out_w), ox_out = (int)(i - (long long)oy * out_w);
-  const int ox = flip ? out_w - 1 - ox_out : ox_out;  // flip acts on the resized map
+// Channel of the first maximum of prob [c, h, w] bilinearly resized (align_corners = False, PyTorch's
+// upsample_bilinear2d arithmetic) to [out_h, out_w], at output pixel (oy, ox); channels streamed.  Every egress kernel
+// goes through this one function, so their id maps agree bit for bit.
+__device__ __forceinline__ int resized_argmax(const float* __restrict__ prob, int c, int h, int w, int out_h, int out_w,
+                                              float rh, float rw, int oy, int ox) {
   int best = 0;
   float best_v;
   const long long plane = (long long)h * w;
@@ -975,9 +972,103 @@ prob_to_ids_kernel(const float* __restrict__ prob, int c, int h, int w, int out_
       if (v > best_v) { best_v = v; best = k; }
     }
   }
+  return best;
+}
+
+// prob [c, h, w] -> ids [out_h, out_w]: bilinear resize, flip, argmax (first maximum), id remap.  One thread per output
+// pixel.
+__global__ void __launch_bounds__(256)
+prob_to_ids_kernel(const float* __restrict__ prob, int c, int h, int w, int out_h, int out_w, int flip, float rh,
+                   float rw, const int* __restrict__ lut, unsigned char* __restrict__ out_u8,
+                   long long* __restrict__ out_i64) {
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= (long long)out_h * out_w) return;
+  const int oy = (int)(i / out_w), ox_out = (int)(i - (long long)oy * out_w);
+  const int ox = flip ? out_w - 1 - ox_out : ox_out;  // flip acts on the resized map
+  const int best = resized_argmax(prob, c, h, w, out_h, out_w, rh, rw, oy, ox);
   const int id = lut ? lut[best] : best;
   if (out_u8) out_u8[i] = (unsigned char)id;
   if (out_i64) out_i64[i] = id;
+}
+
+// Result-saver egress: the same argmax as prob_to_ids_kernel, then per output pixel (each output optional)
+//   index u8 = (uint8)lut[k]; id image = bytes of rgb[k] (id % 256, id / 256 % 256, id / 65536, or 0 when the id is not
+//   coloured); overlay = frame where lut[k] == 0, else (frame + id image) >> 1.
+// The overlay is the reference's float32 blend image * a + rgb * (1 - a), a = 1 where the id is 0 and 0.5 elsewhere,
+// truncated to uint8: with a = 1 it is image * 1 + rgb * 0 = image; with a = 0.5 both halves of 8-bit integers and
+// their sum are exact in float32, so the blend is (image + rgb) / 2 exactly and truncation is the floor.
+// Per channel k, counts[k] (pixels whose argmax is k) and boxes[k] = (x_min, y_min, x_max, y_max) accumulate in shared
+// memory (5 ints per channel) over a grid-stride loop, then merge into global memory with atomics.
+__global__ void __launch_bounds__(256)
+prob_to_segments_kernel(const float* __restrict__ prob, int c, int h, int w, int out_h, int out_w, float rh, float rw,
+                        const int* __restrict__ lut, const unsigned* __restrict__ rgb,
+                        const unsigned char* __restrict__ frame, unsigned char* __restrict__ out_u8,
+                        unsigned char* __restrict__ out_rgb, unsigned char* __restrict__ out_overlay,
+                        unsigned long long* __restrict__ counts, int* __restrict__ boxes) {
+  extern __shared__ int stats[];  // [5][c]: count, x_min, y_min, x_max, y_max
+  const bool with_stats = counts != nullptr;
+  if (with_stats) {
+    for (int k = threadIdx.x; k < c; k += 256) {
+      stats[k] = 0;
+      stats[c + k] = INT_MAX;
+      stats[2 * c + k] = INT_MAX;
+      stats[3 * c + k] = -1;
+      stats[4 * c + k] = -1;
+    }
+    __syncthreads();
+  }
+  const long long n = (long long)out_h * out_w;
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+    const int oy = (int)(i / out_w), ox = (int)(i - (long long)oy * out_w);
+    const int k = resized_argmax(prob, c, h, w, out_h, out_w, rh, rw, oy, ox);
+    if (out_u8) out_u8[i] = (unsigned char)lut[k];
+    if (out_rgb || out_overlay) {
+      const unsigned v = rgb[k];
+      const unsigned char r = v & 255u, g = (v >> 8) & 255u, b = (v >> 16) & 255u;
+      if (out_rgb) {
+        out_rgb[3 * i] = r;
+        out_rgb[3 * i + 1] = g;
+        out_rgb[3 * i + 2] = b;
+      }
+      if (out_overlay) {
+        const unsigned char* f = frame + 3 * i;
+        const bool keep = lut[k] == 0;
+        out_overlay[3 * i] = keep ? f[0] : (unsigned char)((f[0] + r) >> 1);
+        out_overlay[3 * i + 1] = keep ? f[1] : (unsigned char)((f[1] + g) >> 1);
+        out_overlay[3 * i + 2] = keep ? f[2] : (unsigned char)((f[2] + b) >> 1);
+      }
+    }
+    if (with_stats) {
+      atomicAdd(&stats[k], 1);
+      atomicMin(&stats[c + k], ox);
+      atomicMin(&stats[2 * c + k], oy);
+      atomicMax(&stats[3 * c + k], ox);
+      atomicMax(&stats[4 * c + k], oy);
+    }
+  }
+  if (with_stats) {
+    __syncthreads();
+    for (int k = threadIdx.x; k < c; k += 256) {
+      if (stats[k] == 0) continue;
+      atomicAdd(&counts[k], (unsigned long long)stats[k]);
+      atomicMin(&boxes[4 * k], stats[c + k]);
+      atomicMin(&boxes[4 * k + 1], stats[2 * c + k]);
+      atomicMax(&boxes[4 * k + 2], stats[3 * c + k]);
+      atomicMax(&boxes[4 * k + 3], stats[4 * c + k]);
+    }
+  }
+}
+
+// counts = 0, boxes = (INT_MAX, INT_MAX, -1, -1): what an empty channel reports.
+__global__ void __launch_bounds__(256)
+segments_init_kernel(int c, unsigned long long* __restrict__ counts, int* __restrict__ boxes) {
+  const int k = blockIdx.x * 256 + threadIdx.x;
+  if (k >= c) return;
+  counts[k] = 0;
+  boxes[4 * k] = INT_MAX;
+  boxes[4 * k + 1] = INT_MAX;
+  boxes[4 * k + 2] = -1;
+  boxes[4 * k + 3] = -1;
 }
 
 // Resized ingest, pass 1 (horizontal, the order torch's CPU separable resampler uses): u8 [h, w, 3] -> fp32 tmp
@@ -1075,6 +1166,31 @@ int ew_prob_to_ids(const float* prob, int c, int h, int w, int out_h, int out_w,
   const long long n = (long long)out_h * out_w;
   ew::prob_to_ids_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, s>>>(prob, c, h, w, out_h, out_w, flip, (float)h / out_h,
                                                                      (float)w / out_w, lut, out_u8, out_i64);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+int ew_prob_to_segments(const float* prob, int c, int h, int w, int out_h, int out_w, const int* lut,
+                        const unsigned* rgb, const unsigned char* frame, unsigned char* out_u8, unsigned char* out_rgb,
+                        unsigned char* out_overlay, unsigned long long* counts, int* boxes, cudaStream_t s) {
+  B200_REQUIRE(c >= 1 && h > 0 && w > 0 && out_h > 0 && out_w > 0 && lut, "prob_to_segments: bad arguments");
+  B200_REQUIRE(c <= kMaxSegmentChannels, "prob_to_segments: %d channels, at most %d supported", c,
+               kMaxSegmentChannels);
+  B200_REQUIRE((!out_rgb && !out_overlay) || rgb, "prob_to_segments: the id image and overlay need the rgb table");
+  B200_REQUIRE(!out_overlay || frame, "prob_to_segments: the overlay needs the frame");
+  B200_REQUIRE(!counts == !boxes, "prob_to_segments: counts and boxes are written together");
+  const long long n = (long long)out_h * out_w;
+  long long blocks = (n + 255) / 256;
+  size_t smem = 0;
+  if (counts) {
+    smem = 5ull * c * sizeof(int);
+    blocks = std::min(blocks, 4ll * sm_count());  // fewer, longer-lived blocks amortise the per-block histogram
+    B200_CUDA(cudaFuncSetAttribute(ew::prob_to_segments_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    ew::segments_init_kernel<<<(unsigned)ceil_div(c, 256), 256, 0, s>>>(c, counts, boxes);
+    B200_LAUNCH_CHECK();
+  }
+  ew::prob_to_segments_kernel<<<(unsigned)blocks, 256, smem, s>>>(prob, c, h, w, out_h, out_w, (float)h / out_h,
+                                                                   (float)w / out_w, lut, rgb, frame, out_u8, out_rgb,
+                                                                   out_overlay, counts, boxes);
   B200_LAUNCH_CHECK();
   return 0;
 }

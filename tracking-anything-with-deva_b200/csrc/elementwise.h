@@ -35,4 +35,8 @@ int ew_mask_nearest(const unsigned char* src, int h, int w, int out_h, int out_w
                     int flip, long long* dst, cudaStream_t s);
 int ew_prob_to_ids(const float* prob, int c, int h, int w, int out_h, int out_w, int flip, const int* lut,
                    unsigned char* out_u8, long long* out_i64, cudaStream_t s);
+constexpr int kMaxSegmentChannels = 8192;  // prob_to_segments' shared-memory histogram: 20 bytes per channel
+int ew_prob_to_segments(const float* prob, int c, int h, int w, int out_h, int out_w, const int* lut,
+                        const unsigned* rgb, const unsigned char* frame, unsigned char* out_u8, unsigned char* out_rgb,
+                        unsigned char* out_overlay, unsigned long long* counts, int* boxes, cudaStream_t s);
 }  // namespace b200

@@ -12,9 +12,10 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 12
+ABI_VERSION = 13
 LIST_PITCH = 32
 MAX_GROUPS = 256
+MAX_SEGMENT_CHANNELS = 8192
 
 _lib = None
 
@@ -101,6 +102,8 @@ _SIGNATURES = {
                                        c_void_p]),
     'deva_b200_prob_to_ids': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                       c_void_p]),
+    'deva_b200_prob_to_segments': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -377,6 +380,12 @@ def mask_nearest(src, h, w, out_h, out_w, x_idx, y_idx, flip, dst):
 def prob_to_ids(prob, c, h, w, out_h, out_w, flip, lut, out_u8, out_i64):
     _check(lib().deva_b200_prob_to_ids(_ptr(prob), c, h, w, out_h, out_w, int(flip), _p(lut), _p(out_u8), _p(out_i64),
                                        _stream()), 'prob_to_ids')
+
+
+def prob_to_segments(prob, c, h, w, out_h, out_w, lut, rgb, frame, out_u8, out_rgb, out_overlay, counts, boxes):
+    _check(lib().deva_b200_prob_to_segments(_ptr(prob), c, h, w, out_h, out_w, _ptr(lut), _p(rgb), _p(frame), _p(out_u8),
+                                            _p(out_rgb), _p(out_overlay), _p(counts), _p(boxes), _stream()),
+           'prob_to_segments')
 
 
 def transpose_append(src, dst, ld_dst, n, c):

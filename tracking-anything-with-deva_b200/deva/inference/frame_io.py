@@ -10,8 +10,11 @@ real pipeline, each as one kernel.
   nearest, not torch's) and the same optional flip.
 * ``prob_to_ids``: the driver's post-step (evaluation/eval_vos.py:169-181) - bilinear resize to the original size,
   optional flip, argmax, ``ObjectManager.tmp_to_obj_cls`` - fused into a single pass that writes the id map.
+* ``prob_to_segments``: the same resize and argmax plus everything the result savers derive from the id map (index
+  mask, long-id RGB image, visualisation overlay, per-segment areas and boxes), in one pass.
 """
-from typing import Dict, Optional, Sequence, Tuple
+from dataclasses import dataclass
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -148,13 +151,32 @@ def mask_from_index8(mask: torch.Tensor, size: Optional[int] = None, *, flip: bo
     return out
 
 
-def id_lut(object_manager, channels: int, device) -> torch.Tensor:
-    """int32 [channels]: temporary id (prob channel) -> object id; channel 0 and unknown channels -> 0."""
+def _lut_list(object_manager, channels: int) -> List[int]:
     lut = [0] * channels
     for tmp_id, obj in object_manager.tmp_id_to_obj.items():
         if 0 < tmp_id < channels:
             lut[tmp_id] = int(obj.id)
-    return torch.tensor(lut, dtype=torch.int32, device=device)
+    return lut
+
+
+def id_lut(object_manager, channels: int, device) -> torch.Tensor:
+    """int32 [channels]: temporary id (prob channel) -> object id; channel 0 and unknown channels -> 0."""
+    return torch.tensor(_lut_list(object_manager, channels), dtype=torch.int32, device=device)
+
+
+def id_rgb(i: int) -> int:
+    """ID2RGBConverter._id_to_rgb(i) (deva/utils/pano_utils.py) packed as r | g << 8 | b << 16: the bytes i % 256,
+    i // 256 % 256, i // 65536 % 256."""
+    return (i % 256) | (i // 256 % 256) << 8 | (i // 65536 % 256) << 16
+
+
+def segment_tables(object_manager, channels: int, remap: bool = True) -> Tuple[List[int], List[int]]:
+    """Host tables of ``prob_to_segments``: ``lut`` [channels], the value written for each channel (its object id,
+    or the channel itself when ``remap`` is False), and ``rgb`` [channels], the packed colour of that value when it
+    is the id of a current object, else 0 (the saver colours only ``all_obj_ids``, result_utils.py:208-215)."""
+    lut = _lut_list(object_manager, channels) if remap else list(range(channels))
+    coloured = {int(o.id) for o in object_manager.obj_to_tmp_id}
+    return lut, [id_rgb(v) if v in coloured else 0 for v in lut]
 
 
 def prob_to_ids(prob: torch.Tensor, object_manager=None, size: Optional[Tuple[int, int]] = None, flip: bool = False,
@@ -171,4 +193,51 @@ def prob_to_ids(prob: torch.Tensor, object_manager=None, size: Optional[Tuple[in
     out = torch.empty(oh, ow, dtype=dtype, device=prob.device)
     nat.prob_to_ids(prob, c, h, w, oh, ow, flip, lut, out if dtype == torch.uint8 else None,
                     out if dtype == torch.long else None)
+    return out
+
+
+@dataclass
+class Segments:
+    """Result of ``prob_to_segments``.  Device tensors, each None unless requested; ``lut`` is the host table the
+    call used (channel -> value in ``index``), so per-channel ``counts`` / ``boxes`` can be grouped by id."""
+    lut: List[int]
+    index: Optional[torch.Tensor] = None  # uint8 [H0, W0]: (uint8) lut[argmax]
+    rgb: Optional[torch.Tensor] = None  # uint8 [H0, W0, 3]: long-id colour image
+    overlay: Optional[torch.Tensor] = None  # uint8 [H0, W0, 3]: frame blended with ``rgb``
+    counts: Optional[torch.Tensor] = None  # int64 [K+1]: pixels per channel
+    boxes: Optional[torch.Tensor] = None  # int32 [K+1, 4]: x_min, y_min, x_max, y_max per channel
+
+
+def prob_to_segments(prob: torch.Tensor, object_manager, size: Optional[Tuple[int, int]] = None, *, index: bool = True,
+                     rgb: bool = False, frame: Optional[torch.Tensor] = None, stats: bool = False,
+                     remap: bool = True) -> Segments:
+    """prob float32 [K+1, H, W] from ``step`` -> the result savers' per-frame outputs at ``size`` (or H, W), one pass.
+
+    The argmax is ``prob_to_ids``' (its id map, bit for bit, without flip).  ``index``: the uint8 id mask (ids above
+    255 wrap, like the saver's ``astype(np.uint8)``).  ``rgb``: the long-id RGB image.  ``frame`` (device uint8
+    [H0, W0, 3]): the overlay, ``frame`` where the id is 0 and ``(frame + rgb) // 2`` elsewhere.  ``stats``: per-channel
+    pixel counts and bounding boxes (empty channels: (INT32_MAX, INT32_MAX, -1, -1)).  ``remap`` False keeps the
+    channel index instead of the object id.  Only enqueues work: no host synchronisation."""
+    assert prob.is_cuda and prob.dtype == torch.float32 and prob.dim() == 3
+    prob = prob.contiguous()
+    c, h, w = prob.shape
+    oh, ow = (h, w) if size is None else (int(size[0]), int(size[1]))
+    dev = prob.device
+    lut, colours = segment_tables(object_manager, c, remap)
+    tables = torch.tensor([lut, colours], dtype=torch.int64).to(torch.int32).pin_memory().to(dev, non_blocking=True)
+    if frame is not None:
+        assert frame.is_cuda and frame.dtype == torch.uint8 and tuple(frame.shape) == (oh, ow, 3), frame.shape
+        frame = frame.contiguous()
+    out = Segments(lut)
+    if index:
+        out.index = torch.empty(oh, ow, dtype=torch.uint8, device=dev)
+    if rgb:
+        out.rgb = torch.empty(oh, ow, 3, dtype=torch.uint8, device=dev)
+    if frame is not None:
+        out.overlay = torch.empty(oh, ow, 3, dtype=torch.uint8, device=dev)
+    if stats:
+        out.counts = torch.empty(c, dtype=torch.int64, device=dev)
+        out.boxes = torch.empty(c, 4, dtype=torch.int32, device=dev)
+    nat.prob_to_segments(prob, c, h, w, oh, ow, tables[0], tables[1], frame, out.index, out.rgb, out.overlay,
+                         out.counts, out.boxes)
     return out

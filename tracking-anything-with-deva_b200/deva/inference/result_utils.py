@@ -1,0 +1,266 @@
+"""Drop-in ``ResultSaver`` (surface and outputs of the reference's deva/inference/result_utils.py) whose per-frame pixel
+work runs on the device.
+
+``save_mask`` runs ``frame_io.prob_to_segments`` on the current stream - resize, argmax, id remap, uint8 / RGB id image,
+overlay, per-channel areas and boxes in one kernel - starts the device-to-host copies into a ring of pinned buffers,
+records an event and queues the frame; it never synchronises the host.  The writer thread waits on the event and does
+only what has to stay on the host: PIL images and PNG / JPEG encoding, the JSON entries, the gradio writer, and the two
+paths that need third-party code - ``supervision`` boxes and labels for prompts, and ``pycocotools`` RLE for burst (the
+one per-object host loop left; a device RLE would remove it).  Both libraries are imported only when those paths run.
+"""
+import copy
+import os
+from dataclasses import dataclass
+from os import path
+from queue import Queue
+from threading import Thread
+from typing import Dict, List, Optional, Tuple
+
+import numpy as np
+import torch
+from PIL import Image
+
+from deva.inference.frame_io import prob_to_ids, prob_to_segments
+
+QUEUE_SIZE = 10
+RING_SIZE = QUEUE_SIZE + 2  # the queued frames, the one the writer holds and the one save_mask is filling
+
+
+class ResultSaver:
+    def __init__(self, output_root: str, video_name: str, *, dataset: str, object_manager, palette=None):
+        self.output_root = output_root
+        self.video_name = video_name
+        self.dataset = dataset.lower()
+        self.palette = palette
+        self.object_manager = object_manager
+
+        self.need_remapping = False
+        self.json_style = None
+        self.output_postfix = None
+        self.visualize = False
+
+        if self.dataset == 'vipseg':
+            self.all_annotations = []
+            self.video_json = {'video_id': video_name, 'annotations': self.all_annotations}
+            self.need_remapping = True
+            self.json_style = 'vipseg'
+            self.output_postfix = 'pan_pred'
+        elif self.dataset == 'burst':
+            self.need_remapping = True
+            self.all_annotations = []
+            self.video_json = {
+                'dataset': path.dirname(video_name),
+                'seq_name': path.basename(video_name),
+                'segmentations': self.all_annotations
+            }
+            self.json_style = 'burst'
+        elif self.dataset == 'unsup_davis17':
+            self.need_remapping = True
+        elif self.dataset == 'ref_davis':
+            pass
+        elif self.dataset == 'demo':
+            self.need_remapping = True
+            self.all_annotations = []
+            self.video_json = {'annotations': self.all_annotations}
+            self.json_style = 'vipseg'
+            self.visualize = True
+            self.visualize_postfix = 'Visualizations'
+            self.output_postfix = 'Annotations'
+        elif self.dataset == 'gradio':
+            # minimal mode: a cv2.VideoWriter is expected to be assigned to self.writer
+            self.writer = None
+            self.need_remapping = True
+            self.visualize = True
+        else:
+            raise NotImplementedError
+
+        self.free_slots = Queue()
+        for _ in range(RING_SIZE):
+            self.free_slots.put({})
+        self.queue = Queue(maxsize=QUEUE_SIZE)
+        self.thread = Thread(target=save_result, args=(self.queue, ))
+        self.thread.daemon = True
+        self.thread.start()
+
+    def save_mask(self,
+                  prob: torch.Tensor,
+                  frame_name: str,
+                  need_resize: bool = False,
+                  shape: Optional[Tuple[int, int]] = None,
+                  save_the_mask: bool = True,
+                  image_np: np.ndarray = None,
+                  prompts: List[str] = None,
+                  path_to_image: str = None):
+        prob = prob.float()
+        size = (int(shape[0]), int(shape[1])) if need_resize else tuple(prob.shape[-2:])
+        long_id = self.object_manager.use_long_id
+        overlay = save_the_mask and self.visualize and long_id
+        on_device = (isinstance(image_np, np.ndarray) and image_np.dtype == np.uint8 and image_np.shape == (*size, 3))
+        if overlay and image_np is None and path_to_image is None:
+            raise ValueError('Cannot visualize without image_np or path_to_image')
+
+        slot = self.free_slots.get()  # blocks only while every slot is queued or being written
+        frame = None
+        if overlay and on_device:
+            staged = _pinned(slot, 'image', image_np.shape, torch.uint8)
+            staged.numpy()[...] = image_np
+            frame = staged.to(prob.device, non_blocking=True)
+        seg = prob_to_segments(prob, self.object_manager, size, index=save_the_mask and not long_id,
+                               rgb=save_the_mask and long_id, frame=frame,
+                               stats=self.json_style is not None or self.visualize, remap=self.need_remapping)
+        host = {}
+        for name in ('index', 'rgb', 'overlay', 'counts', 'boxes'):
+            t = getattr(seg, name)
+            if t is not None:
+                host[name] = _pinned(slot, name, t.shape, t.dtype)
+                host[name].copy_(t, non_blocking=True)
+        if self.json_style == 'burst' or (overlay and not on_device):
+            # the full id map: burst's per-segment RLE and the host blend need ids, not colours
+            lut = torch.tensor(seg.lut, dtype=torch.int32).pin_memory().to(prob.device, non_blocking=True)
+            ids = prob_to_ids(prob, size=size, lut=lut)
+            host['ids'] = _pinned(slot, 'ids', ids.shape, ids.dtype)
+            host['ids'].copy_(ids, non_blocking=True)
+        done = torch.cuda.Event()
+        done.record()
+
+        self.queue.put(ResultArgs(
+            saver=self,
+            slot=slot,
+            host=host,
+            done=done,
+            lut=seg.lut,
+            long_id=long_id,
+            frame_name=frame_name,
+            save_the_mask=save_the_mask,
+            image_np=None if on_device else image_np,
+            prompts=prompts,
+            path_to_image=path_to_image,
+            all_obj_ids=[int(o.id) for o in self.object_manager.obj_to_tmp_id],
+            segments_info=copy.deepcopy(self.object_manager.get_current_segments_info()),
+        ))
+
+    def end(self):
+        self.queue.put(None)
+        self.queue.join()
+        self.thread.join()
+
+
+def _pinned(slot: Dict[str, torch.Tensor], name: str, shape, dtype) -> torch.Tensor:
+    """The slot's pinned buffer ``name``, reallocated when the shape or dtype changes."""
+    t = slot.get(name)
+    if t is None or t.shape != shape or t.dtype != dtype:
+        t = slot[name] = torch.empty(shape, dtype=dtype, pin_memory=True)
+    return t
+
+
+@dataclass
+class ResultArgs:
+    saver: ResultSaver
+    slot: Dict[str, torch.Tensor]  # pinned ring slot, returned to saver.free_slots when written
+    host: Dict[str, torch.Tensor]  # views of the slot's buffers that this frame's copies fill
+    done: torch.cuda.Event  # recorded after the copies
+    lut: List[int]  # prob channel -> id written for it
+    long_id: bool
+    frame_name: str
+    save_the_mask: bool
+    image_np: np.ndarray  # only when the overlay is blended on the host
+    prompts: List[str]
+    path_to_image: str
+    all_obj_ids: List[int]
+    segments_info: List[Dict]
+
+
+def save_result(queue: Queue):
+    while True:
+        args: ResultArgs = queue.get()
+        if args is None:
+            queue.task_done()
+            break
+        args.done.synchronize()
+        _write(args)
+        args.saver.free_slots.put(args.slot)
+        queue.task_done()
+
+
+def _write(args: ResultArgs):
+    saver, host, frame_name, segments_info = args.saver, args.host, args.frame_name, args.segments_info
+    area, box = {}, {}
+    if 'counts' in host:
+        counts, boxes = host['counts'].tolist(), host['boxes'].tolist()
+        for k, v in enumerate(args.lut):
+            if counts[k] == 0:
+                continue
+            area[v] = area.get(v, 0) + counts[k]
+            b = box.get(v, boxes[k])
+            box[v] = [min(b[0], boxes[k][0]), min(b[1], boxes[k][1]), max(b[2], boxes[k][2]), max(b[3], boxes[k][3])]
+
+    # record output in the json file
+    if saver.json_style == 'vipseg':
+        for seg in segments_info:
+            seg['area'] = area.get(seg['id'], 0)
+        segments_info = [s for s in segments_info if s['area'] > 0]
+        saver.all_annotations.append({'file_name': frame_name[:-4] + '.jpg', 'segments_info': segments_info})
+    elif saver.json_style == 'burst':
+        import pycocotools.mask as mask_util
+        ids = host['ids'].numpy()
+        for seg in segments_info:
+            m = ids == seg['id']
+            seg['area'] = area.get(seg['id'], 0)
+            coco_mask = mask_util.encode(np.asfortranarray(m))
+            coco_mask['counts'] = coco_mask['counts'].decode('utf-8')
+            seg['rle_mask'] = coco_mask
+        segments_info = [s for s in segments_info if s['area'] > 0]
+        saver.all_annotations.append({
+            'file_name': frame_name[:-4] + '.jpg',
+            'segmentations': [{'id': s['id'], 'score': s['score'], 'rle': s['rle_mask']} for s in segments_info],
+        })
+    elif saver.visualize:
+        for seg in segments_info:
+            seg['area'] = area.get(seg['id'], 0)
+        segments_info = [s for s in segments_info if s['area'] > 0]
+
+    if not args.save_the_mask:
+        return
+    if args.long_id:
+        rgb_mask = host['rgb'].numpy()
+        out_img = Image.fromarray(rgb_mask)
+    else:
+        out_img = Image.fromarray(host['index'].numpy())
+        if saver.palette is not None:
+            out_img.putpalette(saver.palette)
+    if saver.dataset != 'gradio':
+        _save(out_img, saver, saver.output_postfix, frame_name[:-4] + '.png')
+
+    if not (saver.visualize and args.long_id):
+        return
+    if 'overlay' in host:
+        blend = host['overlay'].numpy()
+    else:
+        image_np = args.image_np
+        if image_np is None:
+            image_np = np.array(Image.open(args.path_to_image))
+        # the reference's blend: alpha = 1 where the id is 0, else 0.5
+        alpha = (host['ids'].numpy() == 0).astype(np.float32)[:, :, None] * 0.5 + 0.5
+        blend = (image_np * alpha + rgb_mask * (1 - alpha)).astype(np.uint8)
+
+    if args.prompts is not None and len(segments_info) > 0:
+        import supervision as sv
+        labels = [f'{args.prompts[s["category_id"]]} {s["score"]:.2f}' for s in segments_info]
+        xyxy = np.array([box[s['id']] for s in segments_info], dtype=np.float32)
+        detections = sv.Detections(xyxy, confidence=np.array([s['score'] for s in segments_info]),
+                                   class_id=np.array([s['category_id'] for s in segments_info]))
+        blend = sv.BoundingBoxAnnotator().annotate(scene=blend, detections=detections)
+        blend = sv.LabelAnnotator().annotate(scene=blend, detections=detections, labels=labels)
+
+    if saver.dataset != 'gradio':
+        _save(Image.fromarray(blend), saver, saver.visualize_postfix, frame_name[:-4] + '.jpg')
+    else:
+        saver.writer.write(blend[:, :, ::-1])
+
+
+def _save(img: Image.Image, saver: ResultSaver, postfix: Optional[str], name: str):
+    out = path.join(saver.output_root, postfix) if postfix is not None else saver.output_root
+    if saver.video_name is not None:
+        out = path.join(out, saver.video_name)
+    os.makedirs(out, exist_ok=True)
+    img.save(path.join(out, name))
