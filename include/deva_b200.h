@@ -27,11 +27,12 @@
 extern "C" {
 #endif
 
-/* v13: deva_b200_prob_to_segments (the result savers' id map, id image, overlay, areas and boxes in one pass).
+/* v14: deva_b200_prob_to_scores and deva_b200_scores_to_ids (multi-scale / flip score export and merge).
+ * v13: deva_b200_prob_to_segments (the result savers' id map, id image, overlay, areas and boxes in one pass).
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 13
+#define DEVA_B200_ABI_VERSION 14
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -321,6 +322,18 @@ DEVA_B200_API int deva_b200_prob_to_segments(const float* prob, int c, int h, in
                                              const int32_t* lut, const uint32_t* rgb, const uint8_t* frame,
                                              uint8_t* out_u8, uint8_t* out_rgb, uint8_t* out_overlay, int64_t* counts,
                                              int32_t* boxes, deva_stream_t stream);
+/* Score export of multi-scale / flip evaluation (evaluation/eval_vos.py:169-177 with --save_scores, :188-189): the
+ * resize and flip of deva_b200_prob_to_ids (the same values, bit for bit), then per channel and output pixel
+ * s = (uint8)(v * 255) with one round-to-nearest float multiply and truncation, numpy's (x * 255).astype(np.uint8) on
+ * float32.  Each output optional, at least one given: scores u8 [c, out_h, out_w] = s; sum int32 [c, out_h, out_w] += s
+ * (the running sum of scripts/merge_multi_scale.py). */
+DEVA_B200_API int deva_b200_prob_to_scores(const float* prob, int c, int h, int w, int out_h, int out_w, int flip,
+                                           uint8_t* scores, int32_t* sum, deva_stream_t stream);
+/* Merge of multi-scale / flip scores (scripts/merge_multi_scale.py:process_vid): the channel of the first maximum of
+ * sum int32 [c, h, w] (np.argmax's tie order), mapped through lut int32 [c] (NULL: the channel itself).  Writes out_u8
+ * [h, w] and/or out_i64 [h, w] (either may be NULL, not both). */
+DEVA_B200_API int deva_b200_scores_to_ids(const int32_t* sum, int c, int h, int w, const int32_t* lut, uint8_t* out_u8,
+                                          int64_t* out_i64, deva_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -269,5 +269,13 @@ DEVA_B200_API int deva_b200_prob_to_segments(const float* prob, int c, int h, in
   return ew_prob_to_segments(prob, c, h, w, out_h, out_w, lut, rgb, frame, out_u8, out_rgb, out_overlay,
                              reinterpret_cast<unsigned long long*>(counts), boxes, S(stream));
 }
+DEVA_B200_API int deva_b200_prob_to_scores(const float* prob, int c, int h, int w, int out_h, int out_w, int flip,
+                                           uint8_t* scores, int32_t* sum, deva_stream_t stream) {
+  return ew_prob_to_scores(prob, c, h, w, out_h, out_w, flip, scores, sum, S(stream));
+}
+DEVA_B200_API int deva_b200_scores_to_ids(const int32_t* sum, int c, int h, int w, const int32_t* lut, uint8_t* out_u8,
+                                          int64_t* out_i64, deva_stream_t stream) {
+  return ew_scores_to_ids(sum, c, h, w, lut, out_u8, reinterpret_cast<long long*>(out_i64), S(stream));
+}
 
 }  // extern "C"

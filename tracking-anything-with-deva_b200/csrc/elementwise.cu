@@ -944,31 +944,58 @@ ingest_rgb8_kernel(const unsigned char* __restrict__ src, float* __restrict__ ds
   dst[2 * hw + i] = __fdiv_rn(__fdiv_rn((float)p[2], 255.f) - m2, s2);
 }
 
-// Channel of the first maximum of prob [c, h, w] bilinearly resized (align_corners = False, PyTorch's
-// upsample_bilinear2d arithmetic) to [out_h, out_w], at output pixel (oy, ox); channels streamed.  Every egress kernel
-// goes through this one function, so their id maps agree bit for bit.
+// Source taps of output pixel (oy, ox) of a bilinear resize (align_corners = False, PyTorch's upsample_bilinear2d
+// arithmetic) of one [h, w] plane to [out_h, out_w]; the same for every channel, so computed once per pixel.
+struct ResizeTaps {
+  long long off;  // offset in the plane of the top-left source pixel (of the pixel itself when `same`)
+  int dx, dy;     // offsets of the right / lower neighbour, 0 at the last column / row
+  float lx0, lx1, ly0, ly1;
+  bool same;      // out_h == h && out_w == w: the value is read, not interpolated
+};
+__device__ __forceinline__ ResizeTaps resize_taps(int h, int w, int out_h, int out_w, float rh, float rw, int oy, int ox) {
+  ResizeTaps t;
+  t.same = out_h == h && out_w == w;
+  if (t.same) {
+    t.off = (long long)oy * w + ox;
+    t.dx = t.dy = 0;
+    t.lx0 = t.ly0 = 1.f;
+    t.lx1 = t.ly1 = 0.f;
+    return t;
+  }
+  const float sy = fmaxf(rh * (oy + 0.5f) - 0.5f, 0.f), sx = fmaxf(rw * (ox + 0.5f) - 0.5f, 0.f);
+  const int y0 = (int)sy, x0 = (int)sx;
+  t.dx = x0 < w - 1 ? 1 : 0;
+  t.dy = y0 < h - 1 ? w : 0;
+  t.ly1 = sy - y0; t.ly0 = 1.f - t.ly1; t.lx1 = sx - x0; t.lx0 = 1.f - t.lx1;
+  t.off = (long long)y0 * w + x0;
+  return t;
+}
+// Value of one channel plane at the output pixel of `t`.  Every egress kernel reads its values through this one
+// function, so their id maps and scores come from the same float, bit for bit.
+__device__ __forceinline__ float resized_value(const float* __restrict__ plane, const ResizeTaps& t) {
+  const float* q = plane + t.off;
+  if (t.same) return q[0];
+  return t.ly0 * (t.lx0 * q[0] + t.lx1 * q[t.dx]) + t.ly1 * (t.lx0 * q[t.dy] + t.lx1 * q[t.dy + t.dx]);
+}
+
+// Channel of the first maximum of prob [c, h, w] resized to [out_h, out_w], at output pixel (oy, ox); channels
+// streamed.
 __device__ __forceinline__ int resized_argmax(const float* __restrict__ prob, int c, int h, int w, int out_h, int out_w,
                                               float rh, float rw, int oy, int ox) {
+  const ResizeTaps t = resize_taps(h, w, out_h, out_w, rh, rw, oy, ox);
+  const long long plane = (long long)h * w;
   int best = 0;
   float best_v;
-  const long long plane = (long long)h * w;
-  if (out_h == h && out_w == w) {
-    const float* p = prob + (long long)oy * w + ox;
-    best_v = p[0];
+  if (t.same) {
+    best_v = resized_value(prob, t);
     for (int k = 1; k < c; ++k) {
-      const float v = p[k * plane];
+      const float v = resized_value(prob + k * plane, t);
       if (v > best_v) { best_v = v; best = k; }
     }
   } else {
-    const float sy = fmaxf(rh * (oy + 0.5f) - 0.5f, 0.f), sx = fmaxf(rw * (ox + 0.5f) - 0.5f, 0.f);
-    const int y0 = (int)sy, x0 = (int)sx;
-    const int yp = y0 < h - 1 ? 1 : 0, xp = x0 < w - 1 ? 1 : 0;
-    const float ly1 = sy - y0, ly0 = 1.f - ly1, lx1 = sx - x0, lx0 = 1.f - lx1;
-    const float* p = prob + (long long)y0 * w + x0;
     best_v = -INFINITY;
     for (int k = 0; k < c; ++k) {
-      const float* q = p + k * plane;
-      const float v = ly0 * (lx0 * q[0] + lx1 * q[xp]) + ly1 * (lx0 * q[yp * w] + lx1 * q[yp * w + xp]);
+      const float v = resized_value(prob + k * plane, t);
       if (v > best_v) { best_v = v; best = k; }
     }
   }
@@ -986,6 +1013,45 @@ prob_to_ids_kernel(const float* __restrict__ prob, int c, int h, int w, int out_
   const int oy = (int)(i / out_w), ox_out = (int)(i - (long long)oy * out_w);
   const int ox = flip ? out_w - 1 - ox_out : ox_out;  // flip acts on the resized map
   const int best = resized_argmax(prob, c, h, w, out_h, out_w, rh, rw, oy, ox);
+  const int id = lut ? lut[best] : best;
+  if (out_u8) out_u8[i] = (unsigned char)id;
+  if (out_i64) out_i64[i] = id;
+}
+
+// Score export of multi-scale / flip evaluation: prob [c, h, w] -> per channel s = (uint8)(v * 255) of the resized (and
+// optionally flipped) value v, with one RN multiply and truncation: numpy's (x * 255).astype(np.uint8) on float32 for
+// v in [0, 256 / 255).  Written to scores u8 [c, out_h, out_w] and / or added to the running sum int32 [c, out_h, out_w].
+// One thread per output pixel, channels streamed; each thread owns its pixel in every plane, so the add needs no atomic.
+__global__ void __launch_bounds__(256)
+prob_to_scores_kernel(const float* __restrict__ prob, int c, int h, int w, int out_h, int out_w, int flip, float rh,
+                      float rw, unsigned char* __restrict__ scores, int* __restrict__ sum) {
+  const long long n = (long long)out_h * out_w;
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= n) return;
+  const int oy = (int)(i / out_w), ox_out = (int)(i - (long long)oy * out_w);
+  const int ox = flip ? out_w - 1 - ox_out : ox_out;  // flip acts on the resized map
+  const ResizeTaps t = resize_taps(h, w, out_h, out_w, rh, rw, oy, ox);
+  const long long plane = (long long)h * w;
+  for (int k = 0; k < c; ++k) {
+    const float v = resized_value(prob + k * plane, t);
+    const unsigned s = __float2uint_rz(__fmul_rn(v, 255.f)) & 255u;
+    if (scores) scores[k * n + i] = (unsigned char)s;
+    if (sum) sum[k * n + i] += (int)s;
+  }
+}
+
+// Merge of multi-scale / flip scores: sum int32 [c, n] -> channel of the first maximum (np.argmax's tie order), mapped
+// through lut (or kept when lut is null).  One thread per pixel, channels streamed.
+__global__ void __launch_bounds__(256)
+scores_to_ids_kernel(const int* __restrict__ sum, int c, long long n, const int* __restrict__ lut,
+                     unsigned char* __restrict__ out_u8, long long* __restrict__ out_i64) {
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= n) return;
+  int best = 0, best_v = sum[i];
+  for (int k = 1; k < c; ++k) {
+    const int v = sum[k * n + i];
+    if (v > best_v) { best_v = v; best = k; }
+  }
   const int id = lut ? lut[best] : best;
   if (out_u8) out_u8[i] = (unsigned char)id;
   if (out_i64) out_i64[i] = id;
@@ -1166,6 +1232,24 @@ int ew_prob_to_ids(const float* prob, int c, int h, int w, int out_h, int out_w,
   const long long n = (long long)out_h * out_w;
   ew::prob_to_ids_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, s>>>(prob, c, h, w, out_h, out_w, flip, (float)h / out_h,
                                                                      (float)w / out_w, lut, out_u8, out_i64);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+int ew_prob_to_scores(const float* prob, int c, int h, int w, int out_h, int out_w, int flip, unsigned char* scores,
+                      int* sum, cudaStream_t s) {
+  B200_REQUIRE(prob && c >= 1 && h > 0 && w > 0 && out_h > 0 && out_w > 0 && (scores || sum),
+               "prob_to_scores: bad arguments");
+  const long long n = (long long)out_h * out_w;
+  ew::prob_to_scores_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, s>>>(prob, c, h, w, out_h, out_w, flip,
+                                                                         (float)h / out_h, (float)w / out_w, scores, sum);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+int ew_scores_to_ids(const int* sum, int c, int h, int w, const int* lut, unsigned char* out_u8, long long* out_i64,
+                     cudaStream_t s) {
+  B200_REQUIRE(sum && c >= 1 && h > 0 && w > 0 && (out_u8 || out_i64), "scores_to_ids: bad arguments");
+  const long long n = (long long)h * w;
+  ew::scores_to_ids_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, s>>>(sum, c, n, lut, out_u8, out_i64);
   B200_LAUNCH_CHECK();
   return 0;
 }

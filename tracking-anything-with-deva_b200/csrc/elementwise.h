@@ -35,6 +35,10 @@ int ew_mask_nearest(const unsigned char* src, int h, int w, int out_h, int out_w
                     int flip, long long* dst, cudaStream_t s);
 int ew_prob_to_ids(const float* prob, int c, int h, int w, int out_h, int out_w, int flip, const int* lut,
                    unsigned char* out_u8, long long* out_i64, cudaStream_t s);
+int ew_prob_to_scores(const float* prob, int c, int h, int w, int out_h, int out_w, int flip, unsigned char* scores,
+                      int* sum, cudaStream_t s);
+int ew_scores_to_ids(const int* sum, int c, int h, int w, const int* lut, unsigned char* out_u8, long long* out_i64,
+                     cudaStream_t s);
 constexpr int kMaxSegmentChannels = 8192;  // prob_to_segments' shared-memory histogram: 20 bytes per channel
 int ew_prob_to_segments(const float* prob, int c, int h, int w, int out_h, int out_w, const int* lut,
                         const unsigned* rgb, const unsigned char* frame, unsigned char* out_u8, unsigned char* out_rgb,

@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 13
+ABI_VERSION = 14
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -104,6 +104,9 @@ _SIGNATURES = {
                                       c_void_p]),
     'deva_b200_prob_to_segments': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'deva_b200_prob_to_scores': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                         c_void_p]),
+    'deva_b200_scores_to_ids': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -386,6 +389,16 @@ def prob_to_segments(prob, c, h, w, out_h, out_w, lut, rgb, frame, out_u8, out_r
     _check(lib().deva_b200_prob_to_segments(_ptr(prob), c, h, w, out_h, out_w, _ptr(lut), _p(rgb), _p(frame), _p(out_u8),
                                             _p(out_rgb), _p(out_overlay), _p(counts), _p(boxes), _stream()),
            'prob_to_segments')
+
+
+def prob_to_scores(prob, c, h, w, out_h, out_w, flip, scores, total):
+    _check(lib().deva_b200_prob_to_scores(_ptr(prob), c, h, w, out_h, out_w, int(bool(flip)), _p(scores), _p(total),
+                                          _stream()), 'prob_to_scores')
+
+
+def scores_to_ids(total, c, h, w, lut, out_u8, out_i64):
+    _check(lib().deva_b200_scores_to_ids(_p(total), c, h, w, _p(lut), _p(out_u8), _p(out_i64), _stream()),
+           'scores_to_ids')
 
 
 def transpose_append(src, dst, ld_dst, n, c):

@@ -12,6 +12,9 @@ real pipeline, each as one kernel.
   optional flip, argmax, ``ObjectManager.tmp_to_obj_cls`` - fused into a single pass that writes the id map.
 * ``prob_to_segments``: the same resize and argmax plus everything the result savers derive from the id map (index
   mask, long-id RGB image, visualisation overlay, per-segment areas and boxes), in one pass.
+* ``prob_to_scores`` / ``scores_to_ids``: multi-scale / flip evaluation - eval_vos.py's ``--save_scores`` array (the
+  same resize and flip, quantised to uint8) and scripts/merge_multi_scale.py's merge of the members' arrays (sum,
+  argmax, ``{object id: tmp id}`` remap).
 """
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -240,4 +243,62 @@ def prob_to_segments(prob: torch.Tensor, object_manager, size: Optional[Tuple[in
         out.boxes = torch.empty(c, 4, dtype=torch.int32, device=dev)
     nat.prob_to_segments(prob, c, h, w, oh, ow, tables[0], tables[1], frame, out.index, out.rgb, out.overlay,
                          out.counts, out.boxes)
+    return out
+
+
+def prob_to_scores(prob: torch.Tensor, size: Optional[Tuple[int, int]] = None, flip: bool = False, *,
+                   scores: bool = True, into: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+    """prob float32 [K+1, H, W] from ``step`` -> uint8 scores [K+1, H0, W0] (``size`` or H, W) on the device.
+
+    Equals ``(flip(interpolate(prob, size, 'bilinear', align_corners=False)) * 255).astype(np.uint8)``, the array
+    eval_vos.py writes with ``--save_scores``: the resize and flip are ``prob_to_ids``' (the same values, bit for bit),
+    the product one float32 multiply, truncated.  ``into`` (int32 [K+1, H0, W0] on the device) gets the scores added
+    in the same pass: the running sum of a multi-scale / flip merge.  Returns the scores, or None with
+    ``scores=False`` (then ``into`` is required).  Only enqueues work: no host synchronisation."""
+    assert prob.is_cuda and prob.dtype == torch.float32 and prob.dim() == 3
+    prob = prob.contiguous()
+    c, h, w = prob.shape
+    oh, ow = (h, w) if size is None else (int(size[0]), int(size[1]))
+    if into is not None:
+        if not (into.is_cuda and into.dtype == torch.int32 and into.is_contiguous() and into.device == prob.device):
+            raise RuntimeError(f'prob_to_scores: into must be a contiguous int32 tensor on {prob.device}')
+        if tuple(into.shape) != (c, oh, ow):
+            raise RuntimeError(f'prob_to_scores: into has shape {tuple(into.shape)}, expected {(c, oh, ow)}')
+    if not scores and into is None:
+        raise RuntimeError('prob_to_scores: nothing to write (scores=False and no into)')
+    out = torch.empty(c, oh, ow, dtype=torch.uint8, device=prob.device) if scores else None
+    nat.prob_to_scores(prob, c, h, w, oh, ow, flip, out, into)
+    return out
+
+
+def mapping_lut(mapping: Dict[int, int], channels: int) -> List[int]:
+    """``{object id: tmp id}`` (``ObjectManager.get_tmp_to_obj_mapping()``, eval_vos' backward.hkl) -> the value of
+    each channel in merge_multi_scale.py's remap loop: ``idx_mask[argmax == tmp] = object id`` for every entry in
+    order, so a later entry for the same channel overwrites an earlier one, and a channel no entry names stays 0."""
+    lut = [0] * channels
+    for obj_id, tmp in mapping.items():
+        if 0 <= tmp < channels:
+            lut[tmp] = int(obj_id)
+    return lut
+
+
+def scores_to_ids(total: torch.Tensor, object_manager=None, *, mapping: Optional[Dict[int, int]] = None,
+                  dtype: torch.dtype = torch.uint8) -> torch.Tensor:
+    """Summed scores int32 [K+1, H, W] -> id map [H, W] (uint8 or long) on the device: merge_multi_scale.py's
+    ``np.argmax`` over channels (the first maximum wins a tie) and its remap through ``mapping`` (``{object id:
+    tmp id}``; default ``object_manager.get_tmp_to_obj_mapping()``, with neither the channel itself).  uint8 ids
+    above 255 wrap.  Only enqueues work: no host synchronisation."""
+    assert dtype in (torch.long, torch.uint8), dtype
+    if not (total.is_cuda and total.dtype == torch.int32 and total.dim() == 3):
+        raise RuntimeError(f'scores_to_ids: expected int32 [K+1, H, W] on the device, got {total.dtype} '
+                           f'{tuple(total.shape)} on {total.device}')
+    total = total.contiguous()
+    c, h, w = total.shape
+    if mapping is None and object_manager is not None:
+        mapping = object_manager.get_tmp_to_obj_mapping()
+    lut = None
+    if mapping is not None:
+        lut = torch.tensor(mapping_lut(mapping, c), dtype=torch.int32).pin_memory().to(total.device, non_blocking=True)
+    out = torch.empty(h, w, dtype=dtype, device=total.device)
+    nat.scores_to_ids(total, c, h, w, lut, out if dtype == torch.uint8 else None, out if dtype == torch.long else None)
     return out
