@@ -5,7 +5,6 @@
 // tokens that change.  All kernels are HBM-bound copy/convert passes.
 #include <cuda_fp16.h>
 
-#include "bank_ops.h"
 #include "common.h"
 
 namespace b200 {
@@ -144,70 +143,86 @@ static int grid_for(long long total) {
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
-int launch_pack_query(const float* qk, const float* qe, long long sc, long long sq, int ck, int q, __half* hi,
-                      __half* lo, float* bsq, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+DEVA_B200_API int deva_b200_pack_query(const float* qk, const float* qe, int64_t stride_c, int64_t stride_q, int ck, int q,
+                                       void* q_hi, void* q_lo, float* bsq, deva_stream_t stream) {
   B200_REQUIRE(q >= 1, "pack_query: empty");
+  __half* hi = H(q_hi);
+  __half* lo = H(q_lo);
+  const cudaStream_t s = S(stream);
   const int grid = ceil_div(q, bank::TOK);
-  if (ck == 64) bank::pack_query_kernel<64><<<grid, 256, 0, stream>>>(qk, qe, sc, sq, q, hi, lo, bsq);
-  else if (ck == 32) bank::pack_query_kernel<32><<<grid, 256, 0, stream>>>(qk, qe, sc, sq, q, hi, lo, bsq);
+  if (ck == 64) bank::pack_query_kernel<64><<<grid, 256, 0, s>>>(qk, qe, stride_c, stride_q, q, hi, lo, bsq);
+  else if (ck == 32) bank::pack_query_kernel<32><<<grid, 256, 0, s>>>(qk, qe, stride_c, stride_q, q, hi, lo, bsq);
   else B200_REQUIRE(false, "pack_query: key_dim %d unsupported (32 or 64)", ck);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-int launch_pack_keys(const float* key, const float* sel, long long sc, long long sn, const float* shr, int ck, int n,
-                     __half* hi, __half* lo, float* neg_s, float* raw_key, float* raw_sel, float* raw_shr,
-                     cudaStream_t stream) {
+DEVA_B200_API int deva_b200_pack_keys(const float* key, const float* selection, int64_t stride_c, int64_t stride_t,
+                                      const float* shrinkage, int ck, int n, void* k_hi, void* k_lo, float* neg_s,
+                                      float* raw_key, float* raw_sel, float* raw_shr, deva_stream_t stream) {
   B200_REQUIRE(n >= 1, "pack_keys: empty");
-  B200_REQUIRE(sel == nullptr || raw_sel != nullptr, "pack_keys: selection given without a destination");
+  B200_REQUIRE(selection == nullptr || raw_sel != nullptr, "pack_keys: selection given without a destination");
+  __half* hi = H(k_hi);
+  __half* lo = H(k_lo);
+  const cudaStream_t s = S(stream);
   const int grid = ceil_div(n, bank::TOK);
   if (ck == 64)
-    bank::pack_keys_kernel<64><<<grid, 256, 0, stream>>>(key, sel, sc, sn, shr, n, hi, lo, neg_s, raw_key, raw_sel, raw_shr);
+    bank::pack_keys_kernel<64><<<grid, 256, 0, s>>>(key, selection, stride_c, stride_t, shrinkage, n, hi, lo, neg_s,
+                                                    raw_key, raw_sel, raw_shr);
   else if (ck == 32)
-    bank::pack_keys_kernel<32><<<grid, 256, 0, stream>>>(key, sel, sc, sn, shr, n, hi, lo, neg_s, raw_key, raw_sel, raw_shr);
+    bank::pack_keys_kernel<32><<<grid, 256, 0, s>>>(key, selection, stride_c, stride_t, shrinkage, n, hi, lo, neg_s,
+                                                    raw_key, raw_sel, raw_shr);
   else B200_REQUIRE(false, "pack_keys: key_dim %d unsupported (32 or 64)", ck);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-int launch_append_values(const float* src, long long ld_src, __half* dst, long long ld_dst, int rows, int n,
-                         cudaStream_t stream) {
+DEVA_B200_API int deva_b200_append_values(const float* src, int64_t ld_src, void* dst, int64_t ld_dst, int rows, int n,
+                                          deva_stream_t stream) {
   B200_REQUIRE(rows >= 1 && n >= 1, "append_values: empty");
-  bank::append_values_kernel<<<grid_for((long long)rows * n), 256, 0, stream>>>(src, ld_src, dst, ld_dst, rows, n);
+  bank::append_values_kernel<<<grid_for((long long)rows * n), 256, 0, S(stream)>>>(src, ld_src, H(dst), ld_dst, rows, n);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-int launch_gather_rows(void* dst, const void* src, const int* idx, int n, int row_bytes, cudaStream_t stream) {
+DEVA_B200_API int deva_b200_gather_rows(void* dst, const void* src, const int32_t* idx, int n, int row_bytes,
+                                        deva_stream_t stream) {
   B200_REQUIRE(row_bytes % 16 == 0, "gather_rows: row_bytes %d not a multiple of 16", row_bytes);
   if (n <= 0) return 0;
   const int vec = row_bytes / 16;
-  bank::gather_rows_kernel<<<grid_for((long long)n * vec), 256, 0, stream>>>(
+  bank::gather_rows_kernel<<<grid_for((long long)n * vec), 256, 0, S(stream)>>>(
       reinterpret_cast<uint4*>(dst), reinterpret_cast<const uint4*>(src), idx, n, vec);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-int launch_gather_f32(float* dst, const float* src, const int* idx, int n, cudaStream_t stream) {
+DEVA_B200_API int deva_b200_gather_f32(float* dst, const float* src, const int32_t* idx, int n, deva_stream_t stream) {
   if (n <= 0) return 0;
-  bank::gather_f32_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(dst, src, idx, n);
+  bank::gather_f32_kernel<<<ceil_div(n, 256), 256, 0, S(stream)>>>(dst, src, idx, n);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-int launch_gather_cols_f16(__half* dst, long long ld_dst, const __half* src, long long ld_src, const int* idx,
-                           int rows, int n, cudaStream_t stream) {
+DEVA_B200_API int deva_b200_gather_cols_f16(void* dst, int64_t ld_dst, const void* src, int64_t ld_src, const int32_t* idx,
+                                            int rows, int n, deva_stream_t stream) {
   if (n <= 0 || rows <= 0) return 0;
-  bank::gather_cols_f16_kernel<<<grid_for((long long)rows * n), 256, 0, stream>>>(dst, ld_dst, src, ld_src, idx, rows, n);
+  bank::gather_cols_f16_kernel<<<grid_for((long long)rows * n), 256, 0, S(stream)>>>(H(dst), ld_dst, H(src), ld_src, idx,
+                                                                                     rows, n);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-int launch_usage(float* out, const float* use, const float* life, int n, cudaStream_t stream) {
+DEVA_B200_API int deva_b200_usage(float* out, const float* use_cnt, const float* life_cnt, int n, deva_stream_t stream) {
   if (n <= 0) return 0;
-  bank::usage_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(out, use, life, n);
+  bank::usage_kernel<<<ceil_div(n, 256), 256, 0, S(stream)>>>(out, use_cnt, life_cnt, n);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-}  // namespace b200
+}  // extern "C"

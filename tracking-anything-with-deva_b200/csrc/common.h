@@ -1,7 +1,10 @@
-// Shared host-side helpers for the C-ABI layer: error slot + launch checks.
+// Shared host-side helpers of the C entry points: error slot, launch checks, casts from the ABI's types.
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdio.h>
+
+#include "deva_b200.h"
 
 namespace b200 {
 
@@ -32,6 +35,13 @@ void count_launch();  // bumps the counter read by deva_b200_launch_count()
   } while (0)
 
 inline int ceil_div(long long a, long long b) { return static_cast<int>((a + b - 1) / b); }
+
+// The ABI passes streams as deva_stream_t and fp16 buffers as void*.
+inline cudaStream_t S(deva_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
+inline __half* H(void* p) { return reinterpret_cast<__half*>(p); }
+inline const __half* H(const void* p) { return reinterpret_cast<const __half*>(p); }
+
+constexpr int kListCap = DEVA_B200_LIST_PITCH;  // max top_k; also the row pitch of the top-k index / weight lists
 
 constexpr int kMaxDevices = 64;
 int device_slot();  // current CUDA device, clamped to [0, kMaxDevices): index of per-device one-time state

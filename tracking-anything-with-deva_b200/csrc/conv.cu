@@ -27,7 +27,6 @@
 #include <type_traits>
 
 #include "common.h"
-#include "conv.h"
 #include "ptx.cuh"
 #include "tmap.h"
 
@@ -46,6 +45,8 @@ constexpr int THREADS = CONSUMER_THREADS + 128;
 // returns 128 each, which is exactly the 64 more each consumer takes.
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 static_assert(128 * PRODUCER_REGS + CONSUMER_THREADS * CONSUMER_REGS <= THREADS * 168, "conv: register budget");
+constexpr int kMaxTaps = 32;  // k-entries (filter tap x pass) of one launch
+constexpr int kMaxHead = 9;   // outputs of the fused 1x1 head
 constexpr int HEAD_BYTES = kMaxHead * 256 * 4;
 constexpr int kMaxBias = 2048;   // bias of the whole layer staged in shared memory (Cout_pad <= kMaxBias)
 constexpr int kMaxRank1 = 1024;  // same for the rank-1 input column
@@ -413,9 +414,16 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
 }
 
 }  // namespace conv
+}  // namespace b200
 
-int launch_conv(const ConvDesc& d, cudaStream_t stream) {
+using namespace b200;
+
+extern "C" {
+
+// The descriptor is read on the host only: the kernel receives the Params built from it.
+DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_t stream) {
   using namespace conv;
+  const deva_b200_conv_desc& d = *desc;
   B200_REQUIRE(d.cin_pad % 64 == 0 && d.cin_pad >= 64, "conv: cin_pad %d must be a multiple of 64", d.cin_pad);
   B200_REQUIRE(d.stride == 1 || d.stride == 2, "conv: stride %d unsupported", d.stride);
   B200_REQUIRE(d.kh == d.kw && (d.kh == 1 || d.kh == 3), "conv: %dx%d filter unsupported here", d.kh, d.kw);
@@ -576,9 +584,9 @@ int launch_conv(const ConvDesc& d, cudaStream_t stream) {
   p.f32_split_stride = (long long)d.batch * ho * wo * d.cout;
   const long long units = (long long)p.m_tiles * p.n_tiles * p.ksplit;
   const int grid = (int)(units < sm_count() ? units : sm_count());
-  kern<<<grid, THREADS, SMEM_BYTES, stream>>>(maps, p);
+  kern<<<grid, THREADS, SMEM_BYTES, S(stream)>>>(maps, p);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-}  // namespace b200
+}  // extern "C"

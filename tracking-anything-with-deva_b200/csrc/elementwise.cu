@@ -10,7 +10,6 @@
 #include <stdint.h>
 
 #include "common.h"
-#include "elementwise.h"
 
 namespace b200 {
 namespace ew {
@@ -785,152 +784,184 @@ static int grid_of(long long total) {
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
-int ew_nchw_to_nhwc(const float* src, __half* dst, int B, int C, int H, int W, int Cp, cudaStream_t s) {
-  ew::nchw_to_nhwc_kernel<<<grid_of((long long)B * H * W * Cp), 256, 0, s>>>(src, dst, B, C, H, W, Cp);
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+DEVA_B200_API int deva_b200_nchw_to_nhwc(const float* src, void* dst, int b, int c, int h, int w, int c_pad,
+                                         deva_stream_t stream) {
+  ew::nchw_to_nhwc_kernel<<<grid_of((long long)b * h * w * c_pad), 256, 0, S(stream)>>>(src, H(dst), b, c, h, w, c_pad);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_nhwc_to_nchw(const __half* src, float* dst, int B, int C, int H, int W, cudaStream_t s) {
-  ew::nhwc_to_nchw_kernel<<<grid_of((long long)B * C * H * W), 256, 0, s>>>(src, dst, B, C, H, W);
+DEVA_B200_API int deva_b200_nhwc_to_nchw(const void* src, float* dst, int b, int c, int h, int w, deva_stream_t stream) {
+  ew::nhwc_to_nchw_kernel<<<grid_of((long long)b * c * h * w), 256, 0, S(stream)>>>(H(src), dst, b, c, h, w);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_stem_im2col(const float* src, __half* dst, __half* dst_lo, int B, int C, int H, int W, int Kp, cudaStream_t s) {
-  B200_REQUIRE(H % 2 == 0 && W % 2 == 0 && Kp % 64 == 0 && Kp >= 49 * C, "stem_im2col: bad shape");
-  B200_REQUIRE(C >= 1 && C <= 8, "stem_im2col: at most 8 input planes");
-  const size_t smem = (size_t)C * 7 * (2 * ew::IM_XT + 5) * sizeof(float);
+DEVA_B200_API int deva_b200_stem_im2col(const float* src, void* dst, void* dst_lo, int b, int c, int h, int w, int k_pad,
+                                        deva_stream_t stream) {
+  B200_REQUIRE(h % 2 == 0 && w % 2 == 0 && k_pad % 64 == 0 && k_pad >= 49 * c, "stem_im2col: bad shape");
+  B200_REQUIRE(c >= 1 && c <= 8, "stem_im2col: at most 8 input planes");
+  __half* hi = H(dst);
+  __half* lo = H(dst_lo);
+  const cudaStream_t s = S(stream);
+  const size_t smem = (size_t)c * 7 * (2 * ew::IM_XT + 5) * sizeof(float);
   // the network's shapes: one thread per output pixel, whole im2col rows written with 16-byte stores
-  const dim3 gx(ceil_div(W / 2, ew::IM1_XT));
-  if (C == 1 && Kp == 64 && !dst_lo) {
-    ew::stem_im2col_px_kernel<1, 4, false><<<dim3(gx.x, B * ceil_div(H / 2, 4)), ew::IM1_XT, 0, s>>>(src, dst, nullptr, B, H, W);
+  const dim3 gx(ceil_div(w / 2, ew::IM1_XT));
+  if (c == 1 && k_pad == 64 && !lo) {
+    ew::stem_im2col_px_kernel<1, 4, false><<<dim3(gx.x, b * ceil_div(h / 2, 4)), ew::IM1_XT, 0, s>>>(src, hi, nullptr, b, h, w);
     B200_LAUNCH_CHECK();
     return 0;
   }
-  if (C == 3 && Kp == 192) {
-    if (dst_lo) ew::stem_im2col_px_kernel<3, 2, true><<<dim3(gx.x, B * ceil_div(H / 2, 2)), ew::IM1_XT, 0, s>>>(src, dst, dst_lo, B, H, W);
-    else ew::stem_im2col_px_kernel<3, 2, false><<<dim3(gx.x, B * ceil_div(H / 2, 2)), ew::IM1_XT, 0, s>>>(src, dst, nullptr, B, H, W);
+  if (c == 3 && k_pad == 192) {
+    if (lo) ew::stem_im2col_px_kernel<3, 2, true><<<dim3(gx.x, b * ceil_div(h / 2, 2)), ew::IM1_XT, 0, s>>>(src, hi, lo, b, h, w);
+    else ew::stem_im2col_px_kernel<3, 2, false><<<dim3(gx.x, b * ceil_div(h / 2, 2)), ew::IM1_XT, 0, s>>>(src, hi, nullptr, b, h, w);
     B200_LAUNCH_CHECK();
     return 0;
   }
-  ew::stem_im2col_kernel<<<dim3(ceil_div(W / 2, ew::IM_XT), B * (H / 2)), 256, smem, s>>>(src, dst, dst_lo, B, C, H, W, Kp);
+  ew::stem_im2col_kernel<<<dim3(ceil_div(w / 2, ew::IM_XT), b * (h / 2)), 256, smem, s>>>(src, hi, lo, b, c, h, w, k_pad);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_maxpool(const __half* x, const __half* x_lo, __half* y, __half* y_lo, int B, int H, int W, int C, cudaStream_t s) {
-  B200_REQUIRE(C % 8 == 0, "maxpool: C %% 8");
-  ew::maxpool_kernel<<<grid_of((long long)B * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8)), 256, 0, s>>>(x, x_lo, y, y_lo, B, H, W, C);
+DEVA_B200_API int deva_b200_maxpool(const void* x, const void* x_lo, void* y, void* y_lo, int b, int h, int w, int c,
+                                    deva_stream_t stream) {
+  B200_REQUIRE(c % 8 == 0, "maxpool: C %% 8");
+  ew::maxpool_kernel<<<grid_of((long long)b * ((h + 1) / 2) * ((w + 1) / 2) * (c / 8)), 256, 0, S(stream)>>>(
+      H(x), H(x_lo), H(y), H(y_lo), b, h, w, c);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_up2_add(const __half* g, const __half* skip, __half* raw, __half* relu, int B, int h, int w, int C, cudaStream_t s) {
-  B200_REQUIRE(C % 8 == 0, "up2_add: C %% 8");
-  ew::up2_add_kernel<<<dim3(ceil_div(2 * w * (C / 8), 256 * 2), B * 2 * h), 256, 0, s>>>(g, skip, raw, relu, B, h, w, C);
+DEVA_B200_API int deva_b200_up2_add(const void* g, const void* skip, void* raw, void* relu, int b, int h, int w, int c,
+                                    deva_stream_t stream) {
+  B200_REQUIRE(c % 8 == 0, "up2_add: C %% 8");
+  ew::up2_add_kernel<<<dim3(ceil_div(2 * w * (c / 8), 256 * 2), b * 2 * h), 256, 0, S(stream)>>>(H(g), H(skip), H(raw),
+                                                                                                H(relu), b, h, w, c);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_up2_add_split(const __half* g, const __half* g_lo, const __half* skip, const __half* skip_lo, __half* raw,
-                     __half* raw_lo, __half* relu, __half* relu_lo, unsigned char* relu_lo8, int B, int h, int w, int C,
-                     cudaStream_t s) {
-  B200_REQUIRE(C % 8 == 0 && g_lo && (raw != nullptr) == (raw_lo != nullptr) && (raw || relu) && (!relu_lo || relu) &&
+DEVA_B200_API int deva_b200_up2_add_split(const void* g, const void* g_lo, const void* skip, const void* skip_lo,
+                                          void* raw, void* raw_lo, void* relu, void* relu_lo, void* relu_lo8, int b, int h,
+                                          int w, int c, deva_stream_t stream) {
+  B200_REQUIRE(c % 8 == 0 && g_lo && (raw != nullptr) == (raw_lo != nullptr) && (raw || relu) && (!relu_lo || relu) &&
                    (!relu_lo8 || (relu && !relu_lo)),
                "up2_add_split: C %% 8, g_lo, and raw/raw_lo (both or neither) with at least one output are required");
-  ew::up2_add_split_kernel<<<dim3(ceil_div((w + 1) * (C / 8), 256), B * (h + 1)), 256, 0, s>>>(
-      g, g_lo, skip, skip_lo, raw, raw_lo, relu, relu_lo, relu_lo8, B, h, w, C);
+  ew::up2_add_split_kernel<<<dim3(ceil_div((w + 1) * (c / 8), 256), b * (h + 1)), 256, 0, S(stream)>>>(
+      H(g), H(g_lo), H(skip), H(skip_lo), H(raw), H(raw_lo), H(relu), H(relu_lo), reinterpret_cast<unsigned char*>(relu_lo8),
+      b, h, w, c);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-int ew_area_down(const __half* x, __half* y, int B, int H, int W, int C, int r, cudaStream_t s) {
-  B200_REQUIRE(C % 8 == 0 && H % r == 0 && W % r == 0, "area_down: shape");
-  ew::area_down_kernel<<<grid_of((long long)B * (H / r) * (W / r) * (C / 8)), 256, 0, s>>>(x, y, B, H, W, C, r);
+DEVA_B200_API int deva_b200_area_down(const void* x, void* y, int b, int h, int w, int c, int r, deva_stream_t stream) {
+  B200_REQUIRE(c % 8 == 0 && h % r == 0 && w % r == 0, "area_down: shape");
+  ew::area_down_kernel<<<grid_of((long long)b * (h / r) * (w / r) * (c / 8)), 256, 0, S(stream)>>>(H(x), H(y), b, h, w, c, r);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_area_down_plane(const float* x, float* y, int B, int H, int W, int r, cudaStream_t s) {
-  B200_REQUIRE(H % r == 0 && W % r == 0, "area_down_plane: shape");
-  ew::area_down_plane_kernel<<<grid_of((long long)B * (H / r) * (W / r)), 256, 0, s>>>(x, y, B, H, W, r);
+DEVA_B200_API int deva_b200_area_down_plane(const float* x, float* y, int b, int h, int w, int r, deva_stream_t stream) {
+  B200_REQUIRE(h % r == 0 && w % r == 0, "area_down_plane: shape");
+  ew::area_down_plane_kernel<<<grid_of((long long)b * (h / r) * (w / r)), 256, 0, S(stream)>>>(x, y, b, h, w, r);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_cbam(const __half* x, const float* w1, const float* b1, const float* w2, const float* b2, const float* ws,
-            const float* bs, float* scratch, __half* raw, __half* relu, int B, int H, int W, int C, int R,
-            cudaStream_t s) {
+DEVA_B200_API int deva_b200_cbam(const void* x, const float* w1, const float* b1, const float* w2, const float* b2,
+                                 const float* ws, const float* bs, float* scratch, void* raw, void* relu, int b, int h,
+                                 int w, int c, int r, deva_stream_t stream) {
+  const __half* xh = H(x);
+  const cudaStream_t s = S(stream);
   // scratch: psum[B*16*C] | pmax[B*16*C] | gate[B*C] | stats[B*H*W*2]
   float* psum = scratch;
-  float* pmax = psum + (long long)B * ew::kPoolSplit * C;
-  float* gate = pmax + (long long)B * ew::kPoolSplit * C;
-  float* stats = gate + (long long)B * C;
-  const int HW = H * W;
-  B200_REQUIRE(C % 8 == 0 && C / 8 <= 256 && 256 % (C / 8) == 0, "cbam: C = %d must be 8 x a divisor of 256", C);
-  ew::cbam_pool_kernel<<<dim3(B, ew::kPoolSplit), 256, 0, s>>>(x, nullptr, psum, pmax, HW, C);
+  float* pmax = psum + (long long)b * ew::kPoolSplit * c;
+  float* gate = pmax + (long long)b * ew::kPoolSplit * c;
+  float* stats = gate + (long long)b * c;
+  const int HW = h * w;
+  B200_REQUIRE(c % 8 == 0 && c / 8 <= 256 && 256 % (c / 8) == 0, "cbam: C = %d must be 8 x a divisor of 256", c);
+  ew::cbam_pool_kernel<<<dim3(b, ew::kPoolSplit), 256, 0, s>>>(xh, nullptr, psum, pmax, HW, c);
   B200_LAUNCH_CHECK();
-  ew::cbam_mlp_kernel<<<B, 256, (2 * C + 2 * R) * sizeof(float), s>>>(psum, pmax, HW, w1, b1, w2, b2, gate, C, R);
+  ew::cbam_mlp_kernel<<<b, 256, (2 * c + 2 * r) * sizeof(float), s>>>(psum, pmax, HW, w1, b1, w2, b2, gate, c, r);
   B200_LAUNCH_CHECK();
-  const long long warps = (long long)B * HW;
-  ew::cbam_stats_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(x, nullptr, gate, stats, B, HW, C);
+  const long long warps = (long long)b * HW;
+  ew::cbam_stats_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(xh, nullptr, gate, stats, b, HW, c);
   B200_LAUNCH_CHECK();
-  ew::cbam_apply_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(x, gate, stats, ws, bs, raw, relu, B, H, W, C);
+  ew::cbam_apply_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(xh, gate, stats, ws, bs, H(raw), H(relu), b, h, w, c);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_cbam_split(const __half* x, const __half* x_lo, const float* w1, const float* b1, const float* w2, const float* b2,
-                  const float* ws, const float* bs, float* scratch, __half* raw, __half* raw_lo, __half* relu, __half* relu_lo,
-                  int pool_lo, int B, int H, int W, int C, int R, cudaStream_t s) {
+DEVA_B200_API int deva_b200_cbam_split(const void* x, const void* x_lo, const float* w1, const float* b1, const float* w2,
+                                       const float* b2, const float* ws, const float* bs, float* scratch, void* raw,
+                                       void* raw_lo, void* relu, void* relu_lo, int pool_lo, int b, int h, int w, int c,
+                                       int r, deva_stream_t stream) {
   // the gate statistics are pooled over x + x_lo as well: a gate error is common to every channel of a pixel, so it
   // does not average out in the next convolution the way independent roundings do
   B200_REQUIRE(x_lo && raw && raw_lo, "cbam_split: the hi/lo tensors are required");
+  const __half* xh = H(x);
+  const __half* xl = H(x_lo);
+  const cudaStream_t s = S(stream);
   float* psum = scratch;
-  float* pmax = psum + (long long)B * ew::kPoolSplit * C;
-  float* gate = pmax + (long long)B * ew::kPoolSplit * C;
-  float* stats = gate + (long long)B * C;
-  const int HW = H * W;
-  B200_REQUIRE(C % 8 == 0 && C / 8 <= 256 && 256 % (C / 8) == 0, "cbam_split: C = %d must be 8 x a divisor of 256", C);
-  ew::cbam_pool_kernel<<<dim3(B, ew::kPoolSplit), 256, 0, s>>>(x, pool_lo ? x_lo : nullptr, psum, pmax, HW, C);
+  float* pmax = psum + (long long)b * ew::kPoolSplit * c;
+  float* gate = pmax + (long long)b * ew::kPoolSplit * c;
+  float* stats = gate + (long long)b * c;
+  const int HW = h * w;
+  B200_REQUIRE(c % 8 == 0 && c / 8 <= 256 && 256 % (c / 8) == 0, "cbam_split: C = %d must be 8 x a divisor of 256", c);
+  ew::cbam_pool_kernel<<<dim3(b, ew::kPoolSplit), 256, 0, s>>>(xh, pool_lo ? xl : nullptr, psum, pmax, HW, c);
   B200_LAUNCH_CHECK();
-  ew::cbam_mlp_kernel<<<B, 256, (2 * C + 2 * R) * sizeof(float), s>>>(psum, pmax, HW, w1, b1, w2, b2, gate, C, R);
+  ew::cbam_mlp_kernel<<<b, 256, (2 * c + 2 * r) * sizeof(float), s>>>(psum, pmax, HW, w1, b1, w2, b2, gate, c, r);
   B200_LAUNCH_CHECK();
-  const long long warps = (long long)B * HW;
-  ew::cbam_stats_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(x, pool_lo ? x_lo : nullptr, gate, stats, B, HW, C);
+  const long long warps = (long long)b * HW;
+  ew::cbam_stats_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(xh, pool_lo ? xl : nullptr, gate, stats, b, HW, c);
   B200_LAUNCH_CHECK();
-  ew::cbam_apply_split_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(x, x_lo, gate, stats, ws, bs, raw, raw_lo, relu,
-                                                                        relu_lo, B, H, W, C);
-  B200_LAUNCH_CHECK();
-  return 0;
-}
-int ew_gru(const __half* values, const __half* h, __half* out, long long pixels, int C, cudaStream_t s) {
-  B200_REQUIRE(C % 8 == 0, "gru: C %% 8");
-  ew::gru_kernel<<<grid_of(pixels * (C / 8)), 256, 0, s>>>(values, h, out, pixels, C);
+  ew::cbam_apply_split_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(xh, xl, gate, stats, ws, bs, H(raw), H(raw_lo),
+                                                                        H(relu), H(relu_lo), b, h, w, c);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_key_tail(const float* y, int ld, int Q, int CK, int n_parts, long long part_stride, float* key, float* shr,
-                float* sel, cudaStream_t s) {
+DEVA_B200_API int deva_b200_gru(const void* values, const void* h, void* out, int64_t pixels, int c,
+                                deva_stream_t stream) {
+  B200_REQUIRE(c % 8 == 0, "gru: C %% 8");
+  ew::gru_kernel<<<grid_of(pixels * (c / 8)), 256, 0, S(stream)>>>(H(values), H(h), H(out), pixels, c);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+DEVA_B200_API int deva_b200_key_tail(const float* y, int ld, int q, int ck, int n_parts, int64_t part_stride, float* key,
+                                     float* shrinkage, float* selection, deva_stream_t stream) {
   B200_REQUIRE(n_parts >= 1, "key_tail: n_parts %d", n_parts);
-  ew::key_tail_kernel<<<grid_of((long long)Q * CK), 256, 0, s>>>(y, ld, Q, CK, n_parts, part_stride, key, shr, sel);
+  ew::key_tail_kernel<<<grid_of((long long)q * ck), 256, 0, S(stream)>>>(y, ld, q, ck, n_parts, part_stride, key, shrinkage,
+                                                                         selection);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_sum_parts(const float* parts, int n_parts, long long part_stride, const __half* res, const __half* res_lo,
-                 __half* raw, __half* raw_lo, __half* relu, __half* relu_lo, long long n, cudaStream_t s) {
+DEVA_B200_API int deva_b200_sum_parts(const float* parts, int n_parts, int64_t part_stride, const void* res,
+                                      const void* res_lo, void* raw, void* raw_lo, void* relu, void* relu_lo, int64_t n,
+                                      deva_stream_t stream) {
   B200_REQUIRE(n_parts >= 1 && n % 8 == 0 && part_stride % 4 == 0 && (raw || relu), "sum_parts: bad shape");
-  ew::sum_parts_kernel<<<grid_of(n / 8), 256, 0, s>>>(parts, n_parts, part_stride, res, res_lo, raw, raw_lo, relu, relu_lo,
-                                                       n / 8);
+  ew::sum_parts_kernel<<<grid_of(n / 8), 256, 0, S(stream)>>>(parts, n_parts, part_stride, H(res), H(res_lo), H(raw),
+                                                              H(raw_lo), H(relu), H(relu_lo), n / 8);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_output_tail(const float* logits, float* agg, float* prob, float* logits_out, int K, int h, int w, cudaStream_t s) {
-  ew::aggregate_kernel<<<ceil_div(h * w, 256), 256, 0, s>>>(logits, agg, K, h * w);
+DEVA_B200_API int deva_b200_output_tail(const float* logits, float* agg, float* prob, float* logits_out, int k, int h,
+                                        int w, deva_stream_t stream) {
+  const cudaStream_t s = S(stream);
+  ew::aggregate_kernel<<<ceil_div(h * w, 256), 256, 0, s>>>(logits, agg, k, h * w);
   B200_LAUNCH_CHECK();
-  ew::up4_softmax_kernel<<<ceil_div(16ll * h * w, 256), 256, 0, s>>>(agg, prob, logits_out, K + 1, h, w);
-  B200_LAUNCH_CHECK();
-  return 0;
-}
-int ew_head_gather3x3(const float* z, float* out, float bias, int B, int H, int W, cudaStream_t s) {
-  ew::head_gather3x3_kernel<<<grid_of((long long)B * H * W), 256, 0, s>>>(z, out, bias, B, H, W);
+  ew::up4_softmax_kernel<<<ceil_div(16ll * h * w, 256), 256, 0, s>>>(agg, prob, logits_out, k + 1, h, w);
   B200_LAUNCH_CHECK();
   return 0;
 }
+DEVA_B200_API int deva_b200_head_gather3x3(const float* z, float* out, float bias, int b, int h, int w,
+                                           deva_stream_t stream) {
+  ew::head_gather3x3_kernel<<<grid_of((long long)b * h * w), 256, 0, S(stream)>>>(z, out, bias, b, h, w);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // extern "C"
+
 // ---------------------------------------------------------------- frame ingest / egress (SURVEY 8f-3)
+namespace b200 {
 namespace ew {
 // u8 [h, w, 3] -> fp32 [3, h, w]: ToTensor (x / 255) then Normalize ((x - mean) / std), IEEE divisions like torch
 __global__ void __launch_bounds__(256)
@@ -1056,6 +1087,9 @@ scores_to_ids_kernel(const int* __restrict__ sum, int c, long long n, const int*
   if (out_u8) out_u8[i] = (unsigned char)id;
   if (out_i64) out_i64[i] = id;
 }
+
+// prob_to_segments' shared-memory histogram takes 20 bytes per channel
+constexpr int kMaxSegmentChannels = DEVA_B200_MAX_SEGMENT_CHANNELS;
 
 // Result-saver egress: the same argmax as prob_to_ids_kernel, then per output pixel (each output optional)
 //   index u8 = (uint8)lut[k]; id image = bytes of rgb[k] (id % 256, id / 256 % 256, id / 65536, or 0 when the id is not
@@ -1196,72 +1230,87 @@ mask_gather_kernel(const unsigned char* __restrict__ src, int w, int out_h, int 
 }
 }  // namespace ew
 
-int ew_ingest_rgb8(const unsigned char* src, float* dst, int h, int w, const float* mean, const float* stdv, cudaStream_t s) {
+}  // namespace b200
+
+extern "C" {
+
+DEVA_B200_API int deva_b200_ingest_rgb8(const uint8_t* src, float* dst, int h, int w, const float mean[3],
+                                        const float stdv[3], deva_stream_t stream) {
   B200_REQUIRE(h > 0 && w > 0 && mean && stdv, "ingest_rgb8: bad arguments");
   const long long hw = (long long)h * w;
-  ew::ingest_rgb8_kernel<<<(unsigned)ceil_div(hw, 256ll), 256, 0, s>>>(src, dst, hw, mean[0], mean[1], mean[2], stdv[0],
-                                                                      stdv[1], stdv[2]);
+  ew::ingest_rgb8_kernel<<<(unsigned)ceil_div(hw, 256ll), 256, 0, S(stream)>>>(src, dst, hw, mean[0], mean[1], mean[2],
+                                                                              stdv[0], stdv[1], stdv[2]);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_ingest_rgb8_resize(const unsigned char* src, int h, int w, int out_h, int out_w, const int* x_idx,
-                          const float* x_w, int x_taps, const int* y_idx, const float* y_w, int y_taps, float* tmp,
-                          float* dst, int flip, const float* mean, const float* stdv, cudaStream_t s) {
+DEVA_B200_API int deva_b200_ingest_rgb8_resize(const uint8_t* src, int h, int w, int out_h, int out_w,
+                                               const int32_t* x_idx, const float* x_w, int x_taps, const int32_t* y_idx,
+                                               const float* y_w, int y_taps, float* scratch, float* dst, int flip,
+                                               const float mean[3], const float stdv[3], deva_stream_t stream) {
   B200_REQUIRE(h > 0 && w > 0 && out_h > 0 && out_w > 0 && x_taps > 0 && y_taps > 0 && x_idx && x_w && y_idx && y_w &&
-               tmp && mean && stdv, "ingest_rgb8_resize: bad arguments");
+               scratch && mean && stdv, "ingest_rgb8_resize: bad arguments");
+  const cudaStream_t s = S(stream);
   const long long n1 = (long long)h * out_w, n2 = 3ll * out_h * out_w;
-  ew::resize_rows_rgb8_kernel<<<(unsigned)ceil_div(n1, 256ll), 256, 0, s>>>(src, h, w, out_w, x_idx, x_w, x_taps, tmp,
+  ew::resize_rows_rgb8_kernel<<<(unsigned)ceil_div(n1, 256ll), 256, 0, s>>>(src, h, w, out_w, x_idx, x_w, x_taps, scratch,
                                                                             mean[0], mean[1], mean[2], stdv[0], stdv[1],
                                                                             stdv[2]);
   B200_LAUNCH_CHECK();
-  ew::resize_cols_kernel<<<(unsigned)ceil_div(n2, 256ll), 256, 0, s>>>(tmp, h, out_h, out_w, y_idx, y_w, y_taps, flip, dst);
+  ew::resize_cols_kernel<<<(unsigned)ceil_div(n2, 256ll), 256, 0, s>>>(scratch, h, out_h, out_w, y_idx, y_w, y_taps, flip,
+                                                                       dst);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_mask_nearest(const unsigned char* src, int h, int w, int out_h, int out_w, const int* x_idx, const int* y_idx,
-                    int flip, long long* dst, cudaStream_t s) {
+DEVA_B200_API int deva_b200_mask_nearest(const uint8_t* src, int h, int w, int out_h, int out_w, const int32_t* x_idx,
+                                         const int32_t* y_idx, int flip, int64_t* dst, deva_stream_t stream) {
   B200_REQUIRE(h > 0 && w > 0 && out_h > 0 && out_w > 0 && x_idx && y_idx, "mask_nearest: bad arguments");
   const long long n = (long long)out_h * out_w;
-  ew::mask_gather_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, s>>>(src, w, out_h, out_w, x_idx, y_idx, flip, dst);
+  ew::mask_gather_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, S(stream)>>>(src, w, out_h, out_w, x_idx, y_idx, flip,
+                                                                             reinterpret_cast<long long*>(dst));
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_prob_to_ids(const float* prob, int c, int h, int w, int out_h, int out_w, int flip, const int* lut,
-                   unsigned char* out_u8, long long* out_i64, cudaStream_t s) {
+DEVA_B200_API int deva_b200_prob_to_ids(const float* prob, int c, int h, int w, int out_h, int out_w, int flip,
+                                        const int32_t* lut, uint8_t* out_u8, int64_t* out_i64, deva_stream_t stream) {
   B200_REQUIRE(c >= 1 && h > 0 && w > 0 && out_h > 0 && out_w > 0 && (out_u8 || out_i64), "prob_to_ids: bad arguments");
   const long long n = (long long)out_h * out_w;
-  ew::prob_to_ids_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, s>>>(prob, c, h, w, out_h, out_w, flip, (float)h / out_h,
-                                                                     (float)w / out_w, lut, out_u8, out_i64);
+  ew::prob_to_ids_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, S(stream)>>>(
+      prob, c, h, w, out_h, out_w, flip, (float)h / out_h, (float)w / out_w, lut, out_u8,
+      reinterpret_cast<long long*>(out_i64));
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_prob_to_scores(const float* prob, int c, int h, int w, int out_h, int out_w, int flip, unsigned char* scores,
-                      int* sum, cudaStream_t s) {
+DEVA_B200_API int deva_b200_prob_to_scores(const float* prob, int c, int h, int w, int out_h, int out_w, int flip,
+                                           uint8_t* scores, int32_t* sum, deva_stream_t stream) {
   B200_REQUIRE(prob && c >= 1 && h > 0 && w > 0 && out_h > 0 && out_w > 0 && (scores || sum),
                "prob_to_scores: bad arguments");
   const long long n = (long long)out_h * out_w;
-  ew::prob_to_scores_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, s>>>(prob, c, h, w, out_h, out_w, flip,
-                                                                         (float)h / out_h, (float)w / out_w, scores, sum);
+  ew::prob_to_scores_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, S(stream)>>>(prob, c, h, w, out_h, out_w, flip,
+                                                                                 (float)h / out_h, (float)w / out_w, scores,
+                                                                                 sum);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_scores_to_ids(const int* sum, int c, int h, int w, const int* lut, unsigned char* out_u8, long long* out_i64,
-                     cudaStream_t s) {
+DEVA_B200_API int deva_b200_scores_to_ids(const int32_t* sum, int c, int h, int w, const int32_t* lut, uint8_t* out_u8,
+                                          int64_t* out_i64, deva_stream_t stream) {
   B200_REQUIRE(sum && c >= 1 && h > 0 && w > 0 && (out_u8 || out_i64), "scores_to_ids: bad arguments");
   const long long n = (long long)h * w;
-  ew::scores_to_ids_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, s>>>(sum, c, n, lut, out_u8, out_i64);
+  ew::scores_to_ids_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, S(stream)>>>(sum, c, n, lut, out_u8,
+                                                                               reinterpret_cast<long long*>(out_i64));
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_prob_to_segments(const float* prob, int c, int h, int w, int out_h, int out_w, const int* lut,
-                        const unsigned* rgb, const unsigned char* frame, unsigned char* out_u8, unsigned char* out_rgb,
-                        unsigned char* out_overlay, unsigned long long* counts, int* boxes, cudaStream_t s) {
+DEVA_B200_API int deva_b200_prob_to_segments(const float* prob, int c, int h, int w, int out_h, int out_w,
+                                             const int32_t* lut, const uint32_t* rgb, const uint8_t* frame,
+                                             uint8_t* out_u8, uint8_t* out_rgb, uint8_t* out_overlay, int64_t* counts,
+                                             int32_t* boxes, deva_stream_t stream) {
   B200_REQUIRE(c >= 1 && h > 0 && w > 0 && out_h > 0 && out_w > 0 && lut, "prob_to_segments: bad arguments");
-  B200_REQUIRE(c <= kMaxSegmentChannels, "prob_to_segments: %d channels, at most %d supported", c,
-               kMaxSegmentChannels);
+  B200_REQUIRE(c <= ew::kMaxSegmentChannels, "prob_to_segments: %d channels, at most %d supported", c,
+               ew::kMaxSegmentChannels);
   B200_REQUIRE((!out_rgb && !out_overlay) || rgb, "prob_to_segments: the id image and overlay need the rgb table");
   B200_REQUIRE(!out_overlay || frame, "prob_to_segments: the overlay needs the frame");
   B200_REQUIRE(!counts == !boxes, "prob_to_segments: counts and boxes are written together");
+  unsigned long long* counts_u64 = reinterpret_cast<unsigned long long*>(counts);
+  const cudaStream_t s = S(stream);
   const long long n = (long long)out_h * out_w;
   long long blocks = (n + 255) / 256;
   size_t smem = 0;
@@ -1269,19 +1318,20 @@ int ew_prob_to_segments(const float* prob, int c, int h, int w, int out_h, int o
     smem = 5ull * c * sizeof(int);
     blocks = std::min(blocks, 4ll * sm_count());  // fewer, longer-lived blocks amortise the per-block histogram
     B200_CUDA(cudaFuncSetAttribute(ew::prob_to_segments_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ew::segments_init_kernel<<<(unsigned)ceil_div(c, 256), 256, 0, s>>>(c, counts, boxes);
+    ew::segments_init_kernel<<<(unsigned)ceil_div(c, 256), 256, 0, s>>>(c, counts_u64, boxes);
     B200_LAUNCH_CHECK();
   }
   ew::prob_to_segments_kernel<<<(unsigned)blocks, 256, smem, s>>>(prob, c, h, w, out_h, out_w, (float)h / out_h,
                                                                    (float)w / out_w, lut, rgb, frame, out_u8, out_rgb,
-                                                                   out_overlay, counts, boxes);
+                                                                   out_overlay, counts_u64, boxes);
   B200_LAUNCH_CHECK();
   return 0;
 }
-int ew_transpose_append(const __half* src, __half* dst, long long ld_dst, int n, int C, cudaStream_t s) {
-  ew::transpose_append_kernel<<<dim3(ceil_div(n, 32), ceil_div(C, 32)), 256, 0, s>>>(src, dst, ld_dst, n, C);
+DEVA_B200_API int deva_b200_transpose_append(const void* src, void* dst, int64_t ld_dst, int n, int c,
+                                             deva_stream_t stream) {
+  ew::transpose_append_kernel<<<dim3(ceil_div(n, 32), ceil_div(c, 32)), 256, 0, S(stream)>>>(H(src), H(dst), ld_dst, n, c);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-}  // namespace b200
+}  // extern "C"

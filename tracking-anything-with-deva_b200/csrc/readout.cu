@@ -15,7 +15,6 @@
 
 #include "common.h"
 #include "ptx.cuh"
-#include "readout.h"
 #include "tmap.h"
 
 namespace b200 {
@@ -30,7 +29,8 @@ constexpr int CONSUMER_THREADS = 256;
 constexpr int THREADS = CONSUMER_THREADS + 32;
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 constexpr int GROUP_M = 16;
-constexpr int kListCapR = 32;  // row pitch of the top-k index / weight lists (== simtopk's kListCap)
+constexpr int kMaxGroups = DEVA_B200_MAX_GROUPS;  // objects per launch
+constexpr int kMaxPeers = 8;  // ranks of one NVLink box (scatter-reduce mode)
 
 struct Params {
   int m_tiles, n_tiles, k_blocks, tiles_per_group;
@@ -200,13 +200,13 @@ bucket_kernel(const int* __restrict__ idx, const float* __restrict__ w, int q, i
   const int q0 = tile * BN;
   const int nq = min(BN, q - q0);
   int* off = offsets + (long long)tile * (k_blocks + 1);
-  uint32_t* ent = entries + (long long)tile * BN * kListCapR;
+  uint32_t* ent = entries + (long long)tile * BN * kListCap;
   for (int i = threadIdx.x; i <= k_blocks; i += 256) hist[i] = 0;
   __syncthreads();
   const int total = nq * top_k;
   for (int i = threadIdx.x; i < total; i += 256) {
     const int ql = i / top_k, j = i - ql * top_k;
-    const long long e = (long long)(q0 + ql) * kListCapR + j;
+    const long long e = (long long)(q0 + ql) * kListCap + j;
     if (w[e] != 0.f) atomicAdd(&hist[idx[e] / BK + 1], 1);  // zero-weight entries (padding, other shards' slots) are dropped
   }
   __syncthreads();
@@ -217,11 +217,11 @@ bucket_kernel(const int* __restrict__ idx, const float* __restrict__ w, int q, i
   __syncthreads();
   for (int i = threadIdx.x; i < total; i += 256) {
     const int ql = i / top_k, j = i - ql * top_k;
-    if (w[(long long)(q0 + ql) * kListCapR + j] == 0.f) continue;
-    const int n = idx[(long long)(q0 + ql) * kListCapR + j];
+    if (w[(long long)(q0 + ql) * kListCap + j] == 0.f) continue;
+    const int n = idx[(long long)(q0 + ql) * kListCap + j];
     const int kb = n / BK;
     const int pos = atomicAdd(&hist[kb], 1);
-    const uint32_t hw = __half_as_ushort(__float2half_rn(w[(long long)(q0 + ql) * kListCapR + j]));
+    const uint32_t hw = __half_as_ushort(__float2half_rn(w[(long long)(q0 + ql) * kListCap + j]));
     ent[pos] = ((uint32_t)ql << 24) | ((uint32_t)(n - kb * BK) << 16) | hw;
   }
 }
@@ -234,7 +234,7 @@ struct SpParams {
   __half* out_tok;
   int rows_per_group;
   const int* offsets;        // [n_tiles][k_blocks + 1]
-  const uint32_t* entries;   // [n_tiles][BN * kListCapR]
+  const uint32_t* entries;   // [n_tiles][BN * kListCap]
   int val_row[kMaxGroups];
   int out_row[kMaxGroups];
   // scatter-reduce mode (bank-sharded read): group g's tile is ADDED (red.add over NVLink / locally) into the buffer
@@ -298,7 +298,7 @@ readout_sparse_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_co
       int m, n;
       tile_coords(tile, p.m_tiles, p.n_tiles, m, n);
       const int* off = p.offsets + (long long)n * (p.k_blocks + 1);
-      const uint32_t* ent = p.entries + (long long)n * BN * kListCapR;
+      const uint32_t* ent = p.entries + (long long)n * BN * kListCap;
       const int e0 = off[kb], cnt = off[kb + 1] - e0;
       uint32_t e_a = 0, e_b = 0;   // first 64 entries prefetched before the stage is free
       if (lane < cnt) e_a = ent[e0 + lane];
@@ -368,20 +368,26 @@ readout_sparse_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_co
 }
 
 }  // namespace readout
+}  // namespace b200
 
-int launch_readout(const __half* values, long long values_ld, long long values_rows, const int* val_row,
-                   const int* out_row, int n_groups, int rows_per_group, const __half* P, long long ldP,
-                   int n_window, int q, float* out, long long ldo, __half* out_tok, cudaStream_t stream) {
+using namespace b200;
+
+extern "C" {
+
+DEVA_B200_API int deva_b200_readout(const void* values, int64_t values_ld, int64_t values_rows, const int32_t* val_row,
+                                    const int32_t* out_row, int n_groups, int rows_per_group, const void* affinity,
+                                    int64_t ld_affinity, int n_window, int q, float* out, int64_t ld_out, void* out_tok,
+                                    deva_stream_t stream) {
   using namespace readout;
   B200_REQUIRE(n_groups >= 1 && n_groups <= kMaxGroups, "readout: n_groups %d out of range [1,%d]", n_groups,
                kMaxGroups);
   B200_REQUIRE(rows_per_group % BM == 0, "readout: rows_per_group %d must be a multiple of %d", rows_per_group, BM);
   B200_REQUIRE(n_window >= 1 && q >= 1, "readout: empty problem");
-  B200_REQUIRE(values_ld % 8 == 0 && ldP % 8 == 0, "readout: leading dimensions must be multiples of 8 halves");
+  B200_REQUIRE(values_ld % 8 == 0 && ld_affinity % 8 == 0, "readout: leading dimensions must be multiples of 8 halves");
   const char* err = nullptr;
   CUtensorMap map_v, map_p;
   if (make_tmap_2d(&map_v, TmapType::F16, values, n_window, values_rows, values_ld * 2, BK, BM, &err) ||
-      make_tmap_2d(&map_p, TmapType::F16, P, n_window, q, ldP * 2, BK, BN, &err)) {
+      make_tmap_2d(&map_p, TmapType::F16, affinity, n_window, q, ld_affinity * 2, BK, BN, &err)) {
     set_error("readout: %s", err ? err : "tensor map");
     return 3;
   }
@@ -391,9 +397,9 @@ int launch_readout(const __half* values, long long values_ld, long long values_r
   p.n_tiles = ceil_div(q, BN);
   p.k_blocks = ceil_div(n_window, BK);
   p.q = q;
-  p.ldo = ldo;
+  p.ldo = ld_out;
   p.out = out;
-  p.out_tok = out_tok;
+  p.out_tok = H(out_tok);
   p.rows_per_group = rows_per_group;
   for (int i = 0; i < n_groups; ++i) {
     p.val_row[i] = val_row[i];
@@ -407,31 +413,32 @@ int launch_readout(const __half* values, long long values_ld, long long values_r
   }
   const int total = p.m_tiles * p.n_tiles;
   const int grid = total < sm_count() ? total : sm_count();
-  readout_kernel<<<grid, THREADS, SMEM_BYTES, stream>>>(map_v, map_p, p);
+  readout_kernel<<<grid, THREADS, SMEM_BYTES, S(stream)>>>(map_v, map_p, p);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-}  // namespace b200
-
-namespace b200 {
-
-size_t readout_sparse_workspace_bytes(int q, int n_window) {
+DEVA_B200_API size_t deva_b200_readout_sparse_workspace_bytes(int q, int n_window) {
   const size_t n_tiles = (q + readout::BN - 1) / readout::BN;
   const size_t k_blocks = (n_window + readout::BK - 1) / readout::BK;
-  return n_tiles * ((k_blocks + 1) * 4 + (size_t)readout::BN * readout::kListCapR * 4) + 256;
+  return n_tiles * ((k_blocks + 1) * 4 + (size_t)readout::BN * kListCap * 4) + 256;
 }
 
-int launch_readout_sparse(const __half* values, long long values_ld, long long values_rows, const int* val_row,
-                          const int* out_row, int n_groups, int rows_per_group, const int* idx, const float* w,
-                          int top_k, int n_window, int q, void* workspace, float* out, long long ldo, __half* out_tok,
-                          cudaStream_t stream, const int* owner, float* const* rank_dst, int n_ranks) {
+}  // extern "C"
+
+// The plain and the scatter-reduce sparse read-out (rank_dst given: group g's tile is red.add'ed into
+// rank_dst[owner[g]] + out_row[g] * ld_out instead of stored to `out`).
+static int readout_sparse(const void* values, int64_t values_ld, int64_t values_rows, const int32_t* val_row,
+                          const int32_t* out_row, const int32_t* owner, int n_groups, int rows_per_group,
+                          const int32_t* idx, const float* w, int top_k, int n_window, int q, void* workspace, float* out,
+                          float* const* rank_dst, int n_ranks, int64_t ld_out, void* out_tok, deva_stream_t stream) {
   using namespace readout;
+  const cudaStream_t s = S(stream);
   B200_REQUIRE(!rank_dst || (owner && n_ranks >= 1 && n_ranks <= kMaxPeers && !out_tok),
                "readout: scatter-reduce needs owners and 1..%d destination ranks", kMaxPeers);
   B200_REQUIRE(n_groups >= 1 && n_groups <= kMaxGroups, "readout: n_groups %d out of range [1,%d]", n_groups, kMaxGroups);
   B200_REQUIRE(rows_per_group % BM == 0, "readout: rows_per_group %d must be a multiple of %d", rows_per_group, BM);
-  B200_REQUIRE(n_window >= 1 && q >= 1 && top_k >= 1 && top_k <= kListCapR, "readout: bad shape");
+  B200_REQUIRE(n_window >= 1 && q >= 1 && top_k >= 1 && top_k <= kListCap, "readout: bad shape");
   B200_REQUIRE(values_ld % 8 == 0, "readout: leading dimension must be a multiple of 8 halves");
   const char* err = nullptr;
   CUtensorMap map_v;
@@ -444,7 +451,7 @@ int launch_readout_sparse(const __half* values, long long values_ld, long long v
   p.m_tiles = n_groups * p.tiles_per_group;
   p.n_tiles = ceil_div(q, BN);
   p.k_blocks = ceil_div(n_window, BK);
-  p.q = q; p.ldo = ldo; p.out = out; p.out_tok = out_tok; p.rows_per_group = rows_per_group;
+  p.q = q; p.ldo = ld_out; p.out = out; p.out_tok = H(out_tok); p.rows_per_group = rows_per_group;
   int* offsets = reinterpret_cast<int*>(workspace);
   uint32_t* entries = reinterpret_cast<uint32_t*>(offsets + (size_t)p.n_tiles * (p.k_blocks + 1));
   p.offsets = offsets; p.entries = entries;
@@ -467,13 +474,34 @@ int launch_readout_sparse(const __half* values, long long values_ld, long long v
     B200_CUDA(cudaFuncSetAttribute(bucket_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     configured = true;
   }
-  bucket_kernel<<<p.n_tiles, 256, (p.k_blocks + 1) * sizeof(int), stream>>>(idx, w, q, top_k, p.k_blocks, offsets, entries);
+  bucket_kernel<<<p.n_tiles, 256, (p.k_blocks + 1) * sizeof(int), s>>>(idx, w, q, top_k, p.k_blocks, offsets, entries);
   B200_LAUNCH_CHECK();
   const int total = p.m_tiles * p.n_tiles;
   const int grid = total < sm_count() ? total : sm_count();
-  readout_sparse_kernel<<<grid, SP_THREADS, SP_SMEM, stream>>>(map_v, p);
+  readout_sparse_kernel<<<grid, SP_THREADS, SP_SMEM, s>>>(map_v, p);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-}  // namespace b200
+extern "C" {
+
+DEVA_B200_API int deva_b200_readout_sparse(const void* values, int64_t values_ld, int64_t values_rows,
+                                           const int32_t* val_row, const int32_t* out_row, int n_groups,
+                                           int rows_per_group, const int32_t* idx, const float* w, int top_k,
+                                           int n_window, int q, void* workspace, float* out, int64_t ld_out,
+                                           void* out_tok, deva_stream_t stream) {
+  return readout_sparse(values, values_ld, values_rows, val_row, out_row, nullptr, n_groups, rows_per_group, idx, w, top_k,
+                        n_window, q, workspace, out, nullptr, 0, ld_out, out_tok, stream);
+}
+
+DEVA_B200_API int deva_b200_readout_sparse_scatter(const void* values, int64_t values_ld, int64_t values_rows,
+                                                   const int32_t* val_row, const int32_t* out_row,
+                                                   const int32_t* owner, int n_groups, int rows_per_group,
+                                                   const int32_t* idx, const float* w, int top_k, int n_window, int q,
+                                                   void* workspace, float* const* rank_dst, int n_ranks,
+                                                   int64_t ld_out, deva_stream_t stream) {
+  return readout_sparse(values, values_ld, values_rows, val_row, out_row, owner, n_groups, rows_per_group, idx, w, top_k,
+                        n_window, q, workspace, nullptr, rank_dst, n_ranks, ld_out, nullptr, stream);
+}
+
+}  // extern "C"

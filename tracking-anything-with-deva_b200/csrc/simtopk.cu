@@ -19,12 +19,13 @@
 
 #include "common.h"
 #include "ptx.cuh"
-#include "simtopk.h"
 #include "tmap.h"
 
 namespace b200 {
 namespace simtopk {
 
+constexpr int kMaxSplit = 4;        // max CTAs sharing one 64-query tile along the memory axis
+constexpr int kMaxMergeLists = 16;  // candidate lists per query of one merge
 constexpr int BQ = 64, BNK = 64, BK = 64;
 constexpr int QTILE_BYTES = BQ * 128;   // 64 query rows x 64 halves
 constexpr int KTILE_BYTES = BNK * 128;  // 64 key rows x 64 halves
@@ -477,24 +478,35 @@ static int choose_split(int q_tiles, int tiles, int max_split) {
   return best;
 }
 
-size_t simtopk_workspace_bytes(int q) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+DEVA_B200_API size_t deva_b200_simtopk_workspace_bytes(int q) {
   const size_t qpad = (size_t)ceil_div(q, simtopk::BQ) * simtopk::BQ;
-  return (size_t)kMaxSplit * simtopk::LISTS * kListCap * qpad * 8;
+  return (size_t)simtopk::kMaxSplit * simtopk::LISTS * kListCap * qpad * 8;
 }
 
-int launch_sim_topk(const __half* k_hi, const __half* k_lo, const float* neg_s, int n_window, int n_lead,
-                    const __half* q_hi, const __half* q_lo, const float* bsq, int q, int ck, int top_k,
-                    void* workspace, int* out_idx, float* out_w, __half* P, long long ldP, float* use_cnt,
-                    float* life_cnt, int n_long, int count_long, int count_work, float* out_sim, const int* prev_idx,
-                    float* thr_ws, cudaStream_t stream) {
+// k_hi/k_lo [n_window, 2*ck] and q_hi/q_lo [q, 2*ck]: the packed rows written by deva_b200_pack_keys /
+// deva_b200_pack_query.
+DEVA_B200_API int deva_b200_sim_topk(const void* k_hi, const void* k_lo, const float* neg_s, int n_window, int n_lead,
+                                     const void* q_hi, const void* q_lo, const float* bsq, int q, int ck, int top_k,
+                                     void* workspace, int32_t* out_idx, float* out_w, void* affinity, int64_t ld_affinity,
+                                     float* use_cnt, float* life_cnt, int n_long, int count_long, int count_work,
+                                     float* out_sim, const int32_t* prev_idx, float* thr_ws, deva_stream_t stream) {
   using namespace simtopk;
+  const __half *kh = H(k_hi), *kl = H(k_lo), *qh = H(q_hi), *ql = H(q_lo);
+  __half* P = H(affinity);
+  const cudaStream_t s = S(stream);
   B200_REQUIRE(ck == 32 || ck == 64, "simtopk: key_dim %d unsupported (32 or 64)", ck);
   B200_REQUIRE(top_k >= 1 && top_k <= kListCap, "simtopk: top_k %d out of range [1,%d]", top_k, kListCap);
   B200_REQUIRE(n_window - n_lead >= top_k, "simtopk: top_k %d exceeds the %d memory slots (the reference raises too)",
                top_k, n_window - n_lead);
   B200_REQUIRE(q >= 1 && n_lead >= 0 && n_lead < 8, "simtopk: bad q / n_lead");
   CUtensorMap maps[4];
-  if (int rc = make_maps(maps, q_hi, q_lo, q, k_hi, k_lo, n_window, ck)) return rc;
+  if (int rc = make_maps(maps, qh, ql, q, kh, kl, n_window, ck)) return rc;
   Params p{};
   p.q = q; p.n_window = n_window; p.n_lead = n_lead; p.kblocks = 2 * ck / 64; p.top_k = top_k;
   p.tiles_total = ceil_div(n_window, BNK);
@@ -513,18 +525,18 @@ int launch_sim_topk(const __half* k_hi, const __half* k_lo, const float* neg_s, 
     B200_CUDA(cudaFuncSetAttribute(simtopk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     configured = true;
   }
-  if (P) B200_CUDA(cudaMemsetAsync(P, 0, (size_t)q * ldP * sizeof(__half), stream));
+  if (P) B200_CUDA(cudaMemsetAsync(P, 0, (size_t)q * ld_affinity * sizeof(__half), s));
   if (prev_idx) {
     B200_REQUIRE(thr_ws != nullptr, "simtopk: prev_idx needs the thr_ws scratch ([q] floats)");
-    thr_floor_kernel<<<ceil_div(q, 8), 256, 0, stream>>>(prev_idx, top_k, q, n_lead, n_window, 2 * ck, k_hi, neg_s, q_hi, bsq,
-                                                         thr_ws);
+    thr_floor_kernel<<<ceil_div(q, 8), 256, 0, s>>>(prev_idx, top_k, q, n_lead, n_window, 2 * ck, kh, neg_s, qh, bsq,
+                                                    thr_ws);
     B200_LAUNCH_CHECK();
     p.thr_floor = thr_ws;
   }
-  simtopk_kernel<false><<<dim3(q_tiles, nsplit), THREADS, SMEM_BYTES, stream>>>(maps[0], maps[1], maps[2], maps[3], p);
+  simtopk_kernel<false><<<dim3(q_tiles, nsplit), THREADS, SMEM_BYTES, s>>>(maps[0], maps[1], maps[2], maps[3], p);
   B200_LAUNCH_CHECK();
-  merge_kernel<<<ceil_div(q, MERGE_WARPS), MERGE_WARPS * 32, 0, stream>>>(
-      p.part_val, p.part_idx, nsplit * LISTS, top_k, q, p.qpad, out_idx, out_w, P, ldP, use_cnt, n_long, count_long,
+  merge_kernel<<<ceil_div(q, MERGE_WARPS), MERGE_WARPS * 32, 0, s>>>(
+      p.part_val, p.part_idx, nsplit * LISTS, top_k, q, p.qpad, out_idx, out_w, P, ld_affinity, use_cnt, n_long, count_long,
       count_work, out_sim);
   B200_LAUNCH_CHECK();
   if (life_cnt) {
@@ -532,7 +544,7 @@ int launch_sim_topk(const __half* k_hi, const __half* k_lo, const float* neg_s, 
     const int lo = count_long ? n_lead : n_long;
     const int hi = count_work ? n_window : n_long;
     if (hi > lo) {
-      tick_kernel<<<ceil_div(hi - lo, 256), 256, 0, stream>>>(life_cnt + lo, hi - lo);
+      tick_kernel<<<ceil_div(hi - lo, 256), 256, 0, s>>>(life_cnt + lo, hi - lo);
       B200_LAUNCH_CHECK();
     }
   }
@@ -540,27 +552,33 @@ int launch_sim_topk(const __half* k_hi, const __half* k_lo, const float* neg_s, 
 }
 
 // Global top-k + softmax over `n_lists` candidate lists per query (layout [n_lists][kListCap][qpad], entries with
-// idx < 0 are empty): the cross-rank merge of a bank-sharded read, and the second stage of launch_sim_topk.
-int launch_merge_lists(const float* part_val, const int* part_idx, int n_lists, int top_k, int q, int qpad, int* out_idx,
-                       float* out_w, float* out_sim, cudaStream_t stream) {
+// idx < 0 are empty): the cross-rank merge of a bank-sharded read, and the second stage of deva_b200_sim_topk.
+DEVA_B200_API int deva_b200_merge_lists(const float* part_val, const int32_t* part_idx, int n_lists, int top_k, int q,
+                                        int q_pitch, int32_t* out_idx, float* out_w, float* out_sim,
+                                        deva_stream_t stream) {
   using namespace simtopk;
+  const cudaStream_t s = S(stream);
   B200_REQUIRE(n_lists >= 1 && n_lists <= kMaxMergeLists, "merge: n_lists %d out of range [1,%d]", n_lists, kMaxMergeLists);
-  B200_REQUIRE(top_k >= 1 && top_k <= kListCap && q >= 1 && qpad >= q, "merge: bad shape");
-  merge_kernel<<<ceil_div(q, MERGE_WARPS), MERGE_WARPS * 32, 0, stream>>>(part_val, part_idx, n_lists, top_k, q, qpad, out_idx,
-                                                                         out_w, nullptr, 0, nullptr, 0, 0, 0, out_sim);
+  B200_REQUIRE(top_k >= 1 && top_k <= kListCap && q >= 1 && q_pitch >= q, "merge: bad shape");
+  merge_kernel<<<ceil_div(q, MERGE_WARPS), MERGE_WARPS * 32, 0, s>>>(part_val, part_idx, n_lists, top_k, q, q_pitch,
+                                                                    out_idx, out_w, nullptr, 0, nullptr, 0, 0, 0, out_sim);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-int launch_sim_dense_softmax(const __half* k_hi, const __half* k_lo, const float* neg_s, const float* shr,
-                             int n_window, int n_lead, const __half* q_hi, const __half* q_lo, const float* bsq,
-                             int q, int ck, float* sim_ws, long long ld_sim, __half* P, long long ldP, float* shr_out,
-                             cudaStream_t stream) {
+DEVA_B200_API int deva_b200_sim_dense_softmax(const void* k_hi, const void* k_lo, const float* neg_s,
+                                              const float* shrinkage, int n_window, int n_lead, const void* q_hi,
+                                              const void* q_lo, const float* bsq, int q, int ck, float* sim_ws,
+                                              int64_t ld_sim, void* affinity, int64_t ld_affinity, float* shr_out,
+                                              deva_stream_t stream) {
   using namespace simtopk;
+  const __half *kh = H(k_hi), *kl = H(k_lo), *qh = H(q_hi), *ql = H(q_lo);
+  __half* P = H(affinity);
+  const cudaStream_t s = S(stream);
   B200_REQUIRE(ck == 32 || ck == 64, "simdense: key_dim %d unsupported (32 or 64)", ck);
   B200_REQUIRE(q >= 1 && n_window > n_lead && n_lead >= 0 && n_lead < 8, "simdense: bad shape");
   CUtensorMap maps[4];
-  if (int rc = make_maps(maps, q_hi, q_lo, q, k_hi, k_lo, n_window, ck)) return rc;
+  if (int rc = make_maps(maps, qh, ql, q, kh, kl, n_window, ck)) return rc;
   Params p{};
   p.q = q; p.n_window = n_window; p.n_lead = n_lead; p.kblocks = 2 * ck / 64; p.top_k = 1;
   p.tiles_total = ceil_div(n_window, BNK);
@@ -578,11 +596,11 @@ int launch_sim_dense_softmax(const __half* k_hi, const __half* k_lo, const float
     B200_CUDA(cudaFuncSetAttribute(simtopk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     configured = true;
   }
-  simtopk_kernel<true><<<dim3(q_tiles, nsplit), THREADS, SMEM_BYTES, stream>>>(maps[0], maps[1], maps[2], maps[3], p);
+  simtopk_kernel<true><<<dim3(q_tiles, nsplit), THREADS, SMEM_BYTES, s>>>(maps[0], maps[1], maps[2], maps[3], p);
   B200_LAUNCH_CHECK();
-  row_softmax_kernel<<<q, 256, 0, stream>>>(sim_ws, ld_sim, n_window, shr, P, ldP, shr_out);
+  row_softmax_kernel<<<q, 256, 0, s>>>(sim_ws, ld_sim, n_window, shrinkage, P, ld_affinity, shr_out);
   B200_LAUNCH_CHECK();
   return 0;
 }
 
-}  // namespace b200
+}  // extern "C"
