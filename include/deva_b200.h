@@ -195,7 +195,7 @@ typedef struct deva_b200_conv_desc {
   float* out_f32;       /* optional fp32 NHWC output */
   void* out_raw_lo;     /* optional fp16 remainders (value - fp16(value)) of out_raw / out_relu */
   void* out_relu_lo;
-  const float* head_w;  /* optional fused 1x1 head on the ReLU'd fp32 result (needs cout_pad == nt): fp32 [head_n, cout] */
+  const float* head_w;  /* optional fused 1x1 head on the ReLU'd fp32 result (needs cout == cout_pad == nt, one of 64 / 128 / 192 / 256): fp32 [head_n, cout] */
   float* head_out;      /* fp32 [batch*ho*wo, head_n]: head_out[p, t] = sum_c relu(out[p, c]) * head_w[t, c] */
   int32_t head_n;       /* <= 9.  Folds MaskDecoder.pred (big_modules.py:189-190) into the last decoder conv. */
   /* optional fused gate epilogue (SensoryUpdater / SensoryDeepUpdater, modules.py:145-149,163-167): the conv output is

@@ -15,6 +15,8 @@ CASES = {
     'up84_c1_lo8': (16, 272, 480, 256, 256, 3, 'actlo8'),
     # what up_8_4.out_conv.c2 runs in the parity plan: the e4m3 correction pass, the residual as (hi, lo) and the fused head
     'up84_c2_parity': (16, 272, 480, 256, 256, 3, 'actlo8+res+head'),
+    # the same launch without the head: the difference to up84_c2_parity is what the fused head costs
+    'up84_c2_parity_nohead': (16, 272, 480, 256, 256, 3, 'actlo8+res'),
     'up84_c2_res': (16, 272, 480, 256, 256, 3, 'raw+res'),
     'up84_c2_head': (16, 272, 480, 256, 256, 3, 'raw+res+head'),
     'gru': (16, 68, 120, 512, 1536, 3, 'two'),

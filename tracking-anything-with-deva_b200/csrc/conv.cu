@@ -47,7 +47,11 @@ constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 static_assert(128 * PRODUCER_REGS + CONSUMER_THREADS * CONSUMER_REGS <= THREADS * 168, "conv: register budget");
 constexpr int kMaxTaps = 32;  // k-entries (filter tap x pass) of one launch
 constexpr int kMaxHead = 9;   // outputs of the fused 1x1 head
-constexpr int HEAD_BYTES = kMaxHead * 256 * 4;
+// Head weights in shared memory, per column pair (c, c + 1): the 9 taps' (w[t][c], w[t][c + 1]) side by side, padded to
+// 20 floats so that a pair's weights are 4 x 16 B + 8 B loads and the four pairs a quad reads at once (80 B apart) hit
+// disjoint banks.
+constexpr int kHeadPairStride = 20;
+constexpr int HEAD_BYTES = 128 * kHeadPairStride * 4;
 constexpr int kMaxBias = 2048;   // bias of the whole layer staged in shared memory (Cout_pad <= kMaxBias)
 constexpr int kMaxRank1 = 1024;  // same for the rank-1 input column
 constexpr int SMEM_BYTES = RING_BYTES + 256 + HEAD_BYTES + kMaxBias * 4 + kMaxRank1 * 4;
@@ -185,8 +189,8 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RING_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  float* s_head = reinterpret_cast<float*>(smem + RING_BYTES + 256);  // [kMaxHead][256] fused-head weights
-  float* s_bias = s_head + kMaxHead * 256;                            // [kMaxBias] bias of every output channel
+  float* s_head = reinterpret_cast<float*>(smem + RING_BYTES + 256);  // [128 pairs][kHeadPairStride] fused-head weights
+  float* s_bias = s_head + HEAD_BYTES / 4;                            // [kMaxBias] bias of every output channel
   float* s_r1w = s_bias + kMaxBias;                                   // [kMaxRank1] rank-1 column
 
   const int warp = threadIdx.x >> 5;
@@ -248,8 +252,9 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
   const int wg = warp >> 2;
   const int qd = lane & 3;  // column pair within each 8-column block of the fragment
   if constexpr (HEAD) {  // stage the head weights once per CTA, zero padded
-    for (int i = threadIdx.x; i < kMaxHead * 256; i += CONSUMER_THREADS) {
-      const int t = i / 256, ch = i - t * 256;
+    for (int i = threadIdx.x; i < HEAD_BYTES / 4; i += CONSUMER_THREADS) {
+      const int pr = i / kHeadPairStride, k = i - pr * kHeadPairStride;
+      const int t = k / 2, ch = 2 * pr + (k & 1);
       s_head[i] = (t < p.head_n && ch < p.cout) ? p.head_w[t * p.cout + ch] : 0.f;
     }
     named_bar_sync(1, CONSUMER_THREADS);
@@ -295,20 +300,83 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
 
     // thread holds rows r_i = wg*64 + (warp%4)*16 + lane/4 + 8i, columns 8j + 2*qd + {0, 1}
     const float acc_scale = p.acc_scale;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
+    struct Row {
+      bool live;
+      long long pix, off;  // pixel index; element offset of (pixel, n0) in the [pixels, cout] outputs
+      const __half* res;
+      const __half* res_lo;
+      float r1x;
+    };
+    auto row_at = [&](const int i) {
       const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
       const int ty = row / p.tw, tx = row - ty * p.tw;
       const int y = y0 + ty, x = x0 + tx;
-      const bool live = (y < p.ho) && (x < p.wo);
-      const long long pix = ((long long)b * p.ho + y) * p.wo + x;
-      const long long off = pix * p.cout + n0;
-      if constexpr (EPI == EPI_GATES) {
+      Row r;
+      r.live = (y < p.ho) && (x < p.wo);
+      r.pix = ((long long)b * p.ho + y) * p.wo + x;
+      r.off = r.pix * p.cout + n0;
+      r.res = p.res ? p.res + (p.res_batch_stride ? r.off : ((long long)y * p.wo + x) * p.cout + n0) : nullptr;
+      r.res_lo = p.res_lo ? p.res_lo + (r.res - p.res) : nullptr;
+      r.r1x = (p.rank1_x && r.live) ? p.rank1_x[r.pix] : 0.f;
+      return r;
+    };
+    // One column pair (8j + 2qd, +1) of row i: bias, rank-1 term and residual added, outputs written; returns the pair.
+    // `full`: the tile spans N existing channels of an even Cout, so the per-column bounds check and the
+    // element-by-element path drop out of the unrolled loop at compile time.
+    auto pair = [&](auto full_t, const Row& r, const int i, const int j) {
+      constexpr bool full = decltype(full_t)::value;
+      const int col = 8 * j + 2 * qd;
+      const int ch = n0 + col;
+      if (!full && (col >= p.nt || ch >= p.cout)) return make_float2(0.f, 0.f);
+      float v0 = d[4 * j + 2 * i] * acc_scale, v1 = d[4 * j + 2 * i + 1] * acc_scale;  // acc_scale: fp8 mode
+      if (full || even) {  // both channels exist (cout even, ch even): 4-byte fp16 pairs, 8-byte fp32 pairs
+        if (ks == 0) { v0 += s_bias[ch]; v1 += s_bias[ch + 1]; }
+        if (p.rank1_w) { v0 = fmaf(s_r1w[ch], r.r1x, v0); v1 = fmaf(s_r1w[ch + 1], r.r1x, v1); }
+        if (r.res) {
+          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(r.res + col));
+          v0 += f.x; v1 += f.y;
+        }
+        if (r.res_lo) {
+          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(r.res_lo + col));
+          v0 += f.x; v1 += f.y;
+        }
+        const long long e = r.off + col;
+        if (p.out_raw) {
+          const __half2 h = __floats2half2_rn(v0, v1);
+          *reinterpret_cast<__half2*>(p.out_raw + e) = h;
+          if (p.out_raw_lo) {
+            const float2 back = __half22float2(h);
+            *reinterpret_cast<__half2*>(p.out_raw_lo + e) = __floats2half2_rn(v0 - back.x, v1 - back.y);
+          }
+        }
+        if (p.out_relu) {
+          const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
+          const __half2 h = __floats2half2_rn(a0, a1);
+          *reinterpret_cast<__half2*>(p.out_relu + e) = h;
+          if (p.out_relu_lo) {
+            const float2 back = __half22float2(h);
+            *reinterpret_cast<__half2*>(p.out_relu_lo + e) = __floats2half2_rn(a0 - back.x, a1 - back.y);
+          }
+        }
+        if (p.out_relu_lo8)
+          *reinterpret_cast<uint16_t*>(p.out_relu_lo8 + e) = to_e4m3x2(lo8_value(v0), lo8_value(v1));
+        if (p.out_f32)
+          *reinterpret_cast<float2*>(p.out_f32 + ks * p.f32_split_stride + e) = make_float2(v0, v1);
+      } else {  // ragged channel count (e.g. Cout = 1, 129): element by element
+        v0 = finish_scalar(p, v0, ch, r.off + col, r.res, r.res_lo, col, r.r1x, ks);
+        if (ch + 1 < p.cout) v1 = finish_scalar(p, v1, ch + 1, r.off + col + 1, r.res, r.res_lo, col + 1, r.r1x, ks);
+      }
+      return make_float2(v0, v1);
+    };
+    if constexpr (EPI == EPI_GATES) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const Row r = row_at(i);
         // channel tile = [forget | update | new] x 64 for hidden channels hc0 .. hc0+63 (modules.py:145-149): the three
         // gates of hidden channel c sit in columns c, 64 + c, 128 + c, i.e. in the same thread
-        if (live) {
+        if (r.live) {
           const int hc0 = (n0 / 192) * 64;
-          const long long hoff = pix * p.gate_c + hc0;
+          const long long hoff = r.pix * p.gate_c + hc0;
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const int c = 8 * j + 2 * qd;
@@ -324,88 +392,61 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
             *reinterpret_cast<__half2*>(p.gate_out + hoff + c) = __floats2half2_rn(o[0], o[1]);
           }
         }
-      } else {
-        const __half* res = p.res ? p.res + (p.res_batch_stride ? off : ((long long)y * p.wo + x) * p.cout + n0)
-                                  : nullptr;
-        const __half* res_lo = p.res_lo ? p.res_lo + (res - p.res) : nullptr;
-        const float r1x = (p.rank1_x && live) ? p.rank1_x[pix] : 0.f;
-        float hacc[kMaxHead];
+      }
+    } else if constexpr (HEAD) {
+      // Logit head: 9 taps over the ReLU'd channels, fp32.  The host admits it only when the tile is the whole Cout and
+      // exactly N wide, so every column pair takes the full-width path.  Column pair outer, row inner: a pair's weights
+      // are loaded once for both rows.  Each row's running sums still take the pairs in ascending order, a1 before a0.
+      const Row rows[2] = {row_at(0), row_at(1)};
+      float hacc[2][kMaxHead];
 #pragma unroll
-        for (int t = 0; t < kMaxHead; ++t) hacc[t] = 0.f;
-        // One column pair (8j + 2qd, +1) of row i.  `full`: the tile spans N existing channels of an even Cout, so the
-        // per-column bounds check and the element-by-element path drop out of the unrolled loop at compile time.
-        auto pair = [&](auto full_t, const int j) {
-          constexpr bool full = decltype(full_t)::value;
-          const int col = 8 * j + 2 * qd;
-          const int ch = n0 + col;
-          if (!full && (col >= p.nt || ch >= p.cout)) return;
-          float v0 = d[4 * j + 2 * i] * acc_scale, v1 = d[4 * j + 2 * i + 1] * acc_scale;  // acc_scale: fp8 mode
-          if (full || even) {  // both channels exist (cout even, ch even): 4-byte fp16 pairs, 8-byte fp32 pairs
-            if (ks == 0) { v0 += s_bias[ch]; v1 += s_bias[ch + 1]; }
-            if (p.rank1_w) { v0 = fmaf(s_r1w[ch], r1x, v0); v1 = fmaf(s_r1w[ch + 1], r1x, v1); }
-            if (res) {
-              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res + col));
-              v0 += f.x; v1 += f.y;
-            }
-            if (res_lo) {
-              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res_lo + col));
-              v0 += f.x; v1 += f.y;
-            }
-            const long long e = off + col;
-            if (p.out_raw) {
-              const __half2 h = __floats2half2_rn(v0, v1);
-              *reinterpret_cast<__half2*>(p.out_raw + e) = h;
-              if (p.out_raw_lo) {
-                const float2 back = __half22float2(h);
-                *reinterpret_cast<__half2*>(p.out_raw_lo + e) = __floats2half2_rn(v0 - back.x, v1 - back.y);
-              }
-            }
-            if (p.out_relu) {
-              const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
-              const __half2 h = __floats2half2_rn(a0, a1);
-              *reinterpret_cast<__half2*>(p.out_relu + e) = h;
-              if (p.out_relu_lo) {
-                const float2 back = __half22float2(h);
-                *reinterpret_cast<__half2*>(p.out_relu_lo + e) = __floats2half2_rn(a0 - back.x, a1 - back.y);
-              }
-            }
-            if (p.out_relu_lo8)
-              *reinterpret_cast<uint16_t*>(p.out_relu_lo8 + e) = to_e4m3x2(lo8_value(v0), lo8_value(v1));
-            if (p.out_f32)
-              *reinterpret_cast<float2*>(p.out_f32 + ks * p.f32_split_stride + e) = make_float2(v0, v1);
-          } else {  // ragged channel count (e.g. Cout = 1, 129): element by element
-            v0 = finish_scalar(p, v0, ch, off + col, res, res_lo, col, r1x, ks);
-            if (ch + 1 < p.cout) v1 = finish_scalar(p, v1, ch + 1, off + col + 1, res, res_lo, col + 1, r1x, ks);
-          }
-          if constexpr (HEAD) {  // logit head: 9 taps over the ReLU'd channels, fp32, weights from shared memory
-            const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
+      for (int i = 0; i < 2; ++i)
 #pragma unroll
-            for (int t = 0; t < kMaxHead; ++t) {
-              const float2 w2 = *reinterpret_cast<const float2*>(s_head + t * 256 + col);
-              hacc[t] = fmaf(a0, w2.x, fmaf(a1, w2.y, hacc[t]));
-            }
-          }
-        };
-        if (live) {
-          // (not with the fused head: its nine running sums leave no registers for a second copy of the loop)
-          if (!HEAD && even && p.nt == N && n0 + N <= p.cout) {  // every tile of the wide layers
+        for (int t = 0; t < kMaxHead; ++t) hacc[i][t] = 0.f;
 #pragma unroll
-            for (int j = 0; j < N / 8; ++j) pair(std::integral_constant<bool, !HEAD>{}, j);
+      for (int j = 0; j < N / 8; ++j) {
+        const float* hw = s_head + (4 * j + qd) * kHeadPairStride;  // pair (8j + 2qd) / 2
+        float w[2 * kMaxHead];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float4 f = reinterpret_cast<const float4*>(hw)[q];
+          w[4 * q] = f.x; w[4 * q + 1] = f.y; w[4 * q + 2] = f.z; w[4 * q + 3] = f.w;
+        }
+        const float2 f = reinterpret_cast<const float2*>(hw)[8];
+        w[16] = f.x; w[17] = f.y;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          if (!rows[i].live) continue;
+          const float2 v = pair(std::true_type{}, rows[i], i, j);
+          const float a0 = fmaxf(v.x, 0.f), a1 = fmaxf(v.y, 0.f);
+#pragma unroll
+          for (int t = 0; t < kMaxHead; ++t) hacc[i][t] = fmaf(a0, w[2 * t], fmaf(a1, w[2 * t + 1], hacc[i][t]));
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {  // the four threads of a quad hold the same pixel's partial sums over disjoint channels
+#pragma unroll
+        for (int t = 0; t < kMaxHead; ++t) {
+          hacc[i][t] += __shfl_xor_sync(0xffffffffu, hacc[i][t], 1);
+          hacc[i][t] += __shfl_xor_sync(0xffffffffu, hacc[i][t], 2);
+        }
+        if (rows[i].live && qd == 0) {
+#pragma unroll
+          for (int t = 0; t < kMaxHead; ++t)
+            if (t < p.head_n) p.head_out[rows[i].pix * p.head_n + t] = hacc[i][t];
+        }
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const Row r = row_at(i);
+        if (r.live) {
+          if (even && p.nt == N && n0 + N <= p.cout) {  // every tile of the wide layers
+#pragma unroll
+            for (int j = 0; j < N / 8; ++j) pair(std::true_type{}, r, i, j);
           } else {
 #pragma unroll
-            for (int j = 0; j < N / 8; ++j) pair(std::false_type{}, j);
-          }
-        }
-        if constexpr (HEAD) {  // the four threads of a quad hold the same pixel's partial sums over disjoint channels
-#pragma unroll
-          for (int t = 0; t < kMaxHead; ++t) {
-            hacc[t] += __shfl_xor_sync(0xffffffffu, hacc[t], 1);
-            hacc[t] += __shfl_xor_sync(0xffffffffu, hacc[t], 2);
-          }
-          if (live && qd == 0) {
-#pragma unroll
-            for (int t = 0; t < kMaxHead; ++t)
-              if (t < p.head_n) p.head_out[pix * p.head_n + t] = hacc[t];
+            for (int j = 0; j < N / 8; ++j) pair(std::false_type{}, r, i, j);
           }
         }
       }
@@ -533,8 +574,11 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
     p.gate_c = d.cout / 3;
   }
   if (d.head_w) {
-    B200_REQUIRE(d.cout_pad == d.nt && d.cout % 32 == 0 && d.cout <= 256 && d.head_n >= 1 && d.head_n <= kMaxHead && d.head_out,
-                 "conv: fused head needs the whole Cout (%d) in one channel tile and head_n <= %d", d.cout, kMaxHead);
+    // the head epilogue has only the full-width column loop: one tile of exactly N = 64 / 128 / 192 / 256 channels
+    B200_REQUIRE(d.cout == d.nt && d.cout_pad == d.nt && d.cout % 64 == 0 && d.cout <= 256 && d.head_n >= 1 &&
+                     d.head_n <= kMaxHead && d.head_out,
+                 "conv: fused head needs Cout (%d) = channel tile (%d) in {64, 128, 192, 256} and 1 <= head_n (%d) <= %d",
+                 d.cout, d.nt, d.head_n, kMaxHead);
     p.head_w = d.head_w; p.head_out = d.head_out; p.head_n = d.head_n;
   }
   // wgmma width: the channel tile rounded up to one of four instantiations.  TMA fills only nt weight rows of a stage;
