@@ -27,12 +27,13 @@
 extern "C" {
 #endif
 
-/* v14: deva_b200_prob_to_scores and deva_b200_scores_to_ids (multi-scale / flip score export and merge).
+/* v15: deva_b200_pano_joint_hist and deva_b200_pano_remap (video panoptic metrics and stuff merging).
+ * v14: deva_b200_prob_to_scores and deva_b200_scores_to_ids (multi-scale / flip score export and merge).
  * v13: deva_b200_prob_to_segments (the result savers' id map, id image, overlay, areas and boxes in one pass).
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 14
+#define DEVA_B200_ABI_VERSION 15
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -334,6 +335,29 @@ DEVA_B200_API int deva_b200_prob_to_scores(const float* prob, int c, int h, int 
  * [h, w] and/or out_i64 [h, w] (either may be NULL, not both). */
 DEVA_B200_API int deva_b200_scores_to_ids(const int32_t* sum, int c, int h, int w, const int32_t* lut, uint8_t* out_u8,
                                           int64_t* out_i64, deva_stream_t stream);
+
+
+/* ---- video panoptic metrics (deva/vps_metrics) -------------------------------------------------------------------
+ * Frames are RGB id images u8 [h, w, 3] with id = r + 256 g + 65536 b (the VIPSeg PNG encoding).  An id table is a
+ * sorted int32 array; a pixel's index is the position of its id in the table, or n (the table's length) when the id is
+ * not in it.  The tables live in shared memory: n_gt + n_pred (n_table + n_out) entries take at most 200 KiB.
+ *
+ * Joint label histogram of one ground-truth and one predicted frame, from which VPQ's intersections and areas
+ * (deva/vps_metrics/eval_vpq_vipseg.py:106-257) and STQ's confusion, tube areas and intersections
+ * (eval_stq_vipseg.py:123-151, segmentation_and_tracking_quality.py:111-195) are regroupings of cells:
+ * hist int32 [n_gt + 1, n_pred + 1], cell (i, j) = pixels whose gt index is i and pred index is j.  The call initialises
+ * hist.  A histogram that fits in shared memory next to the tables is kept per block there; a larger one is counted
+ * with global atomics. */
+DEVA_B200_API int deva_b200_pano_joint_hist(const uint8_t* gt, const uint8_t* pred, int h, int w, const int32_t* gt_ids,
+                                            int n_gt, const int32_t* pred_ids, int n_pred, int32_t* hist,
+                                            deva_stream_t stream);
+/* Stuff merging's id rewrite (deva/vps_metrics/stuff_merging.py:45-83): a pixel of pred index i takes the id
+ * out_ids[slot[i]] (slot int32 [n_table + 1]; slot[n_table] for ids not in the table), written to out u8 [h, w, 3] as
+ * bytes (id >> 8k) & 255.  counts int32 [n_out]: pixels written per slot; unknown int32 [1]: pixels whose id is not in the
+ * table.  The call initialises counts and unknown. */
+DEVA_B200_API int deva_b200_pano_remap(const uint8_t* pred, int h, int w, const int32_t* ids, int n_table,
+                                       const int32_t* slot, const int32_t* out_ids, int n_out, uint8_t* out,
+                                       int32_t* counts, int32_t* unknown, deva_stream_t stream);
 
 #ifdef __cplusplus
 }

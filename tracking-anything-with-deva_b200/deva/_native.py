@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 14
+ABI_VERSION = 15
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -107,6 +107,10 @@ _SIGNATURES = {
     'deva_b200_prob_to_scores': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                          c_void_p]),
     'deva_b200_scores_to_ids': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'deva_b200_pano_joint_hist': (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                          c_void_p]),
+    'deva_b200_pano_remap': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                     c_void_p, c_void_p, c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -399,6 +403,30 @@ def prob_to_scores(prob, c, h, w, out_h, out_w, flip, scores, total):
 def scores_to_ids(total, c, h, w, lut, out_u8, out_i64):
     _check(lib().deva_b200_scores_to_ids(_p(total), c, h, w, _p(lut), _p(out_u8), _p(out_i64), _stream()),
            'scores_to_ids')
+
+
+def pano_joint_hist(gt, pred, gt_ids, pred_ids, hist):
+    """gt, pred: uint8 [h, w, 3] RGB id frames; gt_ids, pred_ids: sorted int32 tables; hist: int32 [n_gt + 1, n_pred + 1]
+    (a view of a larger buffer is fine when it is contiguous)."""
+    h, w = gt.shape[:2]
+    assert gt.shape == pred.shape == (h, w, 3) and gt.dtype == pred.dtype == torch.uint8 and gt.is_contiguous() and \
+        pred.is_contiguous(), (gt.shape, pred.shape)
+    assert gt_ids.dtype == pred_ids.dtype == hist.dtype == torch.int32 and hist.is_contiguous()
+    assert hist.shape == (gt_ids.numel() + 1, pred_ids.numel() + 1), hist.shape
+    _check(lib().deva_b200_pano_joint_hist(_ptr(gt), _ptr(pred), h, w, _ptr(gt_ids), gt_ids.numel(), _ptr(pred_ids),
+                                           pred_ids.numel(), _ptr(hist), _stream()), 'pano_joint_hist')
+
+
+def pano_remap(pred, ids, slot, out_ids, out, counts, unknown):
+    """pred, out: uint8 [h, w, 3]; ids: sorted int32 table; slot: int32 [len(ids) + 1]; out_ids, counts: int32 [n_out];
+    unknown: int32 [1]."""
+    h, w = pred.shape[:2]
+    assert pred.shape == out.shape == (h, w, 3) and pred.dtype == out.dtype == torch.uint8
+    assert pred.is_contiguous() and out.is_contiguous()
+    assert ids.dtype == slot.dtype == out_ids.dtype == counts.dtype == unknown.dtype == torch.int32
+    assert slot.numel() == ids.numel() + 1 and counts.numel() == out_ids.numel()
+    _check(lib().deva_b200_pano_remap(_ptr(pred), h, w, _ptr(ids), ids.numel(), _ptr(slot), _ptr(out_ids),
+                                      out_ids.numel(), _ptr(out), _ptr(counts), _ptr(unknown), _stream()), 'pano_remap')
 
 
 def transpose_append(src, dst, ld_dst, n, c):
