@@ -27,13 +27,14 @@
 extern "C" {
 #endif
 
-/* v15: deva_b200_pano_joint_hist and deva_b200_pano_remap (video panoptic metrics and stuff merging).
+/* v16: deva_b200_label_areas and deva_b200_label_to_index (unsupervised DAVIS 2017 object limit).
+ * v15: deva_b200_pano_joint_hist and deva_b200_pano_remap (video panoptic metrics and stuff merging).
  * v14: deva_b200_prob_to_scores and deva_b200_scores_to_ids (multi-scale / flip score export and merge).
  * v13: deva_b200_prob_to_segments (the result savers' id map, id image, overlay, areas and boxes in one pass).
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 15
+#define DEVA_B200_ABI_VERSION 16
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -358,6 +359,23 @@ DEVA_B200_API int deva_b200_pano_joint_hist(const uint8_t* gt, const uint8_t* pr
 DEVA_B200_API int deva_b200_pano_remap(const uint8_t* pred, int h, int w, const int32_t* ids, int n_table,
                                        const int32_t* slot, const int32_t* out_ids, int n_out, uint8_t* out,
                                        int32_t* counts, int32_t* unknown, deva_stream_t stream);
+
+/* ---- label statistics and rewrite (deva/inference/postprocess_unsup_davis17.py) ----------------------------------
+ * A frame is u8 [h, w, channels] with channels 1 (the label is the byte: a P or L image) or 3 / 4 (the label is
+ * r << 16 | g << 8 | b, alpha ignored: postprocess_unsup_davis17.py:22-24).  Label 0 is background.
+ *
+ * Pixel count of every non-zero label of one frame.  labels / counts int32 [capacity] are the call's open-addressed table
+ * and then its result: once the work completes, state[0] = n and labels[0, n) / counts[0, n) are the frame's n distinct
+ * non-zero labels and their pixel counts, in no particular order.  If the frame has more than `capacity` distinct
+ * non-zero labels, state[0] = -1 and the lists are not valid: since the call does not synchronise, a capacity overflow
+ * is reported there, and the caller must check state[0] before it uses the lists (deva/_native.py raises).  state int32
+ * [2] (state[1] is scratch).  The call initialises all three. */
+DEVA_B200_API int deva_b200_label_areas(const uint8_t* frame, int h, int w, int channels, int capacity, int32_t* labels,
+                                        int32_t* counts, int32_t* state, deva_stream_t stream);
+/* out u8 [h, w]: (uint8)index[i] for a pixel whose label is labels[i], 0 for a label not in the table.  labels int32 [n]
+ * sorted ascending (distinct), index int32 [n]; 2 n entries take at most 200 KiB (shared memory). */
+DEVA_B200_API int deva_b200_label_to_index(const uint8_t* frame, int h, int w, int channels, const int32_t* labels,
+                                           const int32_t* index, int n, uint8_t* out, deva_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 15
+ABI_VERSION = 16
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -111,6 +111,9 @@ _SIGNATURES = {
                                           c_void_p]),
     'deva_b200_pano_remap': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,
                                      c_void_p, c_void_p, c_void_p]),
+    'deva_b200_label_areas': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'deva_b200_label_to_index': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                         c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -427,6 +430,41 @@ def pano_remap(pred, ids, slot, out_ids, out, counts, unknown):
     assert slot.numel() == ids.numel() + 1 and counts.numel() == out_ids.numel()
     _check(lib().deva_b200_pano_remap(_ptr(pred), h, w, _ptr(ids), ids.numel(), _ptr(slot), _ptr(out_ids),
                                       out_ids.numel(), _ptr(out), _ptr(counts), _ptr(unknown), _stream()), 'pano_remap')
+
+
+def _label_frame(frame):
+    """-> (h, w, channels) of a uint8 [h, w] or [h, w, 1 | 3 | 4] frame."""
+    assert frame.dtype == torch.uint8 and frame.is_contiguous() and frame.dim() in (2, 3), (frame.dtype, frame.shape)
+    return frame.shape[0], frame.shape[1], 1 if frame.dim() == 2 else frame.shape[2]
+
+
+def label_areas(frame, labels, counts, state):
+    """frame: uint8 [h, w] or [h, w, 3 | 4]; labels, counts: int32 [capacity]; state: int32 [2].  Enqueues the count; read
+    the result with ``label_areas_result``."""
+    h, w, c = _label_frame(frame)
+    assert labels.dtype == counts.dtype == state.dtype == torch.int32 and labels.numel() == counts.numel()
+    assert labels.is_contiguous() and counts.is_contiguous() and state.numel() == 2 and state.is_contiguous()
+    _check(lib().deva_b200_label_areas(_ptr(frame), h, w, c, labels.numel(), _ptr(labels), _ptr(counts), _ptr(state),
+                                       _stream()), 'label_areas')
+
+
+def label_areas_result(labels, counts, state):
+    """Host arrays of a completed label_areas call -> (labels, counts) [n]; raises when the frame had more distinct
+    labels than the table's capacity."""
+    n = int(state[0])
+    if n < 0:
+        raise RuntimeError(f'deva_b200.label_areas: the frame has more than {len(labels)} distinct labels (the table '
+                           f'capacity)')
+    return labels[:n], counts[:n]
+
+
+def label_to_index(frame, labels, index, out):
+    """frame: uint8 [h, w] or [h, w, 3 | 4]; labels: sorted int32 [n]; index: int32 [n]; out: uint8 [h, w]."""
+    h, w, c = _label_frame(frame)
+    assert labels.dtype == index.dtype == torch.int32 and labels.numel() == index.numel()
+    assert out.dtype == torch.uint8 and out.shape == (h, w) and out.is_contiguous(), (out.dtype, out.shape)
+    _check(lib().deva_b200_label_to_index(_ptr(frame), h, w, c, _ptr(labels), _ptr(index), labels.numel(), _ptr(out),
+                                          _stream()), 'label_to_index')
 
 
 def transpose_append(src, dst, ld_dst, n, c):

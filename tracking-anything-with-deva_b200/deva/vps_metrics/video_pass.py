@@ -7,15 +7,14 @@ initialise CUDA.
 """
 import json
 import os
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 from PIL import Image
 
+from deva.utils import png_pipeline
+from deva.utils.png_pipeline import RING, Uploader  # noqa: F401  (part of this module's interface)
 from deva.vps_metrics import scoring
-
-RING = 4  # pinned staging slots: a slot is refilled only after its previous upload has completed
 
 
 def read_rgb(path) -> np.ndarray:
@@ -26,42 +25,11 @@ def read_rgb(path) -> np.ndarray:
     return np.ascontiguousarray(a[:, :, :3])
 
 
-class Uploader:
-    """uint8 host arrays -> device tensors on the current stream, through pinned slots; never synchronises the device."""
-
-    def __init__(self, device):
-        self.device = device
-        self.slots = [None] * RING
-        self.i = 0
-
-    def __call__(self, a: np.ndarray) -> torch.Tensor:
-        k = self.i % RING
-        self.i += 1
-        n = a.size
-        slot = self.slots[k]
-        if slot is None or slot[0].numel() < n:
-            slot = (torch.empty(n, dtype=torch.uint8, pin_memory=True), torch.cuda.Event())
-            self.slots[k] = slot
-        host, done = slot
-        done.synchronize()
-        host[:n].numpy()[:] = a.reshape(-1)  # PIL's arrays are read-only: numpy copies without wrapping them
-        dev = torch.empty(a.shape, dtype=torch.uint8, device=self.device)
-        dev.view(-1).copy_(host[:n], non_blocking=True)
-        done.record()
-        return dev
-
-
-class Decoder:
-    """A pool of host threads decoding PNGs; ``frames(paths)`` yields arrays in order while later ones decode."""
+class Decoder(png_pipeline.Decoder):
+    """The thread pool decoding RGB id PNGs (read_rgb)."""
 
     def __init__(self, num_threads=None):
-        self.pool = ThreadPoolExecutor(max_workers=num_threads or min(16, os.cpu_count() or 1))
-
-    def frames(self, paths):
-        return self.pool.map(read_rgb, paths)
-
-    def close(self):
-        self.pool.shutdown()
+        super().__init__(read_rgb, num_threads)
 
 
 def require_device():
