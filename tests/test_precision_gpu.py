@@ -125,29 +125,84 @@ def test_fast_plan_is_still_available(golden_dir, synthetic_sd, monkeypatch):
     assert worst < 2.5e-3, worst
 
 
-@pytest.mark.parametrize('ksplit', [1, 4, 8])
-def test_conv_split_k_partial_sums(ksplit):
+@pytest.mark.parametrize('stride,cin,ksplit,n_parts', [
+    (1, 512, 1, 1), (1, 512, 4, 4), (1, 512, 8, 8),
+    (2, 128, 4, 4), (2, 256, 8, 8),        # stride 2: the four phase tensor maps, as layer2.0.c2 / layer3.0.c2
+    (1, 512, 5, 5), (1, 512, 7, 7),        # 216 k-iterations in chains of 44 / 31: boundaries inside a tap
+    (1, 128, 10, 9), (2, 128, 20, 18)])    # 54 k-iterations in chains of 6 / 3: the empty trailing splits are dropped
+def test_conv_split_k_partial_sums(stride, cin, ksplit, n_parts):
     """ksplit: the K loop runs as short accumulation chains whose fp32 partial sums the consumer adds - the result
     must equal the convolution (and, for a deep split-precision K loop, be closer to fp64 than one long chain: the tensor
-    core's accumulator rounds toward zero at every step)."""
+    core's accumulator rounds toward zero at every step).  A 3x3 split-precision conv has 3 x 9 x cin / 64 k-iterations;
+    ksplit asks for chains of ceil(k_iters / ksplit) of them, and only the non-empty chains are returned."""
     ops = _ops()
     g = torch.Generator(device='cuda').manual_seed(31)
-    b, h, w, cin, cout, k = 1, 30, 43, 512, 129, 3   # the key projection's shape: ragged Cout, one channel tile
+    b, h, w, cout, k = 1, 30, 43, 129, 3   # the key projection's shape: ragged Cout, one channel tile
     x = torch.randn(b, cin, h, w, device='cuda', generator=g)
     wgt = torch.randn(cout, cin, k, k, device='cuda', generator=g) / (cin * k * k)**0.5
     bias = torch.randn(cout, device='cuda', generator=g)
-    pc = ops.PackedConv(wgt, bias, 1, precise=True)
+    pc = ops.PackedConv(wgt, bias, stride, precise=True)
     xh, xl = _split(_nhwc(x))
-    ref = F.conv2d(x.double(), wgt.double(), bias.double(), padding=1)
+    ref = F.conv2d(x.double(), wgt.double(), bias.double(), stride=stride, padding=1)
     o = ops.conv_ex(xh, pc, x_lo=xl, want_f32=True, ksplit=ksplit)
     torch.cuda.synchronize()
     parts = o.f32 if ksplit > 1 else o.f32.unsqueeze(0)
-    assert parts.shape[0] == max(ksplit, 1)
+    assert parts.shape[0] == n_parts
     got = parts.double().sum(0).permute(0, 3, 1, 2)
     scale = float(ref.abs().max())
     err = float((got - ref).abs().max()) / scale
-    print(f'split-K {ksplit}: max rel err {err:.2e}')
+    print(f'split-K stride {stride} cin {cin} ksplit {ksplit} ({n_parts} parts): max rel err {err:.2e}')
     assert err < (5e-5 if ksplit == 1 else 5e-6), err  # one chain: the accumulator's round-toward-zero shows
+
+
+@pytest.mark.parametrize('b,h,w,cin,cout,k,stride,with_res', [
+    (1, 120, 216, 128, 128, 3, 2, False),   # pixel encoder layer2.0.c2 at 480p
+    (1, 60, 108, 256, 256, 3, 2, False),    # layer3.0.c2
+    (1, 30, 54, 256, 256, 3, 1, False),     # layer3.x.c2
+    (1, 30, 54, 1024, 512, 1, 1, False),    # proj1 / proj2
+    (1, 68, 120, 256, 256, 3, 1, False),    # layer3.x.c2 at 1080p
+    (1, 30, 54, 256, 256, 3, 1, True)])     # with a split residual
+def test_conv_auto_split_k(b, h, w, cin, cout, k, stride, with_res):
+    """A split-precision conv with more than MAX_CHAIN k-iterations and no fp32 output runs as chains of at most CHAIN
+    k-iterations finished by sum_parts.  Its (hi, lo) outputs must be (1) within 5e-6 of the fp64 convolution - at that
+    bound one dropped or doubled low-order k-iteration fails - and (2) bit-exact with the parts requested explicitly
+    (ksplit = ceil(k_iters / CHAIN)), added in fp32 in order, then res, then res_lo, and split into fp16 pairs."""
+    ops = _ops()
+    g = torch.Generator(device='cuda').manual_seed(41 + cin + h)
+    x = torch.randn(b, cin, h, w, device='cuda', generator=g)
+    wgt = torch.randn(cout, cin, k, k, device='cuda', generator=g) / (cin * k * k)**0.5
+    bias = torch.randn(cout, device='cuda', generator=g)
+    pc = ops.PackedConv(wgt, bias, stride, precise=True)
+    k_iters = k * k * (pc.cin_pad // 64) * 3
+    assert k_iters > ops.MAX_CHAIN
+    xh, xl = _split(_nhwc(x))
+    ref = F.conv2d(x.double(), wgt.double(), bias.double(), stride=stride, padding=k // 2)
+    res = res_lo = None
+    if with_res:
+        res, res_lo = _split(_nhwc(torch.randn(ref.shape, device='cuda', generator=g)))
+        ref = ref + _nchw(res).double() + _nchw(res_lo).double()
+    o = ops.conv_ex(xh, pc, x_lo=xl, res=res, res_lo=res_lo, want_raw=True, want_relu=True, want_lo=True)
+    torch.cuda.synchronize()
+    scale = float(ref.abs().max())
+    err_raw = float((_nchw(o.raw).double() + _nchw(o.raw_lo).double() - ref).abs().max()) / scale
+    err_relu = float((_nchw(o.relu).double() + _nchw(o.relu_lo).double() - ref.clamp_min(0)).abs().max()) / scale
+    print(f'auto split-K {h}x{w} {cin}->{cout} {k}x{k} s{stride} res={with_res}: max rel err raw {err_raw:.2e}, '
+          f'relu {err_relu:.2e} (bound 5e-6)')
+    assert err_raw < 5e-6 and err_relu < 5e-6, (err_raw, err_relu)
+    n_parts = -(-k_iters // ops.CHAIN)
+    parts = ops.conv_ex(xh, pc, x_lo=xl, want_f32=True, ksplit=n_parts).f32
+    torch.cuda.synchronize()
+    assert parts.shape[0] == n_parts
+    v = parts[0].clone()
+    for p in range(1, n_parts):
+        v = v + parts[p]
+    if with_res:
+        v = v + res.float()
+        v = v + res_lo.float()
+    for hi, lo, val in ((o.raw, o.raw_lo, v), (o.relu, o.relu_lo, v.clamp_min(0))):
+        want_hi = val.half()
+        assert torch.equal(hi, want_hi)
+        assert torch.equal(lo, (val - want_hi.float()).half())
 
 
 def _e4m3_bytes(x):
