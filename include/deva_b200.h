@@ -34,7 +34,7 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 16
+#define DEVA_B200_ABI_VERSION 17
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -217,6 +217,10 @@ typedef struct deva_b200_conv_desc {
                          * ceil(k_iters / ceil(k_iters / ksplit)) partial sums [part, batch, ho, wo, cout] (bias in part 0)
                          * for the consumer to add in fp32.  The tensor core's accumulator rounds toward zero at every
                          * accumulation step; short chains keep a split-precision convolution at fp32 accuracy. */
+  void* out_pool4;      /* optional fp16 NHWC [batch, ho/4, wo/4, cout]: 4x4 average of the raw (pre-ReLU) fp16 output,
+                         * equal to deva_b200_area_down(out_raw, 4) bit for bit.  Needs the staged epilogue (every channel
+                         * tile exactly 64 / 128 / 192 / 256 wide and cout == cout_pad, no fp32 output, no split-K), tile
+                         * sides th, tw and output sides ho, wo multiples of 4; other launches are refused. */
 } deva_b200_conv_desc;
 /* nn.Conv2d + folded BatchNorm (+ residual, + ReLU) as in deva/model/resnet.py:46-114, group_modules.py:41-67,
  * modules.py:22-39; `desc` is a HOST struct. */

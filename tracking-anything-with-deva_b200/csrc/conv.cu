@@ -16,6 +16,11 @@
 // Epilogue (straight from the accumulator registers): + bias (folded BatchNorm), + optional residual (own or
 //   batch-broadcast), + optional rank-1 term w1[cout] * x1[b, pixel] (the "+1" mask / logit input channel of
 //   sensory_compress and g4_conv), then writes any of: raw fp16, ReLU'd fp16, raw fp32.
+//   Staged form (full-width tiles, at most three 8/16-bit outputs): after a tile's k-iterations the producer fills
+//   N/64 more ring stages, one per 64-channel chunk, with the chunk's residual box (hi in the A slot, lo in the B slot)
+//   or, without a residual, reserves them.  The consumers read the residual from the stage, write their outputs into
+//   it in place and one thread drains them with TMA stores, which clip at the image edge.  Otherwise (ragged Cout,
+//   split-K fp32 partials, the gate epilogue, larger output sets) residuals are loaded and outputs stored per thread.
 // Warp roles: warps 0..7 = two consumer warpgroups (pixels 0..63 / 64..127 of the tile: wgmma m64nNk16 + epilogue),
 //   warps 8..11 = producer warpgroup, of which one thread issues the TMA loads.  The producer warpgroup exists so
 //   that setmaxnreg can hand its registers to the consumers (a 64 x 256 fp32 accumulator is 128 registers per
@@ -23,6 +28,9 @@
 //   consumers run the epilogue of the current one.
 #include <cuda_fp16.h>
 #include <stdlib.h>
+#include <string.h>
+
+#include <algorithm>
 
 #include <type_traits>
 
@@ -63,6 +71,7 @@ struct Params {
   int n_tiles, nt;
   int taps, cblocks;
   int m_tiles;   // batch * tiles_y * tiles_x
+  int units;     // m_tiles * n_tiles * ksplit work units (read from the parameter bank: no register held across a tile)
   signed char tap_map[kMaxTaps], tap_w[kMaxTaps], tap_dx[kMaxTaps], tap_dy[kMaxTaps];  // per k-entry: activation
                                                          // map, weight tap group, input offset
   const float* bias;
@@ -97,6 +106,13 @@ struct Params {
   int taps16, cblocks8;
   float acc_scale;
   uint8_t* out_relu_lo8;  // optional: e4m3 of (relu - fp16(relu)) * 4096, the low-order operand of the next fp8 pass
+  // staged epilogue: 1 = through the ring (see the file comment).  Each wanted output owns one 16 KB region of a stage:
+  // region 0 = the A slot (where the residual's hi part lands), 1 / 2 = the halves of the B slot (lo part in 1).  fp16
+  // regions hold the chunk as 128 rows of 128 B, 128B-swizzled like the residual box; the e4m3 region 64 B rows.
+  int staged;
+  __half* out_pool4;  // staged only: [batch, ho/4, wo/4, cout] 4x4 average of the raw output (raw staged, maybe not stored)
+  int store_mask;                                          // bit k: region k is stored through maps.out[k]
+  signed char reg_raw, reg_raw_lo, reg_relu, reg_relu_lo, reg_lo8;  // region of each output (when wanted)
 };
 
 struct Maps {
@@ -104,6 +120,8 @@ struct Maps {
   CUtensorMap wgt;        // box {64, nt}
   CUtensorMap act8;       // e4m3 low-order activations, box {128 B, tw, th}
   CUtensorMap wgt8;       // e4m3 weights, box {128 B, nt}
+  CUtensorMap res, res_lo;  // staged epilogue: residual (hi, lo) [B or 1, Ho, Wo, Cout], box {64, tw, th}
+  CUtensorMap out[3];       // staged epilogue: the output stored from region k, box {64, tw, th}
 };
 
 __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, const int (&c)[5]) {
@@ -195,7 +213,6 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int total_units = p.m_tiles * p.n_tiles * p.ksplit;
   const int k8 = (p.taps - p.taps16) * p.cblocks8;  // fp8 correction k-iterations come first ...
   const int k_iters = k8 + p.taps16 * p.cblocks;     // ... then the fp16 ones
   const uint32_t stage_tx = A_BYTES + p.nt * BK * 2;
@@ -223,7 +240,7 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
     if (threadIdx.x == CONSUMER_THREADS) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
+      for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
         int b, y0, x0, n0, ks;
         tile_decode(u, p, b, y0, x0, n0, ks);
         const int k_lo = ks * p.k_per_split, k_hi = min(k_iters, k_lo + p.k_per_split);
@@ -242,6 +259,21 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
           for (int cb = 0; cb < p.cblocks8; ++cb) issue(t, cb, true);
         for (int t = k_lo / p.cblocks; t < p.taps16 && t * p.cblocks < k_hi; ++t)
           for (int cb = max(0, k_lo - t * p.cblocks); cb < p.cblocks && t * p.cblocks + cb < k_hi; ++cb) issue(t, cb, false);
+        if (p.staged) {  // one stage per 64-channel chunk: its residual box, or a reservation for the outputs
+          const uint32_t res_tx = (p.res ? A_BYTES : 0) + (p.res_lo ? A_BYTES : 0);
+          for (int n = 0; n < p.nt; n += 64) {
+            mbar_wait(&empty[stage], phase ^ 1);
+            if (res_tx) {
+              const int c[5] = {n0 + n, x0, y0, p.res_batch_stride ? b : 0, 0};
+              mbar_expect_tx(&full[stage], res_tx);
+              if (p.res) tma_load_5d(sA + stage * A_BYTES, &maps.res, &full[stage], c);
+              if (p.res_lo) tma_load_5d(sB + stage * B_BYTES_MAX, &maps.res_lo, &full[stage], c);
+            } else {
+              mbar_arrive(&full[stage]);
+            }
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          }
+        }
       }
     }
     return;
@@ -264,7 +296,7 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
   float d[N / 2];
   int stage = 0;
   uint32_t phase = 0;
-  for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
+  for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
     int b, y0, x0, n0, ks;
     tile_decode(u, p, b, y0, x0, n0, ks);
     const int k_lo = ks * p.k_per_split;
@@ -368,6 +400,152 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
       }
       return make_float2(v0, v1);
     };
+    if constexpr (EPI != EPI_GATES) {
+      if (p.staged) {
+        // Row i of this thread: tile row r, its pixel index (-1 past the image edge).  Recomputed where it is used so
+        // that nothing but the accumulators and the head sums stays live across the chunks.
+        auto tile_row = [&](const int i) { return wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i; };
+        auto pixel = [&](const int i) {
+          const int r = tile_row(i), ty = r / p.tw, y = y0 + ty, x = x0 + r - ty * p.tw;
+          return (y < p.ho && x < p.wo) ? ((long long)b * p.ho + y) * p.wo + x : -1ll;
+        };
+        float r1x[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const long long pix = pixel(i);
+          r1x[i] = (p.rank1_x && pix >= 0) ? p.rank1_x[pix] : 0.f;
+        }
+        // Rows past the image edge read the zero fill and compute values that no store writes.
+        float hacc[2][HEAD ? kMaxHead : 1];
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int t = 0; t < (HEAD ? kMaxHead : 1); ++t) hacc[i][t] = 0.f;
+        int prev = 0;
+#pragma unroll
+        for (int c = 0; c < N / 64; ++c) {
+          mbar_wait(&full[stage], phase);
+          uint8_t* const slot_a = sA + stage * A_BYTES;
+          uint8_t* const slot_b = sB + stage * B_BYTES_MAX;
+          auto region = [&](const int k) { return k == 0 ? slot_a : slot_b + (k - 1) * A_BYTES; };
+#pragma unroll
+          for (int jl = 0; jl < 8; ++jl) {  // column block of the chunk; the thread reads and writes the same elements
+            const int j = 8 * c + jl;
+            float w[2 * kMaxHead];
+            if constexpr (HEAD) {
+              const float* hw = s_head + (4 * j + qd) * kHeadPairStride;
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const float4 f = reinterpret_cast<const float4*>(hw)[q];
+                w[4 * q] = f.x; w[4 * q + 1] = f.y; w[4 * q + 2] = f.z; w[4 * q + 3] = f.w;
+              }
+              const float2 f = reinterpret_cast<const float2*>(hw)[8];
+              w[16] = f.x; w[17] = f.y;
+            }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const int r = tile_row(i);
+              const uint32_t o16 = r * 128 + (((jl ^ (r & 7)) << 4) | (qd << 2));  // 128B swizzle: conflict-free
+              const int ch = n0 + 8 * j + 2 * qd;
+              float v0 = d[4 * j + 2 * i] * acc_scale, v1 = d[4 * j + 2 * i + 1] * acc_scale;
+              v0 += s_bias[ch]; v1 += s_bias[ch + 1];
+              if (p.rank1_w) { v0 = fmaf(s_r1w[ch], r1x[i], v0); v1 = fmaf(s_r1w[ch + 1], r1x[i], v1); }
+              if (p.res) {
+                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(slot_a + o16));
+                v0 += f.x; v1 += f.y;
+              }
+              if (p.res_lo) {
+                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(slot_b + o16));
+                v0 += f.x; v1 += f.y;
+              }
+              if (p.out_raw || p.out_pool4) {
+                const __half2 h = __floats2half2_rn(v0, v1);
+                *reinterpret_cast<__half2*>(region(p.reg_raw) + o16) = h;
+                if (p.out_raw_lo) {
+                  const float2 back = __half22float2(h);
+                  *reinterpret_cast<__half2*>(region(p.reg_raw_lo) + o16) = __floats2half2_rn(v0 - back.x, v1 - back.y);
+                }
+              }
+              const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
+              if (p.out_relu) {
+                const __half2 h = __floats2half2_rn(a0, a1);
+                *reinterpret_cast<__half2*>(region(p.reg_relu) + o16) = h;
+                if (p.out_relu_lo) {
+                  const float2 back = __half22float2(h);
+                  *reinterpret_cast<__half2*>(region(p.reg_relu_lo) + o16) = __floats2half2_rn(a0 - back.x, a1 - back.y);
+                }
+              }
+              if (p.out_relu_lo8)
+                *reinterpret_cast<uint16_t*>(region(p.reg_lo8) + r * 64 + 8 * jl + 2 * qd) =
+                    to_e4m3x2(lo8_value(v0), lo8_value(v1));
+              if constexpr (HEAD) {
+#pragma unroll
+                for (int t = 0; t < kMaxHead; ++t) hacc[i][t] = fmaf(a0, w[2 * t], fmaf(a1, w[2 * t + 1], hacc[i][t]));
+              }
+            }
+          }
+          fence_proxy_async();  // this thread's writes -> the TMA store's reads
+          named_bar_sync(1, CONSUMER_THREADS);
+          if (threadIdx.x == 0) {
+            const int cc[5] = {n0 + 64 * c, x0, y0, b, 0};
+            for (int k = 0; k < 3; ++k)
+              if (p.store_mask >> k & 1) tma_store_5d(&maps.out[k], region(k), cc);
+            bulk_commit();
+            if (c > 0) {  // the previous chunk's stores have read their stage: hand it back to the producer
+              bulk_wait_read<1>();
+              mbar_arrive(&empty[prev], CONSUMER_THREADS);
+            }
+          }
+          if (p.out_pool4) {
+            // 4x4 windows of the staged raw chunk in area_down_kernel's order (fp32 sum from 0 over dy, then dx, then
+            // * 1/16, one fp16 rounding), so the result is area_down(raw, 4) bit for bit.  The tile holds 8 windows;
+            // warp w takes window w, lane l its channel pair 2l: one 128-byte row per read, conflict-free.
+            const int win = threadIdx.x >> 5, pc = lane;
+            const int wy = win / (p.tw >> 2), wx = win - wy * (p.tw >> 2);
+            const uint8_t* raw = region(p.reg_raw);
+            float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+            for (int dy = 0; dy < 4; ++dy)
+#pragma unroll
+              for (int dx = 0; dx < 4; ++dx) {
+                const int r = (4 * wy + dy) * p.tw + 4 * wx + dx;
+                const float2 f = __half22float2(
+                    *reinterpret_cast<const __half2*>(raw + r * 128 + ((((pc >> 2) ^ (r & 7)) << 4) | ((pc & 3) << 2))));
+                s0 += f.x; s1 += f.y;
+              }
+            const int y = y0 + 4 * wy, x = x0 + 4 * wx;
+            if (y < p.ho && x < p.wo)  // ho, wo are multiples of 4: a window is wholly inside or wholly outside
+              *reinterpret_cast<__half2*>(
+                  p.out_pool4 + (((long long)b * (p.ho >> 2) + (y >> 2)) * (p.wo >> 2) + (x >> 2)) * p.cout + n0 + 64 * c + 2 * pc) =
+                  __floats2half2_rn(s0 * 0.0625f, s1 * 0.0625f);
+          }
+          prev = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+        if (p.out_pool4) named_bar_sync(1, CONSUMER_THREADS);  // every thread has read the last chunk for the pool
+        if (threadIdx.x == 0) {
+          bulk_wait_read<0>();
+          mbar_arrive(&empty[prev], CONSUMER_THREADS);
+        }
+        if constexpr (HEAD) {
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+#pragma unroll
+            for (int t = 0; t < kMaxHead; ++t) {
+              hacc[i][t] += __shfl_xor_sync(0xffffffffu, hacc[i][t], 1);
+              hacc[i][t] += __shfl_xor_sync(0xffffffffu, hacc[i][t], 2);
+            }
+            const long long pix = pixel(i);
+            if (pix >= 0 && qd == 0) {
+#pragma unroll
+              for (int t = 0; t < kMaxHead; ++t)
+                if (t < p.head_n) p.head_out[pix * p.head_n + t] = hacc[i][t];
+            }
+          }
+        }
+        continue;
+      }
+    }
     if constexpr (EPI == EPI_GATES) {
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
@@ -609,7 +787,7 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
   if (d.split_mode == 3) {
     const uint64_t k8 = (uint64_t)ktaps * d.cin_pad;  // bytes per weight row (cin_pad is a multiple of 128)
     if (make_tmap_act5_u8(&maps.act8, d.x_lo8, d.cin_pad, d.w, d.h, d.batch, (long long)d.cin_pad, (long long)d.w * d.cin_pad,
-                          (long long)d.h * d.w * d.cin_pad, d.tw, d.th, &err) ||
+                          (long long)d.h * d.w * d.cin_pad, 128, d.tw, d.th, &err) ||
         make_tmap_2d(&maps.wgt8, TmapType::U8, d.w8_packed, k8, d.cout_pad, k8, 128, d.nt, &err)) {
       set_error("conv: %s", err ? err : "fp8 tensor maps");
       return 3;
@@ -626,7 +804,65 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
   p.k_per_split = (k_iters_total + p.ksplit - 1) / p.ksplit;
   p.ksplit = (k_iters_total + p.k_per_split - 1) / p.k_per_split;  // no empty trailing split
   p.f32_split_stride = (long long)d.batch * ho * wo * d.cout;
+  // staged epilogue: every tile spans exactly N existing channels, fp16 / e4m3 outputs that fit the three regions of a
+  // stage, 16-byte aligned operands (TMA).  DEVA_B200_CONV_EPI=regs keeps the per-thread epilogue (A/B comparisons);
+  // DEVA_B200_CONV_EPI=staged refuses a launch that cannot take the staged one (tests).
+  {
+    const char* env = getenv("DEVA_B200_CONV_EPI");
+    const bool regs = env && strcmp(env, "regs") == 0, must = env && strcmp(env, "staged") == 0;
+    auto aligned = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    const bool pool = d.out_pool4 != nullptr;
+    // fp16 regions in order: raw (also staged, unstored, when only its pool is wanted), raw_lo, relu, relu_lo
+    const void* outs[4] = {d.out_raw, d.out_raw_lo, d.out_relu, d.out_relu_lo};
+    const bool used[4] = {d.out_raw || pool, d.out_raw_lo != nullptr, d.out_relu != nullptr, d.out_relu_lo != nullptr};
+    int n16 = 0;
+    for (int k = 0; k < 4; ++k) n16 += used[k] ? 1 : 0;
+    // the e4m3 region (64-byte rows) must not overlay a residual half that other threads have yet to read
+    const int r_lo8 = std::max({n16, d.res ? 1 : 0, d.res_lo ? 2 : 0});
+    // a low-order part without its fp16 output is written by neither epilogue form, so the staged one must not store it
+    const bool ok = !regs && !p.gate_out && p.ksplit == 1 && !d.out_f32 && d.nt == n_mma && d.cout == d.cout_pad &&
+                    (!d.res_lo || d.res) && !(d.out_raw_lo && !d.out_raw) && !(d.out_relu_lo && !d.out_relu) &&
+                    aligned(d.res) && aligned(d.res_lo) && aligned(d.out_raw) && aligned(d.out_raw_lo) &&
+                    aligned(d.out_relu) && aligned(d.out_relu_lo) && aligned(d.out_relu_lo8) && aligned(d.out_pool4) &&
+                    (d.out_relu_lo8 ? r_lo8 <= 2 : n16 <= 3);
+    B200_REQUIRE(ok || !(must || pool), "conv: %s needs the staged epilogue (full-width channel tiles, cout == cout_pad, "
+                 "no fp32 / split-K / gate outputs, outputs that fit a ring stage)%s", pool ? "out_pool4" : "DEVA_B200_CONV_EPI=staged",
+                 regs ? ", which DEVA_B200_CONV_EPI=regs turns off" : "");
+    B200_REQUIRE(!pool || (d.th % 4 == 0 && d.tw % 4 == 0 && ho % 4 == 0 && wo % 4 == 0),
+                 "conv: out_pool4 needs th, tw (%d, %d) and ho, wo (%d, %d) multiples of 4", d.th, d.tw, ho, wo);
+    if (ok) {
+      const long long cstr = d.cout, wstr = (long long)wo * d.cout, bstr = (long long)ho * wo * d.cout;
+      signed char* regs_of[4] = {&p.reg_raw, &p.reg_raw_lo, &p.reg_relu, &p.reg_relu_lo};
+      int rc = 0, k16 = 0;
+      for (int k = 0; k < 4; ++k) {
+        if (!used[k]) continue;
+        *regs_of[k] = (signed char)k16;
+        if (outs[k]) {
+          rc |= make_tmap_act5(&maps.out[k16], outs[k], d.cout, wo, ho, d.batch, cstr, wstr, bstr, d.tw, d.th, &err);
+          p.store_mask |= 1 << k16;
+        }
+        ++k16;
+      }
+      if (d.out_relu_lo8) {
+        p.reg_lo8 = (signed char)r_lo8;
+        rc |= make_tmap_act5_u8(&maps.out[r_lo8], d.out_relu_lo8, d.cout, wo, ho, d.batch, cstr, wstr, bstr, 64, d.tw, d.th,
+                                &err);
+        p.store_mask |= 1 << r_lo8;
+      }
+      const int rb = d.res_broadcast ? 1 : d.batch;
+      if (d.res) rc |= make_tmap_act5(&maps.res, d.res, d.cout, wo, ho, rb, cstr, wstr, bstr, d.tw, d.th, &err);
+      if (d.res_lo) rc |= make_tmap_act5(&maps.res_lo, d.res_lo, d.cout, wo, ho, rb, cstr, wstr, bstr, d.tw, d.th, &err);
+      if (rc) {
+        set_error("conv: %s", err ? err : "epilogue tensor maps");
+        return 3;
+      }
+      p.staged = 1;
+      p.out_pool4 = reinterpret_cast<__half*>(d.out_pool4);
+    }
+  }
   const long long units = (long long)p.m_tiles * p.n_tiles * p.ksplit;
+  B200_REQUIRE(units <= INT32_MAX, "conv: %lld work units", units);
+  p.units = (int)units;
   const int grid = (int)(units < sm_count() ? units : sm_count());
   kern<<<grid, THREADS, SMEM_BYTES, S(stream)>>>(maps, p);
   B200_LAUNCH_CHECK();

@@ -85,21 +85,22 @@ int make_tmap_f16_5d(CUtensorMap* out, const void* base, const uint64_t (&dims)[
 }
 
 int make_tmap_act5_u8(CUtensorMap* out, const void* base, uint64_t c, uint64_t w, uint64_t h, uint64_t b,
-                      long long stride_w, long long stride_h, long long stride_b, uint32_t box_w, uint32_t box_h,
-                      const char** err) {
+                      long long stride_w, long long stride_h, long long stride_b, uint32_t box_c, uint32_t box_w,
+                      uint32_t box_h, const char** err) {
   EncodeTiledFn fn = resolve_encode(err);
   if (!fn) return 1;
   const long long strides[4] = {stride_w, stride_h, stride_b, stride_b * (long long)b};
-  bool bad = (reinterpret_cast<uintptr_t>(base) & 15) != 0 || c < 128 || box_w == 0 || box_h == 0 || box_w > 256 || box_h > 256;
+  bool bad = (reinterpret_cast<uintptr_t>(base) & 15) != 0 || (box_c != 128 && box_c != 64) || c < box_c || box_w == 0 ||
+             box_h == 0 || box_w > 256 || box_h > 256;
   cuuint64_t gdim[5] = {c, w, h, b, 1}, gstride[4];
-  cuuint32_t bx[5] = {128, box_w, box_h, 1, 1}, estr[5] = {1, 1, 1, 1, 1};
+  cuuint32_t bx[5] = {box_c, box_w, box_h, 1, 1}, estr[5] = {1, 1, 1, 1, 1};
   for (int i = 0; i < 4; ++i) { gstride[i] = (cuuint64_t)strides[i]; bad |= (strides[i] & 15) != 0 || strides[i] <= 0; }
   if (bad) {
     if (err) *err = "make_tmap_act5_u8: bad alignment / box";
     return 2;
   }
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 5, const_cast<void*>(base), gdim, gstride, bx, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, box_c == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     if (err) *err = "cuTensorMapEncodeTiled(5d u8) failed";

@@ -21,10 +21,11 @@ int make_tmap_act5(CUtensorMap* out, const void* base, uint64_t c, uint64_t w, u
                    long long stride_w, long long stride_h, long long stride_b, uint32_t box_w, uint32_t box_h,
                    const char** err);
 
-// Same for an 8-bit (e4m3) activation tensor: dims (C bytes, W, H, B, 1), box (128, box_w, box_h, 1, 1), strides in bytes.
+// Same for an 8-bit (e4m3) tensor: dims (C bytes, W, H, B, 1), box (box_c, box_w, box_h, 1, 1), strides in bytes.
+// box_c 128: 128-byte swizzle (the wgmma operand layout); box_c 64: unswizzled 64-byte rows.
 int make_tmap_act5_u8(CUtensorMap* out, const void* base, uint64_t c, uint64_t w, uint64_t h, uint64_t b,
-                      long long stride_w, long long stride_h, long long stride_b, uint32_t box_w, uint32_t box_h,
-                      const char** err);
+                      long long stride_w, long long stride_h, long long stride_b, uint32_t box_c, uint32_t box_w,
+                      uint32_t box_h, const char** err);
 
 // General rank-5 fp16 tiled map, 128-byte swizzle: dims / box in elements, strides (dims 1..4) in elements.
 int make_tmap_f16_5d(CUtensorMap* out, const void* base, const uint64_t (&dims)[5], const long long (&strides)[4],

@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 16
+ABI_VERSION = 17
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -31,7 +31,7 @@ class ConvDesc(ctypes.Structure):
                 ('out_raw_lo', c_void_p), ('out_relu_lo', c_void_p),
                 ('head_w', c_void_p), ('head_out', c_void_p), ('head_n', c_int32),
                 ('gate_h', c_void_p), ('gate_out', c_void_p), ('x_lo8', c_void_p), ('w8_packed', c_void_p),
-                ('acc_scale', ctypes.c_float), ('out_relu_lo8', c_void_p), ('ksplit', c_int32)]
+                ('acc_scale', ctypes.c_float), ('out_relu_lo8', c_void_p), ('ksplit', c_int32), ('out_pool4', c_void_p)]
 
 
 _SIGNATURES = {
@@ -296,11 +296,11 @@ def _p(t):
 def conv2d(x, batch, h, w, cin_pad, w_packed, kh, stride, cout, cout_pad, nt, th, tw, bias, x2=None, x_lo=None, res=None,
            res_lo=None, res_broadcast=False, rank1_w=None, rank1_x=None, out_raw=None, out_relu=None, out_f32=None,
            out_raw_lo=None, out_relu_lo=None, head_w=None, head_out=None, head_n=0, gate_h=None, gate_out=None,
-           split_mode=0, ksplit=0, x_lo8=None, w8_packed=None, acc_scale=0.0, out_relu_lo8=None):
+           split_mode=0, ksplit=0, x_lo8=None, w8_packed=None, acc_scale=0.0, out_relu_lo8=None, out_pool4=None):
     d = ConvDesc(_p(x), _p(x2), _p(x_lo), split_mode, batch, h, w, cin_pad, _p(w_packed), kh, kh, stride, cout, cout_pad, nt, th, tw,
                  _p(bias), _p(res), _p(res_lo), int(res_broadcast), _p(rank1_w), _p(rank1_x), _p(out_raw), _p(out_relu),
                  _p(out_f32), _p(out_raw_lo), _p(out_relu_lo), _p(head_w), _p(head_out), head_n, _p(gate_h), _p(gate_out), _p(x_lo8), _p(w8_packed), acc_scale,
-                 _p(out_relu_lo8), ksplit)
+                 _p(out_relu_lo8), ksplit, _p(out_pool4))
     _check(lib().deva_b200_conv2d(ctypes.byref(d), _stream()), 'conv2d')
 
 

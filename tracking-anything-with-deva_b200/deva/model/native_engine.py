@@ -344,9 +344,10 @@ class NativeEngine:
                 y4 = self._C(q + '.c1', g4_relu, g4_relu_lo, want_relu=True, want_lo=tl(q + '.c2'),
                              want_relu_lo8=self._tl8(q + '.c2'))
                 # p4 = c2(...) + g4; the logit conv pred(relu(p4)) (big_modules.py:189-190) is folded in: the epilogue
-                # emits the 9 per-tap dot products in fp32, a 3x3 gather finishes the convolution.
+                # emits the 9 per-tap dot products in fp32, a 3x3 gather finishes the convolution.  p4 itself is only
+                # read 4x4-pooled by su.g4_conv, so the epilogue writes that pool instead of p4.
                 o4 = self._C(q + '.c2', y4.relu, y4.relu_lo8 if self._tl8(q + '.c2') else y4.relu_lo, res=g4_raw, res_lo=g4_lo,
-                             want_raw=True, head_w=self.pred_w)
+                             want_pool4=update_sensory, head_w=self.pred_w)
             else:
                 p16_raw, p16_relu = ops.conv(h, P[p + '.sensory_compress'], rank1_x=last[i:i + step].contiguous(),
                                              res=ro_all[i:i + step].contiguous(), want_raw=True, want_relu=True)
@@ -361,15 +362,14 @@ class NativeEngine:
                 y = ops.conv(g4_relu, P[q + '.c1'], want_relu=True)
                 # p4 = c2(...) + g4; the logit conv pred(relu(p4)) (big_modules.py:189-190) is folded in: the epilogue
                 # emits the 9 per-tap dot products in fp32, a 3x3 gather finishes the convolution.
-                o4 = ops.conv_ex(y, P[q + '.c2'], res=g4_raw, want_raw=True, head_w=self.pred_w)
-            p4_raw = o4.raw
+                o4 = ops.conv_ex(y, P[q + '.c2'], res=g4_raw, want_pool4=update_sensory, head_w=self.pred_w)
             logits = torch.empty(o4.head.shape[0], 4 * hh, 4 * ww, 1, dtype=torch.float32, device=o4.head.device)
             nat.head_gather3x3(o4.head, logits, self.pred_b, o4.head.shape[0], 4 * hh, 4 * ww)
             logits_all.append(logits)
             if update_sensory:
                 g = ops.conv(p16, P[p + '.su.g16_conv'], want_raw=True)
                 g = ops.conv(ops.area_down(p8, 2), P[p + '.su.g8_conv'], res=g, want_raw=True)
-                g = ops.conv(ops.area_down(p4_raw, 4), P[p + '.su.g4_conv'], res=g, want_raw=True,
+                g = ops.conv(o4.pool4, P[p + '.su.g4_conv'], res=g, want_raw=True,
                              rank1_x=ops.area_down_plane(logits.view(-1, 4 * hh, 4 * ww), 4))
                 hiddens.append(self._gru(p + '.gru', g, h))
         logits = logits_all[0] if len(logits_all) == 1 else torch.cat(logits_all, 0)

@@ -18,10 +18,13 @@ PROFILE = None  # set to a list by bench.py to collect (start event, end event, 
 _TILES = ((1, 128), (2, 64), (4, 32), (8, 16), (16, 8), (32, 4))
 
 
-def choose_tile(ho: int, wo: int) -> Tuple[int, int]:
-    """(th, tw) with th*tw = 128 that wastes the fewest MMA rows on an ho x wo output."""
+def choose_tile(ho: int, wo: int, pool4: bool = False) -> Tuple[int, int]:
+    """(th, tw) with th*tw = 128 that wastes the fewest MMA rows on an ho x wo output (``pool4``: among the tiles
+    whose sides are multiples of 4, which the epilogue's 4x4 pooling needs; the tile does not change any result)."""
     best, best_cost = None, None
     for th, tw in _TILES:
+        if pool4 and (th % 4 or tw % 4):
+            continue
         cost = -(-ho // th) * th * (-(-wo // tw) * tw)
         if best_cost is None or cost < best_cost or (cost == best_cost and tw > best[1]):
             best, best_cost = (th, tw), cost
@@ -132,10 +135,11 @@ class PackedConv:
 
 
 class ConvOut:
-    __slots__ = ('raw', 'raw_lo', 'relu', 'relu_lo', 'relu_lo8', 'f32', 'head', 'hidden')
+    __slots__ = ('raw', 'raw_lo', 'relu', 'relu_lo', 'relu_lo8', 'f32', 'head', 'hidden', 'pool4')
 
     def __init__(self):
         self.raw = self.raw_lo = self.relu = self.relu_lo = self.relu_lo8 = self.f32 = self.head = self.hidden = None
+        self.pool4 = None
 
 
 def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = None, x_lo: Optional[torch.Tensor] = None,
@@ -143,8 +147,17 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
             rank1_x: Optional[torch.Tensor] = None, want_raw: bool = False, want_relu: bool = False,
             want_f32: bool = False, want_lo: bool = False, head_w: Optional[torch.Tensor] = None,
             gate_h: Optional[torch.Tensor] = None, ksplit: int = 0, x_lo8: Optional[torch.Tensor] = None,
-            want_relu_lo8: bool = False) -> ConvOut:
-    """x fp16 NHWC [B,H,W,cin_pad] (+ x2: implicit channel concat, or + x_lo: split precision) -> ConvOut."""
+            want_relu_lo8: bool = False, want_pool4: bool = False) -> ConvOut:
+    """x fp16 NHWC [B,H,W,cin_pad] (+ x2: implicit channel concat, or + x_lo: split precision) -> ConvOut.
+    ``want_pool4``: ``pool4`` = area_down(raw, 4), pooled in the epilogue without writing ``raw`` unless it is wanted too."""
+    if want_pool4 and os.environ.get('DEVA_B200_CONV_EPI') == 'regs':  # the per-thread epilogue cannot pool (A/B runs)
+        o = conv_ex(x, pc, x2=x2, x_lo=x_lo, res=res, res_lo=res_lo, rank1_x=rank1_x, want_raw=True, want_relu=want_relu,
+                    want_f32=want_f32, want_lo=want_lo, head_w=head_w, gate_h=gate_h, ksplit=ksplit, x_lo8=x_lo8,
+                    want_relu_lo8=want_relu_lo8)
+        o.pool4 = area_down(o.raw, 4)
+        if not want_raw:
+            o.raw = o.raw_lo = None
+        return o
     assert x.dtype == torch.float16 and x.is_contiguous() and x.shape[-1] == pc.cin_pad, (x.shape, pc.cin_pad)
     assert (x2 is not None) == pc.two_inputs and (x_lo is not None) == pc.takes_lo, (x_lo is None, pc.takes_lo)
     assert (x_lo8 is not None) == pc.takes_lo8
@@ -155,7 +168,7 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
             assert other.dtype == torch.float16 and other.is_contiguous() and other.shape == x.shape
     b, h, w, _ = x.shape
     ho, wo = pc.out_hw(h, w)
-    th, tw = choose_tile(ho, wo)
+    th, tw = choose_tile(ho, wo, want_pool4)
     dev = x.device
 
     def new(dtype=torch.float16):
@@ -167,7 +180,7 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
     # (tools/accum_probe.py measures it).  Longer loops run as chains of <= CHAIN k-iterations
     # whose fp32 partial sums are added - with the bias, the residual and the output conversions - by sum_parts.
     k_iters = pc.k * pc.k * (pc.cin_pad // 64) * (3 if pc.precise else (2 if (pc.act_lo or pc.w_lo or pc.two_inputs) else 1))
-    if (pc.precise and ksplit == 0 and k_iters > MAX_CHAIN and not (want_f32 or head_w is not None or pc.rank1_w is not None)
+    if (pc.precise and ksplit == 0 and k_iters > MAX_CHAIN and not (want_f32 or want_pool4 or head_w is not None or pc.rank1_w is not None)
             and pc.cout % 8 == 0 and (res is None or res.shape[0] == b)):
         parts = conv_ex(x, pc, x_lo=x_lo, want_f32=True, ksplit=-(-k_iters // CHAIN)).f32
         o = ConvOut()
@@ -188,6 +201,8 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
         o.relu = new()
         o.relu_lo = new() if want_lo else None
         o.relu_lo8 = new(torch.uint8) if want_relu_lo8 else None
+    if want_pool4:
+        o.pool4 = torch.empty(b, ho // 4, wo // 4, pc.cout, dtype=torch.float16, device=dev)
     if want_f32:
         o.f32 = new(torch.float32)
         if ksplit > 1:  # fp32 partial sums [parts, b, ho, wo, cout] of a split K loop; the consumer adds them
@@ -220,7 +235,7 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
                rank1_x=rank1_x if pc.rank1_w is not None else None, out_raw=o.raw, out_relu=o.relu, out_f32=o.f32,
                out_raw_lo=o.raw_lo, out_relu_lo=o.relu_lo, head_w=head_w, head_out=o.head, head_n=head_n,
                gate_h=gate_h, gate_out=o.hidden, split_mode=pc.split_mode, ksplit=ksplit, x_lo8=x_lo8,
-               w8_packed=pc.w8_packed, acc_scale=pc.acc_scale, out_relu_lo8=o.relu_lo8)
+               w8_packed=pc.w8_packed, acc_scale=pc.acc_scale, out_relu_lo8=o.relu_lo8, out_pool4=o.pool4)
     if PROFILE is not None:
         ev1.record()
         flops = 2.0 * b * ho * wo * pc.cout * pc.k * pc.k * pc.cin * (2 if pc.two_inputs else 1)
