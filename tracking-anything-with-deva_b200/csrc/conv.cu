@@ -21,6 +21,10 @@
 //   or, without a residual, reserves them.  The consumers read the residual from the stage, write their outputs into
 //   it in place and one thread drains them with TMA stores, which clip at the image edge.  Otherwise (ragged Cout,
 //   split-K fp32 partials, the gate epilogue, larger output sets) residuals are loaded and outputs stored per thread.
+//   After the k-loop the kernel runs epilogue_staged, epilogue_regs (per thread) or epilogue_gates.  The first two share
+//   the pair arithmetic (pair_value, pair_store), the head (head_weights, head_add, head_store) and the row -> pixel
+//   map (tile_row, row_pixel), so that they produce identical bits.  Odd Cout (per thread only) has its own
+//   element-wise finish_scalar.
 // Warp roles: warps 0..7 = two consumer warpgroups (pixels 0..63 / 64..127 of the tile: wgmma m64nNk16 + epilogue),
 //   warps 8..11 = producer warpgroup, of which one thread issues the TMA loads.  The producer warpgroup exists so
 //   that setmaxnreg can hand its registers to the consumers (a 64 x 256 fp32 accumulator is 128 registers per
@@ -138,11 +142,8 @@ __device__ __forceinline__ uint16_t to_e4m3x2(float lo, float hi) {
   asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
   return r;
 }
-// (relu(v) - fp16(relu(v))) * 4096: the 8-bit low-order operand of an fp8 correction pass
-__device__ __forceinline__ float lo8_value(float v) {
-  const float a = fmaxf(v, 0.f);
-  return (a - __half2float(__float2half_rn(a))) * 4096.f;
-}
+// (a - fp16(a)) * 4096 of a ReLU'd value a: the 8-bit low-order operand of an fp8 correction pass
+__device__ __forceinline__ float lo8_value(float a) { return (a - __half2float(__float2half_rn(a))) * 4096.f; }
 
 // Work unit `u` -> tile.  Units enumerate (k-split, channel tile, pixel tile).
 __device__ __forceinline__ void tile_decode(int u, const Params& p, int& b, int& y0, int& x0, int& n0, int& ks) {
@@ -169,8 +170,49 @@ enum { EPI_PLAIN = 0, EPI_HEAD = 1, EPI_GATES = 2 };
 __device__ __forceinline__ float sigmoid_fast(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
 __device__ __forceinline__ float tanh_fast(float x) { return 1.f - __fdividef(2.f, 1.f + __expf(2.f * x)); }
 
-// One output element of the plain / head epilogue: bias, rank-1 term and residual added, outputs written.
-// `e`: element offset of (pixel, channel) in the [pixels, cout] outputs; `r` relative to the residual row.
+// One column pair (channels ch, ch + 1) of one row, in both plain / head forms.  The callers pass the pair's addresses:
+// global per thread, the stage's regions staged.  Which terms and outputs apply is read from Params, not from null
+// addresses: the compiler cannot prove a ring address non-null, and a null test per element splits the bias's
+// multiply-add (other bits) and spills.  (v0, v1): the accumulator times acc_scale, scaled by the callers where every use
+// of the product shares the block, which keeps that fusion as it was.  Then the bias (when add_bias), the rank-1 term
+// w1[ch] * x1 and the residual's hi and lo parts; the terms stay conditional, as adding a zero turns -0 into +0.
+__device__ __forceinline__ float2 pair_value(const Params& p, float v0, float v1, bool add_bias, const float* bias,
+                                             const float* r1w, float r1x, const __half* res, const __half* res_lo) {
+  if (add_bias) { v0 += bias[0]; v1 += bias[1]; }
+  if (p.rank1_w) { v0 = fmaf(r1w[0], r1x, v0); v1 = fmaf(r1w[1], r1x, v1); }
+  if (p.res) {
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res));
+    v0 += f.x; v1 += f.y;
+  }
+  if (p.res_lo) {
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(res_lo));
+    v0 += f.x; v1 += f.y;
+  }
+  return make_float2(v0, v1);
+}
+// fp16 of (v0, v1) and, when `with_lo`, the fp16 of what that rounding dropped
+__device__ __forceinline__ void store_hi_lo(__half* hi, bool with_lo, __half* lo, float v0, float v1) {
+  const __half2 h = __floats2half2_rn(v0, v1);
+  *reinterpret_cast<__half2*>(hi) = h;
+  if (with_lo) {
+    const float2 back = __half22float2(h);
+    *reinterpret_cast<__half2*>(lo) = __floats2half2_rn(v0 - back.x, v1 - back.y);
+  }
+}
+__device__ __forceinline__ float2 relu2(float2 v) { return make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f)); }
+// The pair's raw fp16 (also for the 4x4 pool, staged) and ReLU'd fp16 outputs with their lo parts, and the e4m3
+// operand of the next fp8 pass.  a = relu2(v), taken once by the caller for these and the head: a ReLU inside each
+// branch was duplicated into both arms of the next (one more branch per pair in the staged head loop).
+__device__ __forceinline__ void pair_store(const Params& p, float2 v, float2 a, __half* raw, __half* raw_lo, __half* relu,
+                                           __half* relu_lo, uint8_t* lo8) {
+  if (p.out_raw || p.out_pool4) store_hi_lo(raw, p.out_raw_lo, raw_lo, v.x, v.y);
+  if (p.out_relu) store_hi_lo(relu, p.out_relu_lo, relu_lo, a.x, a.y);
+  if (p.out_relu_lo8) *reinterpret_cast<uint16_t*>(lo8) = to_e4m3x2(lo8_value(a.x), lo8_value(a.y));
+}
+
+// One element of an odd Cout (unaligned pairs; per-thread form only): its own copy of the terms and conversions.  Its
+// unconditional `ks == 0 ? bias : 0` (the sign of a zero on later k-splits) and its fusion are kept as they were.
+// `e`: element offset of (pixel, channel) in the [pixels, cout] outputs; `rc` relative to the residual row.
 __device__ __forceinline__ float finish_scalar(const Params& p, float o, int ch, long long e, const __half* res,
                                               const __half* res_lo, int rc, float r1x, int ks) {
   o += ks == 0 ? p.bias[ch] : 0.f;
@@ -188,9 +230,255 @@ __device__ __forceinline__ float finish_scalar(const Params& p, float o, int ch,
     p.out_relu[e] = hv;
     if (p.out_relu_lo) p.out_relu_lo[e] = __float2half_rn(ro - __half2float(hv));
   }
-  if (p.out_relu_lo8) p.out_relu_lo8[e] = (uint8_t)(to_e4m3x2(lo8_value(o), 0.f) & 0xffu);
+  if (p.out_relu_lo8) p.out_relu_lo8[e] = (uint8_t)(to_e4m3x2(lo8_value(fmaxf(o, 0.f)), 0.f) & 0xffu);
   if (p.out_f32) p.out_f32[ks * p.f32_split_stride + e] = o;
   return o;
+}
+
+// Fused logit head (9 taps over the ReLU'd channels, fp32): w[2t + e] = tap t's weight of channel 8j + 2qd + e.
+__device__ __forceinline__ void head_weights(const float* s_head, int j, int qd, float (&w)[2 * kMaxHead]) {
+  const float* hw = s_head + (4 * j + qd) * kHeadPairStride;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float4 f = reinterpret_cast<const float4*>(hw)[q];
+    w[4 * q] = f.x; w[4 * q + 1] = f.y; w[4 * q + 2] = f.z; w[4 * q + 3] = f.w;
+  }
+  const float2 f = reinterpret_cast<const float2*>(hw)[8];
+  w[16] = f.x; w[17] = f.y;
+}
+// Adds a pair's ReLU'd values (a0, a1) to a pixel's running sums.  Both forms take the pairs in ascending order, a1
+// before a0, so their sums agree bit for bit.
+__device__ __forceinline__ void head_add(float (&acc)[kMaxHead], const float (&w)[2 * kMaxHead], float a0, float a1) {
+#pragma unroll
+  for (int t = 0; t < kMaxHead; ++t) acc[t] = fmaf(a0, w[2 * t], fmaf(a1, w[2 * t + 1], acc[t]));
+}
+// The four threads of a quad hold the same pixel's sums over disjoint channels: reduce them, and the quad's first thread
+// stores the pixel's head_n outputs (pix < 0: past the image edge, nothing stored).
+__device__ __forceinline__ void head_store(const Params& p, float (&acc)[kMaxHead], long long pix, int qd) {
+#pragma unroll
+  for (int t = 0; t < kMaxHead; ++t) {
+    acc[t] += __shfl_xor_sync(0xffffffffu, acc[t], 1);
+    acc[t] += __shfl_xor_sync(0xffffffffu, acc[t], 2);
+  }
+  if (pix >= 0 && qd == 0) {
+#pragma unroll
+    for (int t = 0; t < kMaxHead; ++t)
+      if (t < p.head_n) p.head_out[pix * p.head_n + t] = acc[t];
+  }
+}
+
+// Consumer thread (warp, lane) holds tile rows 16 warp + lane / 4 + 8i (i = 0, 1): wgmma's fragment layout.
+__device__ __forceinline__ int tile_row(int warp, int lane, int i) { return 16 * warp + (lane >> 2) + 8 * i; }
+// Tile row r of the tile at (b, y0, x0): its pixel index in [batch, ho, wo], or -1 past the image edge.
+__device__ __forceinline__ long long row_pixel(const Params& p, int b, int y0, int x0, int r) {
+  const int ty = r / p.tw, y = y0 + ty, x = x0 + r - ty * p.tw;
+  return (y < p.ho && x < p.wo) ? ((long long)b * p.ho + y) * p.wo + x : -1ll;
+}
+
+// Shared memory: the ring's A and B slots and barriers, then the head weights, the bias and the rank-1 column.
+struct Smem {
+  uint8_t *sA, *sB;
+  uint64_t *full, *empty;
+  float *head, *bias, *r1w;  // [128 pairs][kHeadPairStride] head weights, [kMaxBias] bias, [kMaxRank1] rank-1 column
+};
+
+// Staged form (see the file comment): the tile's N / 64 chunks through the ring stages the producer issued after its
+// k-iterations.  Rows past the image edge read the zero fill and compute values that no store writes.
+template <int N, bool HEAD>
+__device__ __forceinline__ void epilogue_staged(const Maps& maps, const Params& p, const Smem& s, const float (&d)[N / 2],
+                                                int& stage, uint32_t& phase, int b, int y0, int x0, int n0) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, qd = lane & 3;
+  // The rows' pixels are recomputed where used: only the accumulators, head sums and rank-1 inputs stay live.
+  float r1x[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const long long pix = row_pixel(p, b, y0, x0, tile_row(warp, lane, i));
+    r1x[i] = (p.rank1_x && pix >= 0) ? p.rank1_x[pix] : 0.f;
+  }
+  float hacc[2][HEAD ? kMaxHead : 1];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int t = 0; t < (HEAD ? kMaxHead : 1); ++t) hacc[i][t] = 0.f;
+  int prev = 0;
+#pragma unroll
+  for (int c = 0; c < N / 64; ++c) {
+    mbar_wait(&s.full[stage], phase);
+    uint8_t* const slot_a = s.sA + stage * A_BYTES;
+    uint8_t* const slot_b = s.sB + stage * B_BYTES_MAX;
+    auto region = [&](const int k) { return k == 0 ? slot_a : slot_b + (k - 1) * A_BYTES; };
+#pragma unroll
+    for (int jl = 0; jl < 8; ++jl) {  // column block of the chunk; the thread reads and writes the same elements
+      const int j = 8 * c + jl;
+      float w[2 * kMaxHead];
+      if constexpr (HEAD) head_weights(s.head, j, qd, w);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int r = tile_row(warp, lane, i);
+        const uint32_t o16 = r * 128 + (((jl ^ (r & 7)) << 4) | (qd << 2));  // 128B swizzle: conflict-free
+        const int ch = n0 + 8 * j + 2 * qd;
+        auto at = [&](const int k) { return reinterpret_cast<__half*>(region(k) + o16); };
+        const float2 v = pair_value(p, d[4 * j + 2 * i] * p.acc_scale, d[4 * j + 2 * i + 1] * p.acc_scale, true,
+                                    s.bias + ch, s.r1w + ch, r1x[i], at(0), at(1));
+        const float2 a = relu2(v);
+        pair_store(p, v, a, at(p.reg_raw), at(p.reg_raw_lo), at(p.reg_relu), at(p.reg_relu_lo),
+                   region(p.reg_lo8) + r * 64 + 8 * jl + 2 * qd);
+        if constexpr (HEAD) head_add(hacc[i], w, a.x, a.y);
+      }
+    }
+    fence_proxy_async();  // this thread's writes -> the TMA store's reads
+    named_bar_sync(1, CONSUMER_THREADS);
+    if (threadIdx.x == 0) {
+      const int cc[5] = {n0 + 64 * c, x0, y0, b, 0};
+      for (int k = 0; k < 3; ++k)
+        if (p.store_mask >> k & 1) tma_store_5d(&maps.out[k], region(k), cc);
+      bulk_commit();
+      if (c > 0) {  // the previous chunk's stores have read their stage: hand it back to the producer
+        bulk_wait_read<1>();
+        mbar_arrive(&s.empty[prev], CONSUMER_THREADS);
+      }
+    }
+    if (p.out_pool4) {
+      // 4x4 windows of the staged raw chunk in area_down_kernel's order (fp32 sum from 0 over dy, then dx, then
+      // * 1/16, one fp16 rounding), so the result is area_down(raw, 4) bit for bit.  The tile holds 8 windows;
+      // warp w takes window w, lane l its channel pair 2l: one 128-byte row per read, conflict-free.
+      const int win = warp, pc = lane;
+      const int wy = win / (p.tw >> 2), wx = win - wy * (p.tw >> 2);
+      const uint8_t* raw = region(p.reg_raw);
+      float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+      for (int dy = 0; dy < 4; ++dy)
+#pragma unroll
+        for (int dx = 0; dx < 4; ++dx) {
+          const int r = (4 * wy + dy) * p.tw + 4 * wx + dx;
+          const float2 f = __half22float2(
+              *reinterpret_cast<const __half2*>(raw + r * 128 + ((((pc >> 2) ^ (r & 7)) << 4) | ((pc & 3) << 2))));
+          s0 += f.x; s1 += f.y;
+        }
+      const int y = y0 + 4 * wy, x = x0 + 4 * wx;
+      if (y < p.ho && x < p.wo)  // ho, wo are multiples of 4: a window is wholly inside or wholly outside
+        *reinterpret_cast<__half2*>(
+            p.out_pool4 + (((long long)b * (p.ho >> 2) + (y >> 2)) * (p.wo >> 2) + (x >> 2)) * p.cout + n0 + 64 * c + 2 * pc) =
+            __floats2half2_rn(s0 * 0.0625f, s1 * 0.0625f);
+    }
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  if (p.out_pool4) named_bar_sync(1, CONSUMER_THREADS);  // every thread has read the last chunk for the pool
+  if (threadIdx.x == 0) {
+    bulk_wait_read<0>();
+    mbar_arrive(&s.empty[prev], CONSUMER_THREADS);
+  }
+  if constexpr (HEAD) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) head_store(p, hacc[i], row_pixel(p, b, y0, x0, tile_row(warp, lane, i)), qd);
+  }
+}
+
+// Per-thread form of the plain / head epilogue: residuals read and outputs written straight from the accumulator
+// registers.  It takes every launch the staged form does not (ragged Cout, split-K fp32 partials, larger output sets).
+template <int N, bool HEAD>
+__device__ __forceinline__ void epilogue_regs(const Params& p, const Smem& s, const float (&d)[N / 2], int b, int y0,
+                                              int x0, int n0, int ks) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, qd = lane & 3;
+  struct Row {
+    long long pix, off;  // pixel index (-1 past the image edge); element offset of (pixel, n0) in the [pixels, cout] outputs
+    const __half *res, *res_lo;
+    float r1x;
+  };
+  auto row_at = [&](const int i) {
+    Row r;
+    r.pix = row_pixel(p, b, y0, x0, tile_row(warp, lane, i));
+    r.off = r.pix * p.cout + n0;
+    r.res = p.res ? p.res + (p.res_batch_stride ? r.off : r.off - (long long)b * p.ho * p.wo * p.cout) : nullptr;
+    r.res_lo = p.res_lo ? p.res_lo + (r.res - p.res) : nullptr;
+    r.r1x = (p.rank1_x && r.pix >= 0) ? p.rank1_x[r.pix] : 0.f;
+    return r;
+  };
+  // Column pair (8j + 2qd, +1) of row i; returns its ReLU'd value (the head's input).  `full`: the tile spans N existing channels of an even Cout,
+  // so the per-column bounds check and the odd-Cout path drop out of the unrolled loop at compile time.
+  auto pair = [&](auto full_t, const Row& r, const int i, const int j) {
+    constexpr bool full = decltype(full_t)::value;
+    const int col = 8 * j + 2 * qd;
+    const int ch = n0 + col;
+    if (!full && (col >= p.nt || ch >= p.cout)) return make_float2(0.f, 0.f);
+    const float v0 = d[4 * j + 2 * i] * p.acc_scale, v1 = d[4 * j + 2 * i + 1] * p.acc_scale;
+    // Unwanted addresses are formed from null bases, never used: `q ? q + e : nullptr` guards spill (N >= 128).
+    const long long e = r.off + col;
+    if (full || p.cout % 2 == 0) {  // both channels exist and the pair is 4-byte aligned in the fp16 outputs
+      const float2 v = pair_value(p, v0, v1, ks == 0, s.bias + ch, s.r1w + ch, r.r1x, r.res + col, r.res_lo + col);
+      const float2 a = relu2(v);
+      pair_store(p, v, a, p.out_raw + e, p.out_raw_lo + e, p.out_relu + e, p.out_relu_lo + e, p.out_relu_lo8 + e);
+      if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + ks * p.f32_split_stride + e) = v;
+      return a;
+    }
+    // odd Cout (e.g. 1, 129): element by element
+    return relu2(make_float2(finish_scalar(p, v0, ch, e, r.res, r.res_lo, col, r.r1x, ks),
+                             ch + 1 < p.cout ? finish_scalar(p, v1, ch + 1, e + 1, r.res, r.res_lo, col + 1, r.r1x, ks) : v1));
+  };
+  if constexpr (HEAD) {
+    // The host admits the head only when the tile is the whole Cout and exactly N wide, so every column pair takes the
+    // full-width path.  Column pair outer, row inner: a pair's weights are loaded once for both rows.
+    const Row rows[2] = {row_at(0), row_at(1)};
+    float hacc[2][kMaxHead] = {};
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      float w[2 * kMaxHead];
+      head_weights(s.head, j, qd, w);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        if (rows[i].pix < 0) continue;
+        const float2 a = pair(std::true_type{}, rows[i], i, j);
+        head_add(hacc[i], w, a.x, a.y);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) head_store(p, hacc[i], rows[i].pix, qd);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const Row r = row_at(i);
+      if (r.pix >= 0) {
+        if (p.cout % 2 == 0 && p.nt == N && n0 + N <= p.cout) {  // every tile of the wide layers
+#pragma unroll
+          for (int j = 0; j < N / 8; ++j) pair(std::true_type{}, r, i, j);
+        } else {
+#pragma unroll
+          for (int j = 0; j < N / 8; ++j) pair(std::false_type{}, r, i, j);
+        }
+      }
+    }
+  }
+}
+
+// Gate form: the gated hidden-state update of the sensory updaters.  The channel tile is [forget | update | new] x 64
+// for hidden channels hc0 .. hc0+63 (modules.py:145-149): the three gates of hidden channel c sit in columns c, 64 + c,
+// 128 + c, i.e. in the same thread.
+__device__ __forceinline__ void epilogue_gates(const Params& p, const Smem& s, const float (&d)[96], int b, int y0,
+                                               int x0, int n0) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, qd = lane & 3;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const long long pix = row_pixel(p, b, y0, x0, tile_row(warp, lane, i));
+    if (pix >= 0) {
+      const int hc0 = (n0 / 192) * 64;
+      const long long hoff = pix * p.gate_c + hc0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int c = 8 * j + 2 * qd;
+        const float2 hp = __half22float2(*reinterpret_cast<const __half2*>(p.gate_h + hoff + c));
+        float o[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float f = sigmoid_fast(d[4 * j + 2 * i + e] + s.bias[n0 + c + e]);
+          const float uu = sigmoid_fast(d[4 * (j + 8) + 2 * i + e] + s.bias[n0 + 64 + c + e]);
+          const float n = tanh_fast(d[4 * (j + 16) + 2 * i + e] + s.bias[n0 + 128 + c + e]);
+          o[e] = f * (e ? hp.y : hp.x) * (1.f - uu) + uu * n;
+        }
+        *reinterpret_cast<__half2*>(p.gate_out + hoff + c) = __floats2half2_rn(o[0], o[1]);
+      }
+    }
+  }
 }
 
 // N: wgmma width (>= p.nt; columns past p.nt are never stored).
@@ -282,7 +570,6 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
   // ---------------------------------------------------------------- consumers: warpgroup wg owns pixels wg*64 .. +63
   setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = warp >> 2;
-  const int qd = lane & 3;  // column pair within each 8-column block of the fragment
   if constexpr (HEAD) {  // stage the head weights once per CTA, zero padded
     for (int i = threadIdx.x; i < HEAD_BYTES / 4; i += CONSUMER_THREADS) {
       const int pr = i / kHeadPairStride, k = i - pr * kHeadPairStride;
@@ -292,7 +579,7 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
     named_bar_sync(1, CONSUMER_THREADS);
   }
   const uint32_t a_off = wg * 64 * 128;  // this warpgroup's 64 rows of the A tile (8 swizzle atoms)
-  const bool even = (p.cout % 2) == 0;   // (channel, channel + 1) pairs are 4-byte aligned in the fp16 outputs
+  const Smem s = {sA, sB, full, empty, s_head, s_bias, s_r1w};
   float d[N / 2];
   int stage = 0;
   uint32_t phase = 0;
@@ -330,305 +617,12 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
     wgmma_fence_regs(d);
     mbar_arrive(&empty[stage == 0 ? STAGES - 1 : stage - 1]);  // the stage of the last k-iteration (my_k >= 1)
 
-    // thread holds rows r_i = wg*64 + (warp%4)*16 + lane/4 + 8i, columns 8j + 2*qd + {0, 1}
-    const float acc_scale = p.acc_scale;
-    struct Row {
-      bool live;
-      long long pix, off;  // pixel index; element offset of (pixel, n0) in the [pixels, cout] outputs
-      const __half* res;
-      const __half* res_lo;
-      float r1x;
-    };
-    auto row_at = [&](const int i) {
-      const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
-      const int ty = row / p.tw, tx = row - ty * p.tw;
-      const int y = y0 + ty, x = x0 + tx;
-      Row r;
-      r.live = (y < p.ho) && (x < p.wo);
-      r.pix = ((long long)b * p.ho + y) * p.wo + x;
-      r.off = r.pix * p.cout + n0;
-      r.res = p.res ? p.res + (p.res_batch_stride ? r.off : ((long long)y * p.wo + x) * p.cout + n0) : nullptr;
-      r.res_lo = p.res_lo ? p.res_lo + (r.res - p.res) : nullptr;
-      r.r1x = (p.rank1_x && r.live) ? p.rank1_x[r.pix] : 0.f;
-      return r;
-    };
-    // One column pair (8j + 2qd, +1) of row i: bias, rank-1 term and residual added, outputs written; returns the pair.
-    // `full`: the tile spans N existing channels of an even Cout, so the per-column bounds check and the
-    // element-by-element path drop out of the unrolled loop at compile time.
-    auto pair = [&](auto full_t, const Row& r, const int i, const int j) {
-      constexpr bool full = decltype(full_t)::value;
-      const int col = 8 * j + 2 * qd;
-      const int ch = n0 + col;
-      if (!full && (col >= p.nt || ch >= p.cout)) return make_float2(0.f, 0.f);
-      float v0 = d[4 * j + 2 * i] * acc_scale, v1 = d[4 * j + 2 * i + 1] * acc_scale;  // acc_scale: fp8 mode
-      if (full || even) {  // both channels exist (cout even, ch even): 4-byte fp16 pairs, 8-byte fp32 pairs
-        if (ks == 0) { v0 += s_bias[ch]; v1 += s_bias[ch + 1]; }
-        if (p.rank1_w) { v0 = fmaf(s_r1w[ch], r.r1x, v0); v1 = fmaf(s_r1w[ch + 1], r.r1x, v1); }
-        if (r.res) {
-          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(r.res + col));
-          v0 += f.x; v1 += f.y;
-        }
-        if (r.res_lo) {
-          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(r.res_lo + col));
-          v0 += f.x; v1 += f.y;
-        }
-        const long long e = r.off + col;
-        if (p.out_raw) {
-          const __half2 h = __floats2half2_rn(v0, v1);
-          *reinterpret_cast<__half2*>(p.out_raw + e) = h;
-          if (p.out_raw_lo) {
-            const float2 back = __half22float2(h);
-            *reinterpret_cast<__half2*>(p.out_raw_lo + e) = __floats2half2_rn(v0 - back.x, v1 - back.y);
-          }
-        }
-        if (p.out_relu) {
-          const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
-          const __half2 h = __floats2half2_rn(a0, a1);
-          *reinterpret_cast<__half2*>(p.out_relu + e) = h;
-          if (p.out_relu_lo) {
-            const float2 back = __half22float2(h);
-            *reinterpret_cast<__half2*>(p.out_relu_lo + e) = __floats2half2_rn(a0 - back.x, a1 - back.y);
-          }
-        }
-        if (p.out_relu_lo8)
-          *reinterpret_cast<uint16_t*>(p.out_relu_lo8 + e) = to_e4m3x2(lo8_value(v0), lo8_value(v1));
-        if (p.out_f32)
-          *reinterpret_cast<float2*>(p.out_f32 + ks * p.f32_split_stride + e) = make_float2(v0, v1);
-      } else {  // ragged channel count (e.g. Cout = 1, 129): element by element
-        v0 = finish_scalar(p, v0, ch, r.off + col, r.res, r.res_lo, col, r.r1x, ks);
-        if (ch + 1 < p.cout) v1 = finish_scalar(p, v1, ch + 1, r.off + col + 1, r.res, r.res_lo, col + 1, r.r1x, ks);
-      }
-      return make_float2(v0, v1);
-    };
-    if constexpr (EPI != EPI_GATES) {
-      if (p.staged) {
-        // Row i of this thread: tile row r, its pixel index (-1 past the image edge).  Recomputed where it is used so
-        // that nothing but the accumulators and the head sums stays live across the chunks.
-        auto tile_row = [&](const int i) { return wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i; };
-        auto pixel = [&](const int i) {
-          const int r = tile_row(i), ty = r / p.tw, y = y0 + ty, x = x0 + r - ty * p.tw;
-          return (y < p.ho && x < p.wo) ? ((long long)b * p.ho + y) * p.wo + x : -1ll;
-        };
-        float r1x[2];
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const long long pix = pixel(i);
-          r1x[i] = (p.rank1_x && pix >= 0) ? p.rank1_x[pix] : 0.f;
-        }
-        // Rows past the image edge read the zero fill and compute values that no store writes.
-        float hacc[2][HEAD ? kMaxHead : 1];
-#pragma unroll
-        for (int i = 0; i < 2; ++i)
-#pragma unroll
-          for (int t = 0; t < (HEAD ? kMaxHead : 1); ++t) hacc[i][t] = 0.f;
-        int prev = 0;
-#pragma unroll
-        for (int c = 0; c < N / 64; ++c) {
-          mbar_wait(&full[stage], phase);
-          uint8_t* const slot_a = sA + stage * A_BYTES;
-          uint8_t* const slot_b = sB + stage * B_BYTES_MAX;
-          auto region = [&](const int k) { return k == 0 ? slot_a : slot_b + (k - 1) * A_BYTES; };
-#pragma unroll
-          for (int jl = 0; jl < 8; ++jl) {  // column block of the chunk; the thread reads and writes the same elements
-            const int j = 8 * c + jl;
-            float w[2 * kMaxHead];
-            if constexpr (HEAD) {
-              const float* hw = s_head + (4 * j + qd) * kHeadPairStride;
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const float4 f = reinterpret_cast<const float4*>(hw)[q];
-                w[4 * q] = f.x; w[4 * q + 1] = f.y; w[4 * q + 2] = f.z; w[4 * q + 3] = f.w;
-              }
-              const float2 f = reinterpret_cast<const float2*>(hw)[8];
-              w[16] = f.x; w[17] = f.y;
-            }
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              const int r = tile_row(i);
-              const uint32_t o16 = r * 128 + (((jl ^ (r & 7)) << 4) | (qd << 2));  // 128B swizzle: conflict-free
-              const int ch = n0 + 8 * j + 2 * qd;
-              float v0 = d[4 * j + 2 * i] * acc_scale, v1 = d[4 * j + 2 * i + 1] * acc_scale;
-              v0 += s_bias[ch]; v1 += s_bias[ch + 1];
-              if (p.rank1_w) { v0 = fmaf(s_r1w[ch], r1x[i], v0); v1 = fmaf(s_r1w[ch + 1], r1x[i], v1); }
-              if (p.res) {
-                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(slot_a + o16));
-                v0 += f.x; v1 += f.y;
-              }
-              if (p.res_lo) {
-                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(slot_b + o16));
-                v0 += f.x; v1 += f.y;
-              }
-              if (p.out_raw || p.out_pool4) {
-                const __half2 h = __floats2half2_rn(v0, v1);
-                *reinterpret_cast<__half2*>(region(p.reg_raw) + o16) = h;
-                if (p.out_raw_lo) {
-                  const float2 back = __half22float2(h);
-                  *reinterpret_cast<__half2*>(region(p.reg_raw_lo) + o16) = __floats2half2_rn(v0 - back.x, v1 - back.y);
-                }
-              }
-              const float a0 = fmaxf(v0, 0.f), a1 = fmaxf(v1, 0.f);
-              if (p.out_relu) {
-                const __half2 h = __floats2half2_rn(a0, a1);
-                *reinterpret_cast<__half2*>(region(p.reg_relu) + o16) = h;
-                if (p.out_relu_lo) {
-                  const float2 back = __half22float2(h);
-                  *reinterpret_cast<__half2*>(region(p.reg_relu_lo) + o16) = __floats2half2_rn(a0 - back.x, a1 - back.y);
-                }
-              }
-              if (p.out_relu_lo8)
-                *reinterpret_cast<uint16_t*>(region(p.reg_lo8) + r * 64 + 8 * jl + 2 * qd) =
-                    to_e4m3x2(lo8_value(v0), lo8_value(v1));
-              if constexpr (HEAD) {
-#pragma unroll
-                for (int t = 0; t < kMaxHead; ++t) hacc[i][t] = fmaf(a0, w[2 * t], fmaf(a1, w[2 * t + 1], hacc[i][t]));
-              }
-            }
-          }
-          fence_proxy_async();  // this thread's writes -> the TMA store's reads
-          named_bar_sync(1, CONSUMER_THREADS);
-          if (threadIdx.x == 0) {
-            const int cc[5] = {n0 + 64 * c, x0, y0, b, 0};
-            for (int k = 0; k < 3; ++k)
-              if (p.store_mask >> k & 1) tma_store_5d(&maps.out[k], region(k), cc);
-            bulk_commit();
-            if (c > 0) {  // the previous chunk's stores have read their stage: hand it back to the producer
-              bulk_wait_read<1>();
-              mbar_arrive(&empty[prev], CONSUMER_THREADS);
-            }
-          }
-          if (p.out_pool4) {
-            // 4x4 windows of the staged raw chunk in area_down_kernel's order (fp32 sum from 0 over dy, then dx, then
-            // * 1/16, one fp16 rounding), so the result is area_down(raw, 4) bit for bit.  The tile holds 8 windows;
-            // warp w takes window w, lane l its channel pair 2l: one 128-byte row per read, conflict-free.
-            const int win = threadIdx.x >> 5, pc = lane;
-            const int wy = win / (p.tw >> 2), wx = win - wy * (p.tw >> 2);
-            const uint8_t* raw = region(p.reg_raw);
-            float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-            for (int dy = 0; dy < 4; ++dy)
-#pragma unroll
-              for (int dx = 0; dx < 4; ++dx) {
-                const int r = (4 * wy + dy) * p.tw + 4 * wx + dx;
-                const float2 f = __half22float2(
-                    *reinterpret_cast<const __half2*>(raw + r * 128 + ((((pc >> 2) ^ (r & 7)) << 4) | ((pc & 3) << 2))));
-                s0 += f.x; s1 += f.y;
-              }
-            const int y = y0 + 4 * wy, x = x0 + 4 * wx;
-            if (y < p.ho && x < p.wo)  // ho, wo are multiples of 4: a window is wholly inside or wholly outside
-              *reinterpret_cast<__half2*>(
-                  p.out_pool4 + (((long long)b * (p.ho >> 2) + (y >> 2)) * (p.wo >> 2) + (x >> 2)) * p.cout + n0 + 64 * c + 2 * pc) =
-                  __floats2half2_rn(s0 * 0.0625f, s1 * 0.0625f);
-          }
-          prev = stage;
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (p.out_pool4) named_bar_sync(1, CONSUMER_THREADS);  // every thread has read the last chunk for the pool
-        if (threadIdx.x == 0) {
-          bulk_wait_read<0>();
-          mbar_arrive(&empty[prev], CONSUMER_THREADS);
-        }
-        if constexpr (HEAD) {
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-#pragma unroll
-            for (int t = 0; t < kMaxHead; ++t) {
-              hacc[i][t] += __shfl_xor_sync(0xffffffffu, hacc[i][t], 1);
-              hacc[i][t] += __shfl_xor_sync(0xffffffffu, hacc[i][t], 2);
-            }
-            const long long pix = pixel(i);
-            if (pix >= 0 && qd == 0) {
-#pragma unroll
-              for (int t = 0; t < kMaxHead; ++t)
-                if (t < p.head_n) p.head_out[pix * p.head_n + t] = hacc[i][t];
-            }
-          }
-        }
-        continue;
-      }
-    }
-    if constexpr (EPI == EPI_GATES) {
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const Row r = row_at(i);
-        // channel tile = [forget | update | new] x 64 for hidden channels hc0 .. hc0+63 (modules.py:145-149): the three
-        // gates of hidden channel c sit in columns c, 64 + c, 128 + c, i.e. in the same thread
-        if (r.live) {
-          const int hc0 = (n0 / 192) * 64;
-          const long long hoff = r.pix * p.gate_c + hc0;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int c = 8 * j + 2 * qd;
-            const float2 hp = __half22float2(*reinterpret_cast<const __half2*>(p.gate_h + hoff + c));
-            float o[2];
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const float f = sigmoid_fast(d[4 * j + 2 * i + e] + s_bias[n0 + c + e]);
-              const float uu = sigmoid_fast(d[4 * (j + 8) + 2 * i + e] + s_bias[n0 + 64 + c + e]);
-              const float n = tanh_fast(d[4 * (j + 16) + 2 * i + e] + s_bias[n0 + 128 + c + e]);
-              o[e] = f * (e ? hp.y : hp.x) * (1.f - uu) + uu * n;
-            }
-            *reinterpret_cast<__half2*>(p.gate_out + hoff + c) = __floats2half2_rn(o[0], o[1]);
-          }
-        }
-      }
-    } else if constexpr (HEAD) {
-      // Logit head: 9 taps over the ReLU'd channels, fp32.  The host admits it only when the tile is the whole Cout and
-      // exactly N wide, so every column pair takes the full-width path.  Column pair outer, row inner: a pair's weights
-      // are loaded once for both rows.  Each row's running sums still take the pairs in ascending order, a1 before a0.
-      const Row rows[2] = {row_at(0), row_at(1)};
-      float hacc[2][kMaxHead];
-#pragma unroll
-      for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int t = 0; t < kMaxHead; ++t) hacc[i][t] = 0.f;
-#pragma unroll
-      for (int j = 0; j < N / 8; ++j) {
-        const float* hw = s_head + (4 * j + qd) * kHeadPairStride;  // pair (8j + 2qd) / 2
-        float w[2 * kMaxHead];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 f = reinterpret_cast<const float4*>(hw)[q];
-          w[4 * q] = f.x; w[4 * q + 1] = f.y; w[4 * q + 2] = f.z; w[4 * q + 3] = f.w;
-        }
-        const float2 f = reinterpret_cast<const float2*>(hw)[8];
-        w[16] = f.x; w[17] = f.y;
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          if (!rows[i].live) continue;
-          const float2 v = pair(std::true_type{}, rows[i], i, j);
-          const float a0 = fmaxf(v.x, 0.f), a1 = fmaxf(v.y, 0.f);
-#pragma unroll
-          for (int t = 0; t < kMaxHead; ++t) hacc[i][t] = fmaf(a0, w[2 * t], fmaf(a1, w[2 * t + 1], hacc[i][t]));
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {  // the four threads of a quad hold the same pixel's partial sums over disjoint channels
-#pragma unroll
-        for (int t = 0; t < kMaxHead; ++t) {
-          hacc[i][t] += __shfl_xor_sync(0xffffffffu, hacc[i][t], 1);
-          hacc[i][t] += __shfl_xor_sync(0xffffffffu, hacc[i][t], 2);
-        }
-        if (rows[i].live && qd == 0) {
-#pragma unroll
-          for (int t = 0; t < kMaxHead; ++t)
-            if (t < p.head_n) p.head_out[rows[i].pix * p.head_n + t] = hacc[i][t];
-        }
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const Row r = row_at(i);
-        if (r.live) {
-          if (even && p.nt == N && n0 + N <= p.cout) {  // every tile of the wide layers
-#pragma unroll
-            for (int j = 0; j < N / 8; ++j) pair(std::true_type{}, r, i, j);
-          } else {
-#pragma unroll
-            for (int j = 0; j < N / 8; ++j) pair(std::false_type{}, r, i, j);
-          }
-        }
-      }
-    }
+    if constexpr (EPI == EPI_GATES)
+      epilogue_gates(p, s, d, b, y0, x0, n0);
+    else if (p.staged)
+      epilogue_staged<N, HEAD>(maps, p, s, d, stage, phase, b, y0, x0, n0);
+    else
+      epilogue_regs<N, HEAD>(p, s, d, b, y0, x0, n0, ks);
   }
 }
 
@@ -636,6 +630,66 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
 }  // namespace b200
 
 using namespace b200;
+
+// Staged epilogue plan (p.staged, output regions, tensor maps): every tile spans exactly N existing channels, fp16 / e4m3
+// outputs that fit the three regions of a stage, 16-byte aligned operands (TMA).  DEVA_B200_CONV_EPI=regs keeps the
+// per-thread epilogue (A/B comparisons); DEVA_B200_CONV_EPI=staged refuses a launch that cannot take the staged one.
+static int plan_staged(const deva_b200_conv_desc& d, int ho, int wo, int n_mma, conv::Params& p, conv::Maps& maps) {
+  using namespace conv;
+  const char* err = nullptr;
+  const char* env = getenv("DEVA_B200_CONV_EPI");
+  const bool regs = env && strcmp(env, "regs") == 0, must = env && strcmp(env, "staged") == 0;
+  auto aligned = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  const bool pool = d.out_pool4 != nullptr;
+  // fp16 regions in order: raw (also staged, unstored, when only its pool is wanted), raw_lo, relu, relu_lo
+  const void* outs[4] = {d.out_raw, d.out_raw_lo, d.out_relu, d.out_relu_lo};
+  const bool used[4] = {d.out_raw || pool, d.out_raw_lo != nullptr, d.out_relu != nullptr, d.out_relu_lo != nullptr};
+  int n16 = 0;
+  for (int k = 0; k < 4; ++k) n16 += used[k] ? 1 : 0;
+  // the e4m3 region (64-byte rows) must not overlay a residual half that other threads have yet to read
+  const int r_lo8 = std::max({n16, d.res ? 1 : 0, d.res_lo ? 2 : 0});
+  // a low-order part without its fp16 output is written by neither epilogue form, so the staged one must not store it
+  const bool ok = !regs && !p.gate_out && p.ksplit == 1 && !d.out_f32 && d.nt == n_mma && d.cout == d.cout_pad &&
+                  (!d.res_lo || d.res) && !(d.out_raw_lo && !d.out_raw) && !(d.out_relu_lo && !d.out_relu) &&
+                  aligned(d.res) && aligned(d.res_lo) && aligned(d.out_raw) && aligned(d.out_raw_lo) &&
+                  aligned(d.out_relu) && aligned(d.out_relu_lo) && aligned(d.out_relu_lo8) && aligned(d.out_pool4) &&
+                  (d.out_relu_lo8 ? r_lo8 <= 2 : n16 <= 3);
+  B200_REQUIRE(ok || !(must || pool), "conv: %s needs the staged epilogue (full-width channel tiles, cout == cout_pad, "
+               "no fp32 / split-K / gate outputs, outputs that fit a ring stage)%s", pool ? "out_pool4" : "DEVA_B200_CONV_EPI=staged",
+               regs ? ", which DEVA_B200_CONV_EPI=regs turns off" : "");
+  B200_REQUIRE(!pool || (d.th % 4 == 0 && d.tw % 4 == 0 && ho % 4 == 0 && wo % 4 == 0),
+               "conv: out_pool4 needs th, tw (%d, %d) and ho, wo (%d, %d) multiples of 4", d.th, d.tw, ho, wo);
+  if (ok) {
+    const long long cstr = d.cout, wstr = (long long)wo * d.cout, bstr = (long long)ho * wo * d.cout;
+    signed char* regs_of[4] = {&p.reg_raw, &p.reg_raw_lo, &p.reg_relu, &p.reg_relu_lo};
+    int rc = 0, k16 = 0;
+    for (int k = 0; k < 4; ++k) {
+      if (!used[k]) continue;
+      *regs_of[k] = (signed char)k16;
+      if (outs[k]) {
+        rc |= make_tmap_act5(&maps.out[k16], outs[k], d.cout, wo, ho, d.batch, cstr, wstr, bstr, d.tw, d.th, &err);
+        p.store_mask |= 1 << k16;
+      }
+      ++k16;
+    }
+    if (d.out_relu_lo8) {
+      p.reg_lo8 = (signed char)r_lo8;
+      rc |= make_tmap_act5_u8(&maps.out[r_lo8], d.out_relu_lo8, d.cout, wo, ho, d.batch, cstr, wstr, bstr, 64, d.tw, d.th,
+                              &err);
+      p.store_mask |= 1 << r_lo8;
+    }
+    const int rb = d.res_broadcast ? 1 : d.batch;
+    if (d.res) rc |= make_tmap_act5(&maps.res, d.res, d.cout, wo, ho, rb, cstr, wstr, bstr, d.tw, d.th, &err);
+    if (d.res_lo) rc |= make_tmap_act5(&maps.res_lo, d.res_lo, d.cout, wo, ho, rb, cstr, wstr, bstr, d.tw, d.th, &err);
+    if (rc) {
+      set_error("conv: %s", err ? err : "epilogue tensor maps");
+      return 3;
+    }
+    p.staged = 1;
+    p.out_pool4 = reinterpret_cast<__half*>(d.out_pool4);
+  }
+  return 0;
+}
 
 extern "C" {
 
@@ -804,62 +858,7 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
   p.k_per_split = (k_iters_total + p.ksplit - 1) / p.ksplit;
   p.ksplit = (k_iters_total + p.k_per_split - 1) / p.k_per_split;  // no empty trailing split
   p.f32_split_stride = (long long)d.batch * ho * wo * d.cout;
-  // staged epilogue: every tile spans exactly N existing channels, fp16 / e4m3 outputs that fit the three regions of a
-  // stage, 16-byte aligned operands (TMA).  DEVA_B200_CONV_EPI=regs keeps the per-thread epilogue (A/B comparisons);
-  // DEVA_B200_CONV_EPI=staged refuses a launch that cannot take the staged one (tests).
-  {
-    const char* env = getenv("DEVA_B200_CONV_EPI");
-    const bool regs = env && strcmp(env, "regs") == 0, must = env && strcmp(env, "staged") == 0;
-    auto aligned = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-    const bool pool = d.out_pool4 != nullptr;
-    // fp16 regions in order: raw (also staged, unstored, when only its pool is wanted), raw_lo, relu, relu_lo
-    const void* outs[4] = {d.out_raw, d.out_raw_lo, d.out_relu, d.out_relu_lo};
-    const bool used[4] = {d.out_raw || pool, d.out_raw_lo != nullptr, d.out_relu != nullptr, d.out_relu_lo != nullptr};
-    int n16 = 0;
-    for (int k = 0; k < 4; ++k) n16 += used[k] ? 1 : 0;
-    // the e4m3 region (64-byte rows) must not overlay a residual half that other threads have yet to read
-    const int r_lo8 = std::max({n16, d.res ? 1 : 0, d.res_lo ? 2 : 0});
-    // a low-order part without its fp16 output is written by neither epilogue form, so the staged one must not store it
-    const bool ok = !regs && !p.gate_out && p.ksplit == 1 && !d.out_f32 && d.nt == n_mma && d.cout == d.cout_pad &&
-                    (!d.res_lo || d.res) && !(d.out_raw_lo && !d.out_raw) && !(d.out_relu_lo && !d.out_relu) &&
-                    aligned(d.res) && aligned(d.res_lo) && aligned(d.out_raw) && aligned(d.out_raw_lo) &&
-                    aligned(d.out_relu) && aligned(d.out_relu_lo) && aligned(d.out_relu_lo8) && aligned(d.out_pool4) &&
-                    (d.out_relu_lo8 ? r_lo8 <= 2 : n16 <= 3);
-    B200_REQUIRE(ok || !(must || pool), "conv: %s needs the staged epilogue (full-width channel tiles, cout == cout_pad, "
-                 "no fp32 / split-K / gate outputs, outputs that fit a ring stage)%s", pool ? "out_pool4" : "DEVA_B200_CONV_EPI=staged",
-                 regs ? ", which DEVA_B200_CONV_EPI=regs turns off" : "");
-    B200_REQUIRE(!pool || (d.th % 4 == 0 && d.tw % 4 == 0 && ho % 4 == 0 && wo % 4 == 0),
-                 "conv: out_pool4 needs th, tw (%d, %d) and ho, wo (%d, %d) multiples of 4", d.th, d.tw, ho, wo);
-    if (ok) {
-      const long long cstr = d.cout, wstr = (long long)wo * d.cout, bstr = (long long)ho * wo * d.cout;
-      signed char* regs_of[4] = {&p.reg_raw, &p.reg_raw_lo, &p.reg_relu, &p.reg_relu_lo};
-      int rc = 0, k16 = 0;
-      for (int k = 0; k < 4; ++k) {
-        if (!used[k]) continue;
-        *regs_of[k] = (signed char)k16;
-        if (outs[k]) {
-          rc |= make_tmap_act5(&maps.out[k16], outs[k], d.cout, wo, ho, d.batch, cstr, wstr, bstr, d.tw, d.th, &err);
-          p.store_mask |= 1 << k16;
-        }
-        ++k16;
-      }
-      if (d.out_relu_lo8) {
-        p.reg_lo8 = (signed char)r_lo8;
-        rc |= make_tmap_act5_u8(&maps.out[r_lo8], d.out_relu_lo8, d.cout, wo, ho, d.batch, cstr, wstr, bstr, 64, d.tw, d.th,
-                                &err);
-        p.store_mask |= 1 << r_lo8;
-      }
-      const int rb = d.res_broadcast ? 1 : d.batch;
-      if (d.res) rc |= make_tmap_act5(&maps.res, d.res, d.cout, wo, ho, rb, cstr, wstr, bstr, d.tw, d.th, &err);
-      if (d.res_lo) rc |= make_tmap_act5(&maps.res_lo, d.res_lo, d.cout, wo, ho, rb, cstr, wstr, bstr, d.tw, d.th, &err);
-      if (rc) {
-        set_error("conv: %s", err ? err : "epilogue tensor maps");
-        return 3;
-      }
-      p.staged = 1;
-      p.out_pool4 = reinterpret_cast<__half*>(d.out_pool4);
-    }
-  }
+  if (const int rc = plan_staged(d, ho, wo, n_mma, p, maps)) return rc;
   const long long units = (long long)p.m_tiles * p.n_tiles * p.ksplit;
   B200_REQUIRE(units <= INT32_MAX, "conv: %lld work units", units);
   p.units = (int)units;
