@@ -27,14 +27,15 @@
 extern "C" {
 #endif
 
-/* v16: deva_b200_label_areas and deva_b200_label_to_index (unsupervised DAVIS 2017 object limit).
+/* v18: dropped conv split_mode 1, the split twins' relu_lo and hi-only pooling, gru, nhwc_to_nchw, enable_peer_access.
+ * v16: deva_b200_label_areas and deva_b200_label_to_index (unsupervised DAVIS 2017 object limit).
  * v15: deva_b200_pano_joint_hist and deva_b200_pano_remap (video panoptic metrics and stuff merging).
  * v14: deva_b200_prob_to_scores and deva_b200_scores_to_ids (multi-scale / flip score export and merge).
  * v13: deva_b200_prob_to_segments (the result savers' id map, id image, overlay, areas and boxes in one pass).
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 17
+#define DEVA_B200_ABI_VERSION 18
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -146,9 +147,6 @@ DEVA_B200_API int deva_b200_readout_sparse_scatter(const void* values, int64_t v
                                                    const int32_t* idx, const float* w, int top_k, int n_window, int q,
                                                    void* workspace, float* const* rank_dst, int n_ranks,
                                                    int64_t ld_out, deva_stream_t stream);
-/* Let kernels launched on `device` dereference memory of `peer_device` (cudaDeviceEnablePeerAccess; already-enabled
- * is not an error).  Needed once per peer before deva_b200_readout_sparse_scatter is given IPC-mapped pointers. */
-DEVA_B200_API int deva_b200_enable_peer_access(int device, int peer_device);
 /* Peer-visible buffers for the scatter read-out.  peer_alloc: cudaMalloc (zeroed) on `device` + its 64-byte CUDA IPC
  * handle, to be sent to the other ranks; peer_open: map a peer's handle INTO `device`'s address space
  * (cudaIpcOpenMemHandle with lazy peer access - an IPC mapping opened under the exporter's device is not reachable
@@ -178,9 +176,8 @@ typedef struct deva_b200_conv_desc {
   const void* x_lo;     /* optional fp16 low-order part of x (x_true = x + x_lo): split-precision mode
                          * D = Xh.Wh + Xl.Wh + Xh.Wl with weights packed [cout_pad, 2 (hi, lo), kh*kw, cin_pad];
                          * ~fp32 accuracy at 3x the MMA work.  Exclusive with x2. */
-  int32_t split_mode;   /* 0: as described above (x_lo => three passes);  1: x_lo with SINGLE fp16 weights,
-                         * D = Xh.W + Xl.W (removes the activation-operand rounding, 2x the MMA work);  2: no x_lo,
-                         * weights packed (hi, lo) as for mode 0, D = X.Wh + X.Wl (removes the weight rounding) */
+  int32_t split_mode;   /* 0: as described above (x_lo => three passes);  2: no x_lo, weights packed (hi, lo) as for
+                         * mode 0, D = X.Wh + X.Wl (removes the weight rounding);  3: see x_lo8 below */
   int32_t batch, h, w, cin_pad;
   const void* w_packed; /* fp16 [cout_pad, kh*kw*cin_pad] */
   int32_t kh, kw, stride; /* 1x1 or 3x3, stride 1 or 2, padding kh/2 (nn.Conv2d semantics) */
@@ -206,7 +203,8 @@ typedef struct deva_b200_conv_desc {
    * gate_out = sigmoid(f) * gate_h * (1 - sigmoid(u)) + sigmoid(u) * tanh(n), evaluated on the fp32 accumulators. */
   const void* gate_h;   /* fp16 NHWC [batch, ho, wo, cout/3] previous hidden state */
   void* gate_out;       /* fp16 NHWC [batch, ho, wo, cout/3] new hidden state */
-  /* split_mode 3: the low-order activation pass on the fp8 tensor-core path (half the cost of split_mode 1):
+  /* split_mode 3: a low-order activation pass on the fp8 tensor-core path (removes the activation-operand rounding at
+   * half the cost of a second fp16 pass):
    * D = (X . W16 + Xlo8 . W8) * acc_scale, W16 = fp16(W * 2^S) in w_packed, W8 = e4m3(W * 2^(S-12)) in w8_packed,
    * Xlo8 = e4m3((x - fp16(x)) * 4096) in x_lo8, acc_scale = 2^-S.  Stride 1, cin_pad % 128 == 0. */
   const void* x_lo8;    /* u8 NHWC [batch, h, w, cin_pad] */
@@ -232,7 +230,6 @@ DEVA_B200_API int deva_b200_stem_im2col(const float* src, void* dst, void* dst_l
                                         deva_stream_t stream);
 DEVA_B200_API int deva_b200_nchw_to_nhwc(const float* src, void* dst, int b, int c, int h, int w, int c_pad,
                                          deva_stream_t stream);
-DEVA_B200_API int deva_b200_nhwc_to_nchw(const void* src, float* dst, int b, int c, int h, int w, deva_stream_t stream);
 /* 3x3 stride-2 max pool (resnet.py:123); x_lo / y_lo: optional low-order parts (pooling acts on x + x_lo) */
 DEVA_B200_API int deva_b200_maxpool(const void* x, const void* x_lo, void* y, void* y_lo, int b, int h, int w, int c,
                                     deva_stream_t stream);
@@ -248,21 +245,15 @@ DEVA_B200_API int deva_b200_cbam(const void* x, const float* w1, const float* b1
                                  int w, int c, int r, deva_stream_t stream);
 /* Split-precision twins for a residual stream carried as fp16 (hi, lo) pairs (the default "parity" precision plan): the
  * input is g + g_lo (x + x_lo) [+ skip_lo, optional], the raw result is written as (raw, raw_lo) (both NULL = not
- * wanted), the ReLU'd copy (an MMA operand) as hi, plus its remainder relu_lo when the consumer runs a second
- * activation pass (conv split_mode 1). */
+ * wanted), the ReLU'd copy (an MMA operand) as hi.  relu_lo8 (optional): u8 NHWC, e4m3 of (relu - fp16(relu)) * 4096 -
+ * the low-order operand of a conv with split_mode 3.  cbam_split takes the gate statistics (channel pooling, per-pixel
+ * max / mean) over x + x_lo. */
 DEVA_B200_API int deva_b200_up2_add_split(const void* g, const void* g_lo, const void* skip, const void* skip_lo,
-                                          void* raw, void* raw_lo, void* relu, void* relu_lo, void* relu_lo8, int b, int h,
-                                          int w, int c, deva_stream_t stream);
-/* relu_lo8 (instead of relu_lo): u8 NHWC, e4m3 of (relu - fp16(relu)) * 4096 - the low-order operand of a conv with
- * split_mode 3. */
+                                          void* raw, void* raw_lo, void* relu, void* relu_lo8, int b, int h, int w, int c,
+                                          deva_stream_t stream);
 DEVA_B200_API int deva_b200_cbam_split(const void* x, const void* x_lo, const float* w1, const float* b1, const float* w2,
                                        const float* b2, const float* ws, const float* bs, float* scratch, void* raw,
-                                       void* raw_lo, void* relu, void* relu_lo, int pool_lo, int b, int h, int w, int c,
-                                       int r, deva_stream_t stream);
-/* pool_lo: 1 = the gate statistics (channel pooling, per-pixel max / mean) are taken over x + x_lo, 0 = over x only. */
-/* sensory GRU gates (modules.py:145-149): values fp16 [pixels, 3c], h fp16 [pixels, c] -> out fp16 */
-DEVA_B200_API int deva_b200_gru(const void* values, const void* h, void* out, int64_t pixels, int c,
-                                deva_stream_t stream);
+                                       void* raw_lo, void* relu, int b, int h, int w, int c, int r, deva_stream_t stream);
 /* Finish of a split-K convolution (deva_b200_conv2d with ksplit > 1): out = sum of the n_parts fp32 partial sums
  * (part_stride elements apart, bias in part 0) + optional fp16 residual (res + res_lo), written as fp16 raw / ReLU'd
  * tensors, each optionally as a (hi, lo) pair.  n = elements per part (multiple of 8). */

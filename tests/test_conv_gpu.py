@@ -244,13 +244,6 @@ def test_helpers_match_torch():
         assert float((_nchw(ops.area_down(yh, r)) - want).abs().max()) < 2e-3
     plane = torch.rand(3, 32, 48, device='cuda', generator=g)
     torch.testing.assert_close(ops.area_down_plane(plane, 16), F.interpolate(plane.unsqueeze(0), size=(2, 3), mode='area')[0])
-    # GRU
-    c = 64
-    vals = torch.randn(2, 5, 7, 3 * c, device='cuda', generator=g).half()
-    h = torch.randn(2, 5, 7, c, device='cuda', generator=g).half()
-    v, hf = vals.float(), h.float()
-    want = torch.sigmoid(v[..., :c]) * hf * (1 - torch.sigmoid(v[..., c:2 * c])) + torch.sigmoid(v[..., c:2 * c]) * torch.tanh(v[..., 2 * c:])
-    assert float((ops.gru(vals, h).float() - want).abs().max()) < 2e-3
     # CBAM residual
     c = 512
     x = torch.randn(2, c, 6, 9, device='cuda', generator=g)
@@ -298,11 +291,9 @@ def test_helpers_match_torch():
     nat.transpose_append(src, dst[:, 8:], 128, 70, 96)
     torch.cuda.synchronize()
     assert torch.equal(dst[:, 8:78], src.t())
-    # layout converters
+    # layout converter: fp32 NCHW -> fp16 NHWC, channels 5..7 zero padding
     img = torch.randn(2, 5, 7, 9, device='cuda', generator=g)
-    d = torch.empty(2, 7, 9, 8, dtype=torch.float16, device='cuda')
+    d = torch.full((2, 7, 9, 8), float('nan'), dtype=torch.float16, device='cuda')
     nat.nchw_to_nhwc(img, d, 2, 5, 7, 9, 8)
-    back = torch.empty(2, 8, 7, 9, device='cuda')
-    nat.nhwc_to_nchw(d, back, 2, 8, 7, 9)
     torch.cuda.synchronize()
-    assert torch.equal(back[:, :5], img.half().float()) and bool((back[:, 5:] == 0).all())
+    assert torch.equal(d[..., :5], img.half().permute(0, 2, 3, 1)) and bool((d[..., 5:] == 0).all())

@@ -9,7 +9,6 @@ from deva.model import native_ops as ops  # noqa: E402
 CASES = {
     # name: (batch, h, w, cin, cout, k, mode)
     'up84_c1': (16, 272, 480, 256, 256, 3, 'relu'),
-    'up84_c1_actlo': (16, 272, 480, 256, 256, 3, 'actlo'),   # activations as (hi, lo), two fp16 MMA passes
     # what up_8_4.out_conv.c1 runs in the parity plan: an e4m3 correction pass over the low-order activations, then the
     # fp16 pass, writing the ReLU'd output and its e4m3 low-order part for the next layer
     'up84_c1_lo8': (16, 272, 480, 256, 256, 3, 'actlo8'),
@@ -42,14 +41,14 @@ def run(name, iters=8):
     two = mode in ('two', 'gates', 'two192')
     wgt = torch.randn(cout, cin * (2 if two else 1), k, k, device=dev, generator=g) / (cin * k * k)**0.5
     bias = torch.randn(cout, device=dev, generator=g)
-    pc = ops.PackedConv(wgt, bias, 1, two_inputs=two, precise=(mode == 'precise'), act_lo=(mode == 'actlo'),
-                        act_lo8=mode.startswith('actlo8'), gates=(mode == 'gates'), nt_override=192 if mode == 'two192' else None)
+    pc = ops.PackedConv(wgt, bias, 1, two_inputs=two, precise=(mode == 'precise'), act_lo8=mode.startswith('actlo8'),
+                        gates=(mode == 'gates'), nt_override=192 if mode == 'two192' else None)
     kw = {}
     if two:
         kw['x2'] = torch.randn_like(x)
     if mode == 'gates':
         kw['gate_h'] = kw['x2']
-    if mode in ('precise', 'actlo'):
+    if mode == 'precise':
         kw['x_lo'] = (torch.randn_like(x) * 1e-3)
     if mode.startswith('actlo8'):  # e4m3 of (x - fp16(x)) * 4096
         kw['x_lo8'] = (torch.randn_like(x, dtype=torch.float32) * 4).to(torch.float8_e4m3fn).view(torch.uint8)
@@ -60,12 +59,12 @@ def run(name, iters=8):
     if 'head' in mode:
         kw['head_w'] = torch.randn(9, cout, device=dev, generator=g)
     want = dict(want_relu=True) if mode in ('relu', ) else (dict() if mode == 'gates' else dict(want_raw=True))
-    if mode in ('precise', 'actlo'):
+    if mode == 'precise':
         want = dict(want_relu=True, want_lo=True)
     if mode == 'actlo8':
         want = dict(want_relu=True, want_relu_lo8=True)
     # fp16-equivalent MMA passes; the e4m3 pass does the same MACs at twice the rate, so it counts as half a pass
-    passes = 3 if mode == 'precise' else (2 if (two or mode == 'actlo') else (1.5 if mode.startswith('actlo8') else 1))
+    passes = 3 if mode == 'precise' else (2 if two else (1.5 if mode.startswith('actlo8') else 1))
     flops = 2.0 * b * h * w * cout * k * k * pc.cin_pad * passes
     for _ in range(3):
         ops.conv_ex(x, pc, **kw, **want)

@@ -37,8 +37,6 @@ def main():
     p4 = torch.randn(K, 4 * h, 4 * w, 256, device=dev).half()
     rec('area_down x4 (256ch @1/4)', timeit(lambda: ops.area_down(p4, 4)), p4.numel() * 2 * (1 + 1 / 16))
     rec('area_down x2 (256ch @1/8)', timeit(lambda: ops.area_down(p8, 2)), p8.numel() * 2 * 1.25)
-    vals = torch.randn(K, h, w, 1536, device=dev).half(); hid = torch.randn(K, h, w, 512, device=dev).half()
-    rec('gru gates', timeit(lambda: ops.gru(vals, hid)), vals.numel() * 2 + 2 * hid.numel() * 2)
     img = torch.randn(1, 3, H, W, device=dev)
     rec('stem_im2col image (hi+lo, K=192)', timeit(lambda: ops.stem_columns(img, 192, with_lo=True)), img.numel() * 4 + 2 * (H // 2) * (W // 2) * 192 * 2)
     masks = torch.rand(K, 1, H, W, device=dev)

@@ -36,14 +36,14 @@ def main():
     def conv_ex(x, pc, **kw):
         b, h, w, _ = x.shape
         ho, wo = pc.out_hw(h, w)
-        passes = 3 if pc.precise else (2 if (pc.two_inputs or pc.act_lo or pc.w_lo) else 1)
+        passes = 3 if pc.precise else (2 if (pc.two_inputs or pc.w_lo) else 1)
         fl = 2.0 * b * ho * wo * pc.cout * pc.k * pc.k * pc.cin_pad * passes  # EXECUTED flops (all MMA passes)
         if kw.get('ksplit', 0) > 1:  # inner call of a chained split-precision conv: already inside the outer record
             return orig_conv(x, pc, **kw)
         return timed('conv:' + names.get(id(pc), '?') + (f' [{passes} passes]' if passes > 1 else ''), fl, orig_conv, x, pc, **kw)
     ops.conv_ex = conv_ex
     for fn in ('maxpool', 'up2_add', 'up2_add_split', 'area_down', 'area_down_plane', 'cbam_residual', 'cbam_residual_split',
-               'gru', 'stem_columns'):
+               'stem_columns'):
         o = getattr(ops, fn)
         setattr(ops, fn, (lambda o, fn: lambda *aa, **kw: timed('ew:' + fn, 0, o, *aa, **kw))(o, fn))
     for fn in ('pack_query', 'sim_topk', 'readout', 'output_tail', 'key_tail', 'pack_keys', 'transpose_append', 'nchw_to_nhwc', 'readout_sparse', 'head_gather3x3'):

@@ -64,18 +64,6 @@ DEVA_B200_API int deva_b200_device_check(void) {
   return 0;
 }
 
-DEVA_B200_API int deva_b200_enable_peer_access(int device, int peer_device) {
-  int prev = 0, can = 0;
-  B200_CUDA(cudaGetDevice(&prev));
-  B200_CUDA(cudaDeviceCanAccessPeer(&can, device, peer_device));
-  B200_REQUIRE(can, "device %d has no peer-to-peer path to device %d", device, peer_device);
-  B200_CUDA(cudaSetDevice(device));
-  cudaError_t e = cudaDeviceEnablePeerAccess(peer_device, 0);
-  if (e == cudaErrorPeerAccessAlreadyEnabled) { (void)cudaGetLastError(); e = cudaSuccess; }
-  (void)cudaSetDevice(prev);
-  B200_CUDA(e);
-  return 0;
-}
 DEVA_B200_API int deva_b200_peer_alloc(int device, int64_t bytes, void** ptr, uint8_t handle[64]) {
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
   B200_REQUIRE(bytes > 0 && ptr && handle, "peer_alloc: bad arguments");

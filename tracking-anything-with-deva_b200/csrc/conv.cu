@@ -718,14 +718,12 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
   const int n_src = (d.x2 || d.x_lo) ? 2 : 1;
   int pass_src[3] = {0, 0, 0}, pass_w[3] = {0, 0, 0}, n_pass = 1, w_groups = 1;
   if (d.x2) { n_pass = 2; pass_src[1] = 1; pass_w[1] = 1; w_groups = 2; }          // cat[x, x2] . [W0 | W1]
-  B200_REQUIRE(d.split_mode >= 0 && d.split_mode <= 3, "conv: split_mode %d unknown", d.split_mode);
-  B200_REQUIRE(d.split_mode != 1 || d.x_lo, "conv: split_mode 1 (activation hi/lo) needs x_lo");
+  B200_REQUIRE(d.split_mode == 0 || d.split_mode == 2 || d.split_mode == 3, "conv: split_mode %d unknown", d.split_mode);
   B200_REQUIRE(d.split_mode != 2 || (!d.x_lo && !d.x2), "conv: split_mode 2 (weight hi/lo) takes a single input");
   B200_REQUIRE(d.split_mode != 3 || (d.x_lo8 && d.w8_packed && !d.x_lo && !d.x2 && d.stride == 1 && d.cin_pad % 128 == 0 &&
                                      d.ksplit <= 1),
                "conv: split_mode 3 (fp8 correction pass) needs x_lo8 + w8_packed, stride 1, cin_pad %% 128 == 0, no x_lo / x2 / ksplit");
-  if (d.split_mode == 1) { n_pass = 2; pass_src[1] = 1; pass_w[1] = 0; }                    // Xh.W + Xl.W
-  else if (d.split_mode == 2) { n_pass = 2; pass_src[1] = 0; pass_w[1] = 1; w_groups = 2; }  // X.Wh + X.Wl
+  if (d.split_mode == 2) { n_pass = 2; pass_src[1] = 0; pass_w[1] = 1; w_groups = 2; }  // X.Wh + X.Wl
   else if (d.x_lo) { n_pass = 3; pass_src[1] = 1; pass_w[1] = 0; pass_src[2] = 0; pass_w[2] = 1; w_groups = 2; }  // Xh.Wh + Xl.Wh + Xh.Wl
   p.taps16 = ktaps * n_pass;
   p.taps = p.taps16 + (d.split_mode == 3 ? ktaps : 0);  // fp8 correction: one more pass, 128 channels per k-iteration

@@ -1,8 +1,7 @@
 // HBM-bound helper kernels of the NHWC fp16 network path: layout/precision conversion at the API boundary,
-// max-pool, bilinear x2 + skip add, area down-sampling, CBAM (reference deva/model/cbam.py:21-77), the
-// non-standard sensory GRU (modules.py:145-149), and the soft-aggregation / x4 upsampling / softmax tail
-// (network.py:33-40,144-168).  One thread per output element (or per pixel x channel-vector); all accesses
-// are coalesced along the channel axis.
+// max-pool, bilinear x2 + skip add, area down-sampling, CBAM (reference deva/model/cbam.py:21-77), and the
+// soft-aggregation / x4 upsampling / softmax tail (network.py:33-40,144-168).  One thread per output element (or per
+// pixel x channel-vector); all accesses are coalesced along the channel axis.
 #include <algorithm>
 #include <climits>
 #include <cuda_fp16.h>
@@ -43,18 +42,6 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, __half* __res
     const int y = (int)(p % H);
     const int b = (int)(p / H);
     dst[i] = (c < C) ? __float2half_rn(src[(((long long)b * C + c) * H + y) * W + x]) : __float2half_rn(0.f);
-  }
-}
-// fp16 NHWC [B,H,W,C] -> fp32 NCHW [B,C,H,W]
-__global__ void nhwc_to_nchw_kernel(const __half* __restrict__ src, float* __restrict__ dst, int B, int C, int H, int W) {
-  const long long total = (long long)B * C * H * W;
-  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
-    const int x = (int)(i % W);
-    long long p = i / W;
-    const int y = (int)(p % H); p /= H;
-    const int c = (int)(p % C);
-    const int b = (int)(p / C);
-    dst[i] = __half2float(src[(((long long)b * H + y) * W + x) * C + c]);
   }
 }
 // im2col for the 7x7 stride-2 pad-3 stems (resnet.py:120): planes fp32 [B, C, H, W] -> fp16 [B, H/2, W/2, Kp]
@@ -274,8 +261,7 @@ __device__ __forceinline__ void st8_split(__half* hi, __half* lo, const float (&
 __global__ void __launch_bounds__(256)
 up2_add_split_kernel(const __half* __restrict__ g, const __half* __restrict__ g_lo, const __half* __restrict__ skip,
                      const __half* __restrict__ skip_lo, __half* __restrict__ raw, __half* __restrict__ raw_lo,
-                     __half* __restrict__ relu, __half* __restrict__ relu_lo, unsigned char* __restrict__ relu_lo8, int B,
-                     int h, int w, int C) {
+                     __half* __restrict__ relu, unsigned char* __restrict__ relu_lo8, int B, int h, int w, int C) {
   // A thread owns 8 channels of the 2 x 2 OUTPUT block {2k-1, 2k} x {2j-1, 2j}: with align_corners = False these four
   // pixels interpolate between the same four source pixels (rows k-1, k / columns j-1, j, clamped at the border) with
   // weights 0.25 / 0.75, so the source quad (hi + lo) is loaded once per four outputs and there is no serial walk:
@@ -326,11 +312,7 @@ up2_add_split_kernel(const __half* __restrict__ g, const __half* __restrict__ g_
         }
         const long long off = (((long long)b * H + Y) * W + X) * C + c;
         if (raw) st8_split(raw + off, raw_lo + off, o);
-        if (relu_lo) {
-#pragma unroll
-          for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], 0.f);
-          st8_split(relu + off, relu_lo + off, o);
-        } else if (relu_lo8) {  // low-order part as e4m3 of (x - fp16(x)) * 4096: operand of an fp8 correction pass
+        if (relu_lo8) {  // low-order part as e4m3 of (x - fp16(x)) * 4096: operand of an fp8 correction pass
           uint32_t w8[2];
 #pragma unroll
           for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], 0.f);
@@ -545,7 +527,7 @@ __global__ void cbam_apply_split_kernel(const __half* __restrict__ x, const __ha
                                         const float* __restrict__ gate, const float* __restrict__ stats,
                                         const float* __restrict__ ws, const float* __restrict__ bs,
                                         __half* __restrict__ raw, __half* __restrict__ raw_lo, __half* __restrict__ relu,
-                                        __half* __restrict__ relu_lo, int B, int H, int W, int C) {
+                                        int B, int H, int W, int C) {
   const long long pix = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (pix >= (long long)B * H * W) return;
@@ -571,36 +553,7 @@ __global__ void cbam_apply_split_kernel(const __half* __restrict__ x, const __ha
       o[e] = t + t * g[c + e] * sg;
     }
     st8_split(raw + pix * C + c, raw_lo + pix * C + c, o);
-    if (relu) {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], 0.f);
-      if (relu_lo) st8_split(relu + pix * C + c, relu_lo + pix * C + c, o);
-      else st8(relu + pix * C + c, o, false);
-    }
-  }
-}
-
-// ---------------------------------------------------------------- sensory GRU (modules.py:145-149, quirk Q7)
-// values fp16 NHWC [B,HW,3C] = [forget | update | new]; h fp16 [B,HW,C] -> h' = f*h*(1-u) + u*tanh(n)
-__global__ void __launch_bounds__(256)
-gru_kernel(const __half* __restrict__ values, const __half* __restrict__ h, __half* __restrict__ out, long long pixels, int C) {
-  const int C8 = C / 8;
-  const long long total = pixels * C8;
-  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
-    const long long p = i / C8;
-    const int c = (int)(i - p * C8) * 8;
-    const __half* v = values + p * 3 * C + c;
-    float f[8], u[8], n[8], hv[8], o[8];
-    ld8(v, f);
-    ld8(v + C, u);
-    ld8(v + 2 * C, n);
-    ld8(h + p * C + c, hv);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const float fg = sigmoidf_(f[e]), ug = sigmoidf_(u[e]);
-      o[e] = fg * hv[e] * (1.f - ug) + ug * tanhf(n[e]);
-    }
-    st8(out + p * C + c, o, false);
+    if (relu) st8(relu + pix * C + c, o, true);
   }
 }
 
@@ -796,11 +749,6 @@ DEVA_B200_API int deva_b200_nchw_to_nhwc(const float* src, void* dst, int b, int
   B200_LAUNCH_CHECK();
   return 0;
 }
-DEVA_B200_API int deva_b200_nhwc_to_nchw(const void* src, float* dst, int b, int c, int h, int w, deva_stream_t stream) {
-  ew::nhwc_to_nchw_kernel<<<grid_of((long long)b * c * h * w), 256, 0, S(stream)>>>(H(src), dst, b, c, h, w);
-  B200_LAUNCH_CHECK();
-  return 0;
-}
 DEVA_B200_API int deva_b200_stem_im2col(const float* src, void* dst, void* dst_lo, int b, int c, int h, int w, int k_pad,
                                         deva_stream_t stream) {
   B200_REQUIRE(h % 2 == 0 && w % 2 == 0 && k_pad % 64 == 0 && k_pad >= 49 * c, "stem_im2col: bad shape");
@@ -843,14 +791,13 @@ DEVA_B200_API int deva_b200_up2_add(const void* g, const void* skip, void* raw, 
   return 0;
 }
 DEVA_B200_API int deva_b200_up2_add_split(const void* g, const void* g_lo, const void* skip, const void* skip_lo,
-                                          void* raw, void* raw_lo, void* relu, void* relu_lo, void* relu_lo8, int b, int h,
-                                          int w, int c, deva_stream_t stream) {
-  B200_REQUIRE(c % 8 == 0 && g_lo && (raw != nullptr) == (raw_lo != nullptr) && (raw || relu) && (!relu_lo || relu) &&
-                   (!relu_lo8 || (relu && !relu_lo)),
+                                          void* raw, void* raw_lo, void* relu, void* relu_lo8, int b, int h, int w, int c,
+                                          deva_stream_t stream) {
+  B200_REQUIRE(c % 8 == 0 && g_lo && (raw != nullptr) == (raw_lo != nullptr) && (raw || relu) && (!relu_lo8 || relu),
                "up2_add_split: C %% 8, g_lo, and raw/raw_lo (both or neither) with at least one output are required");
   ew::up2_add_split_kernel<<<dim3(ceil_div((w + 1) * (c / 8), 256), b * (h + 1)), 256, 0, S(stream)>>>(
-      H(g), H(g_lo), H(skip), H(skip_lo), H(raw), H(raw_lo), H(relu), H(relu_lo), reinterpret_cast<unsigned char*>(relu_lo8),
-      b, h, w, c);
+      H(g), H(g_lo), H(skip), H(skip_lo), H(raw), H(raw_lo), H(relu), reinterpret_cast<unsigned char*>(relu_lo8), b, h, w,
+      c);
   B200_LAUNCH_CHECK();
   return 0;
 }
@@ -892,8 +839,7 @@ DEVA_B200_API int deva_b200_cbam(const void* x, const float* w1, const float* b1
 }
 DEVA_B200_API int deva_b200_cbam_split(const void* x, const void* x_lo, const float* w1, const float* b1, const float* w2,
                                        const float* b2, const float* ws, const float* bs, float* scratch, void* raw,
-                                       void* raw_lo, void* relu, void* relu_lo, int pool_lo, int b, int h, int w, int c,
-                                       int r, deva_stream_t stream) {
+                                       void* raw_lo, void* relu, int b, int h, int w, int c, int r, deva_stream_t stream) {
   // the gate statistics are pooled over x + x_lo as well: a gate error is common to every channel of a pixel, so it
   // does not average out in the next convolution the way independent roundings do
   B200_REQUIRE(x_lo && raw && raw_lo, "cbam_split: the hi/lo tensors are required");
@@ -906,22 +852,15 @@ DEVA_B200_API int deva_b200_cbam_split(const void* x, const void* x_lo, const fl
   float* stats = gate + (long long)b * c;
   const int HW = h * w;
   B200_REQUIRE(c % 8 == 0 && c / 8 <= 256 && 256 % (c / 8) == 0, "cbam_split: C = %d must be 8 x a divisor of 256", c);
-  ew::cbam_pool_kernel<<<dim3(b, ew::kPoolSplit), 256, 0, s>>>(xh, pool_lo ? xl : nullptr, psum, pmax, HW, c);
+  ew::cbam_pool_kernel<<<dim3(b, ew::kPoolSplit), 256, 0, s>>>(xh, xl, psum, pmax, HW, c);
   B200_LAUNCH_CHECK();
   ew::cbam_mlp_kernel<<<b, 256, (2 * c + 2 * r) * sizeof(float), s>>>(psum, pmax, HW, w1, b1, w2, b2, gate, c, r);
   B200_LAUNCH_CHECK();
   const long long warps = (long long)b * HW;
-  ew::cbam_stats_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(xh, pool_lo ? xl : nullptr, gate, stats, b, HW, c);
+  ew::cbam_stats_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(xh, xl, gate, stats, b, HW, c);
   B200_LAUNCH_CHECK();
   ew::cbam_apply_split_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(xh, xl, gate, stats, ws, bs, H(raw), H(raw_lo),
-                                                                        H(relu), H(relu_lo), b, h, w, c);
-  B200_LAUNCH_CHECK();
-  return 0;
-}
-DEVA_B200_API int deva_b200_gru(const void* values, const void* h, void* out, int64_t pixels, int c,
-                                deva_stream_t stream) {
-  B200_REQUIRE(c % 8 == 0, "gru: C %% 8");
-  ew::gru_kernel<<<grid_of(pixels * (c / 8)), 256, 0, S(stream)>>>(H(values), H(h), H(out), pixels, c);
+                                                                        H(relu), b, h, w, c);
   B200_LAUNCH_CHECK();
   return 0;
 }

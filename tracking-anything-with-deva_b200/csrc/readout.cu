@@ -241,7 +241,7 @@ struct SpParams {
   // of the rank that owns the object, rank_dst[owner[g]] + out_row[g] * ldo, instead of stored to `out`
   float* rank_dst[kMaxPeers];
   unsigned char owner[kMaxGroups];
-  int reduce;
+  bool reduce;
 };
 
 // Raise the stage's expected transaction bytes without arriving (the arrive follows once the affinity tile is built).
@@ -348,7 +348,7 @@ readout_sparse_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_co
         const long long obj = R / p.rows_per_group;
         __half* dt = p.out_tok ? p.out_tok + (obj * p.q) * p.rows_per_group + (R - obj * p.rows_per_group) : nullptr;
         if (p.reduce) {  // partial sums of this rank's slots -> the owner's buffer (peer memory or local)
-          const bool vec = p.reduce == 1 && p.ldo % 2 == 0;  // 8-byte vector reductions
+          const bool vec = p.ldo % 2 == 0;  // 8-byte vector reductions need 8-byte aligned rows
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
             const int q = n * BN + 8 * j + 2 * qd;
@@ -456,9 +456,7 @@ static int readout_sparse(const void* values, int64_t values_ld, int64_t values_
   uint32_t* entries = reinterpret_cast<uint32_t*>(offsets + (size_t)p.n_tiles * (p.k_blocks + 1));
   p.offsets = offsets; p.entries = entries;
   for (int i = 0; i < n_groups; ++i) { p.val_row[i] = val_row[i]; p.out_row[i] = out_row[i]; }
-  // DEVA_B200_SCATTER_RED=scalar: one 4-byte reduction per element instead of red.add.v2 (debugging aid)
-  static const bool scalar_red = [] { const char* e = getenv("DEVA_B200_SCATTER_RED"); return e && e[0] == 's'; }();
-  p.reduce = rank_dst ? (scalar_red ? 2 : 1) : 0;
+  p.reduce = rank_dst != nullptr;
   if (rank_dst) {
     for (int r = 0; r < n_ranks; ++r) p.rank_dst[r] = rank_dst[r];
     for (int i = 0; i < n_groups; ++i) {

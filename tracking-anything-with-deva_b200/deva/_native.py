@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 17
+ABI_VERSION = 18
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -62,7 +62,6 @@ _SIGNATURES = {
     'deva_b200_readout_sparse_scatter': (c_int, [c_void_p, c_int64, c_int64, POINTER(c_int32), POINTER(c_int32),
                                                  POINTER(c_int32), c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                                  c_void_p, POINTER(c_void_p), c_int, c_int64, c_void_p]),
-    'deva_b200_enable_peer_access': (c_int, [c_int, c_int]),
     'deva_b200_peer_alloc': (c_int, [c_int, c_int64, POINTER(c_void_p), c_char_p]),
     'deva_b200_peer_open': (c_int, [c_int, c_char_p, POINTER(c_void_p)]),
     'deva_b200_peer_close': (c_int, [c_int, c_void_p]),
@@ -74,7 +73,6 @@ _SIGNATURES = {
     'deva_b200_conv2d': (c_int, [POINTER(ConvDesc), c_void_p]),
     'deva_b200_stem_im2col': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_nchw_to_nhwc': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
-    'deva_b200_nhwc_to_nchw': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_maxpool': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_up2_add': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_area_down': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -82,11 +80,10 @@ _SIGNATURES = {
     'deva_b200_cbam': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_up2_add_split': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                        c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+                                        c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_cbam_split': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
-                                     c_int, c_void_p]),
-    'deva_b200_gru': (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                     c_void_p]),
     'deva_b200_sum_parts': (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_int64, c_void_p]),
     'deva_b200_key_tail': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -267,10 +264,6 @@ def peer_free(device: int, ptr: int):
     _check(lib().deva_b200_peer_free(device, c_void_p(ptr)), 'peer_free')
 
 
-def enable_peer_access(device: int, peer_device: int):
-    _check(lib().deva_b200_enable_peer_access(device, peer_device), 'enable_peer_access')
-
-
 def gather_rows(dst, src, idx, n, row_bytes):
     _check(lib().deva_b200_gather_rows(_ptr(dst), _ptr(src), _ptr(idx), n, row_bytes, _stream()), 'gather_rows')
 
@@ -313,10 +306,6 @@ def nchw_to_nhwc(src, dst, b, c, h, w, c_pad):
     _check(lib().deva_b200_nchw_to_nhwc(_ptr(src), _ptr(dst), b, c, h, w, c_pad, _stream()), 'nchw_to_nhwc')
 
 
-def nhwc_to_nchw(src, dst, b, c, h, w):
-    _check(lib().deva_b200_nhwc_to_nchw(_ptr(src), _ptr(dst), b, c, h, w, _stream()), 'nhwc_to_nchw')
-
-
 def maxpool(x, y, b, h, w, c, x_lo=None, y_lo=None):
     _check(lib().deva_b200_maxpool(_ptr(x), _ptr(x_lo), _ptr(y), _ptr(y_lo), b, h, w, c, _stream()), 'maxpool')
 
@@ -338,19 +327,15 @@ def cbam(x, w1, b1, w2, b2, ws, bs, scratch, raw, relu, b, h, w, c, r):
                                 _ptr(raw), _ptr(relu), b, h, w, c, r, _stream()), 'cbam')
 
 
-def up2_add_split(g, g_lo, skip, raw, raw_lo, relu, b, h, w, c, skip_lo=None, relu_lo=None, relu_lo8=None):
+def up2_add_split(g, g_lo, skip, raw, raw_lo, relu, b, h, w, c, skip_lo=None, relu_lo8=None):
     _check(lib().deva_b200_up2_add_split(_ptr(g), _ptr(g_lo), _ptr(skip), _ptr(skip_lo), _ptr(raw), _ptr(raw_lo),
-                                         _ptr(relu), _ptr(relu_lo), _ptr(relu_lo8), b, h, w, c, _stream()), 'up2_add_split')
+                                         _ptr(relu), _ptr(relu_lo8), b, h, w, c, _stream()), 'up2_add_split')
 
 
-def cbam_split(x, x_lo, w1, b1, w2, b2, ws, bs, scratch, raw, raw_lo, relu, b, h, w, c, r, relu_lo=None, pool_lo=True):
+def cbam_split(x, x_lo, w1, b1, w2, b2, ws, bs, scratch, raw, raw_lo, relu, b, h, w, c, r):
     _check(lib().deva_b200_cbam_split(_ptr(x), _ptr(x_lo), _ptr(w1), _ptr(b1), _ptr(w2), _ptr(b2), _ptr(ws), _ptr(bs),
-                                      _ptr(scratch), _ptr(raw), _ptr(raw_lo), _ptr(relu), _ptr(relu_lo), int(pool_lo), b, h,
-                                      w, c, r, _stream()), 'cbam_split')
-
-
-def gru(values, h, out, pixels, c):
-    _check(lib().deva_b200_gru(_ptr(values), _ptr(h), _ptr(out), pixels, c, _stream()), 'gru')
+                                      _ptr(scratch), _ptr(raw), _ptr(raw_lo), _ptr(relu), b, h, w, c, r, _stream()),
+           'cbam_split')
 
 
 def sum_parts(parts, n_parts, part_stride, n, res=None, res_lo=None, raw=None, raw_lo=None, relu=None, relu_lo=None):

@@ -10,7 +10,6 @@ the math runs in the sm_90a kernels behind ``deva._native``:
 
 There is no PyTorch fallback for any of these.
 """
-import os
 from typing import Dict, List, Optional, Tuple
 
 import torch
@@ -54,7 +53,6 @@ class MemoryManager:
         # 'nhwc': match_memory returns fp16 token-major-backed views (what the native NHWC decoder consumes)
         self.readout_layout = 'nchw'
         self.fused_min_work = 16_000_000  # n_window * q above which the fused sparse-affinity readout is used
-        self.warm_start = os.environ.get('DEVA_B200_TOPK_WARM_START', '1') == '1'
         self.work_frames_without_long_term = 16  # bank capacity (frames) when long-term memory is disabled
 
     def _read_long_term_config(self, config: Dict) -> None:
@@ -183,7 +181,7 @@ class MemoryManager:
         if bank.read_idx is None or bank.read_idx.shape[0] != q or bank.read_idx.device != dev:
             bank.read_idx = torch.empty(q, nat.LIST_PITCH, dtype=torch.int32, device=dev)
             bank.read_key = None
-        prev = bank.read_idx if (self.warm_start and bank.read_key == key) else None
+        prev = bank.read_idx if bank.read_key == key else None
         bank.read_key = key
         return bank.read_idx, prev
 

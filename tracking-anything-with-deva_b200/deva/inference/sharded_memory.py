@@ -21,7 +21,6 @@ multiplied.  Each rank ends up with the complete readout of its K/R objects (wha
 the bulk all-reduce is gone, the only collectives left are the 2 MB all-gather of candidates (which also orders the
 zeroing of the buffers before the first remote add) and a one-element fence.
 """
-import os
 from typing import List, Optional, Tuple
 
 import torch
@@ -77,12 +76,6 @@ class PeerBuffers:
                 ptr = nat.peer_open(device.index, handles[r])
                 self._opened.append(ptr)
                 self.ptrs.append(ptr)
-                if os.environ.get('DEVA_B200_PEER_DEBUG'):  # read the peer's buffer with a kernel of THIS device
-                    idx = torch.arange(4, dtype=torch.int32, device=device)
-                    got = torch.empty(4, dtype=torch.float32, device=device)
-                    nat.gather_f32(got, torch.as_tensor(_RawCudaArray(ptr, (4, )), device=device), idx, 4)
-                    torch.cuda.synchronize(device)
-                    print(f'[peer-debug] rank {rank} read rank {r} buffer at {ptr:#x}: {got.tolist()}', flush=True)
             torch.cuda.synchronize(device)
             dist.barrier(group=group)
 

@@ -39,18 +39,18 @@ class PackedConv:
     """One convolution ready for ``deva_b200_conv2d``."""
     def __init__(self, weight: torch.Tensor, bias: Optional[torch.Tensor], stride: int,
                  rank1_in: Optional[int] = None, two_inputs: bool = False, precise: bool = False,
-                 gates: bool = False, act_lo: bool = False, w_lo: bool = False, act_lo8: bool = False,
+                 gates: bool = False, w_lo: bool = False, act_lo8: bool = False,
                  nt_override: Optional[int] = None):
         """weight [Cout, Cin, k, k] fp32 (BN folded); if ``rank1_in`` is given, that input channel is split
         off as a rank-1 term (out += w[:, rank1_in] * x1) - used for the '+1' mask / logit channels.
         ``gates``: Cout = [forget | update | new] x C of a sensory updater; rows are regrouped so that every
         192-channel tile holds the three gates of 64 hidden channels and the conv epilogue applies the update.
         Precision modes (exclusive): ``precise`` = inputs (hi, lo) x weights (hi, lo), three MMA passes, ~fp32;
-        ``act_lo`` = inputs (hi, lo) x single fp16 weights, two passes (no activation-operand rounding);
         ``w_lo`` = single fp16 input x weights (hi, lo), two passes (no weight rounding);
-        ``act_lo8`` = like act_lo with the low-order pass on the fp8 path: the activation remainder arrives as e4m3 of
-        (x - fp16(x)) * 4096, the weights are packed twice - fp16(W * 2^S) and e4m3(W * 2^(S-12)) - and the epilogue scales
-        the common accumulator by 2^-S; the correction pass covers 128 channels per k-iteration, i.e. costs half a pass."""
+        ``act_lo8`` = fp16 inputs plus a low-order pass on the fp8 path (no activation-operand rounding): the activation
+        remainder arrives as e4m3 of (x - fp16(x)) * 4096, the weights are packed twice - fp16(W * 2^S) and
+        e4m3(W * 2^(S-12)) - and the epilogue scales the common accumulator by 2^-S; the correction pass covers 128
+        channels per k-iteration, i.e. costs half a pass."""
         cout, cin, kh, kw = weight.shape
         self.gates = gates
         if gates:
@@ -70,10 +70,10 @@ class PackedConv:
             cin -= 1
         self.two_inputs = two_inputs
         self.precise = precise  # split precision: weights stored as fp16 (hi, lo), inputs arrive as (hi, lo)
-        self.act_lo, self.w_lo, self.act_lo8 = act_lo, w_lo, act_lo8
-        assert int(precise) + int(act_lo) + int(w_lo) + int(act_lo8) <= 1 and not (two_inputs and (precise or act_lo or w_lo or act_lo8))
-        self.split_mode = 1 if act_lo else (2 if w_lo else (3 if act_lo8 else 0))
-        self.takes_lo = precise or act_lo
+        self.w_lo, self.act_lo8 = w_lo, act_lo8
+        assert int(precise) + int(w_lo) + int(act_lo8) <= 1 and not (two_inputs and (precise or w_lo or act_lo8))
+        self.split_mode = 2 if w_lo else (3 if act_lo8 else 0)
+        self.takes_lo = precise
         self.takes_lo8 = act_lo8
         self.w8_packed, self.acc_scale = None, 0.0
         if two_inputs:  # the layer consumes cat[x, x2]: pack [cout, source, tap, cin/2]
@@ -179,7 +179,7 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
     # systematic relative error that the top-k read downstream of the key path does not tolerate
     # (tools/accum_probe.py measures it).  Longer loops run as chains of <= CHAIN k-iterations
     # whose fp32 partial sums are added - with the bias, the residual and the output conversions - by sum_parts.
-    k_iters = pc.k * pc.k * (pc.cin_pad // 64) * (3 if pc.precise else (2 if (pc.act_lo or pc.w_lo or pc.two_inputs) else 1))
+    k_iters = pc.k * pc.k * (pc.cin_pad // 64) * (3 if pc.precise else (2 if (pc.w_lo or pc.two_inputs) else 1))
     if (pc.precise and ksplit == 0 and k_iters > MAX_CHAIN and not (want_f32 or want_pool4 or head_w is not None or pc.rank1_w is not None)
             and pc.cout % 8 == 0 and (res is None or res.shape[0] == b)):
         parts = conv_ex(x, pc, x_lo=x_lo, want_f32=True, ksplit=-(-k_iters // CHAIN)).f32
@@ -206,7 +206,7 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
     if want_f32:
         o.f32 = new(torch.float32)
         if ksplit > 1:  # fp32 partial sums [parts, b, ho, wo, cout] of a split K loop; the consumer adds them
-            k_iters = pc.k * pc.k * (pc.cin_pad // 64) * (3 if pc.precise else (2 if (pc.act_lo or pc.w_lo or pc.two_inputs) else 1))
+            k_iters = pc.k * pc.k * (pc.cin_pad // 64) * (3 if pc.precise else (2 if (pc.w_lo or pc.two_inputs) else 1))
             per = -(-k_iters // ksplit)
             o.f32 = torch.empty(-(-k_iters // per), b, ho, wo, pc.cout, dtype=torch.float32, device=dev)
     res_b = False
@@ -239,7 +239,7 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
     if PROFILE is not None:
         ev1.record()
         flops = 2.0 * b * ho * wo * pc.cout * pc.k * pc.k * pc.cin * (2 if pc.two_inputs else 1)
-        PROFILE.append((ev0, ev1, flops, 3 if pc.precise else (2 if (pc.act_lo or pc.w_lo) else (1.5 if pc.act_lo8 else 1))))
+        PROFILE.append((ev0, ev1, flops, 3 if pc.precise else (2 if pc.w_lo else (1.5 if pc.act_lo8 else 1))))
     return o
 
 
@@ -288,19 +288,18 @@ def up2_add(g: torch.Tensor, skip: torch.Tensor, want_raw=True, want_relu=True):
 
 
 def up2_add_split(g: torch.Tensor, g_lo: torch.Tensor, skip: torch.Tensor, skip_lo: Optional[torch.Tensor] = None,
-                  want_raw: bool = True, want_relu_lo: bool = False, want_relu_lo8: bool = False):
-    """(g + g_lo) bilinear x2 + (skip + skip_lo) -> (raw, raw_lo, relu, relu_lo): the residual stream stays a fp16
-    hi/lo pair; relu_lo only when the consumer runs a second activation pass."""
+                  want_raw: bool = True, want_relu_lo8: bool = False):
+    """(g + g_lo) bilinear x2 + (skip + skip_lo) -> (raw, raw_lo, relu, relu_lo8): the residual stream stays a fp16
+    hi/lo pair; relu_lo8 (the e4m3 remainder of relu) only when the consumer runs the fp8 correction pass."""
     b, h, w, c = g.shape
     assert skip.shape == (1, 2 * h, 2 * w, c) and g_lo.shape == g.shape
     assert skip_lo is None or skip_lo.shape == skip.shape
     new = lambda: torch.empty(b, 2 * h, 2 * w, c, dtype=torch.float16, device=g.device)  # noqa: E731
     raw, raw_lo = (new(), new()) if want_raw else (None, None)
     relu = new()
-    relu_lo = new() if want_relu_lo else None
     relu_lo8 = torch.empty(b, 2 * h, 2 * w, c, dtype=torch.uint8, device=g.device) if want_relu_lo8 else None
-    nat.up2_add_split(g, g_lo, skip, raw, raw_lo, relu, b, h, w, c, skip_lo=skip_lo, relu_lo=relu_lo, relu_lo8=relu_lo8)
-    return raw, raw_lo, relu, (relu_lo8 if want_relu_lo8 else relu_lo)
+    nat.up2_add_split(g, g_lo, skip, raw, raw_lo, relu, b, h, w, c, skip_lo=skip_lo, relu_lo8=relu_lo8)
+    return raw, raw_lo, relu, relu_lo8
 
 
 def area_down(x: torch.Tensor, r: int) -> torch.Tensor:
@@ -330,23 +329,12 @@ def cbam_residual(x: torch.Tensor, params: dict, want_raw=True, want_relu=True):
     return raw, relu
 
 
-CBAM_POOL_LO = os.environ.get('DEVA_B200_CBAM_POOL_LO', '1') == '1'
-
-
-def cbam_residual_split(x: torch.Tensor, x_lo: torch.Tensor, params: dict, want_relu_lo: bool = False):
-    """(x + x_lo) + CBAM(x + x_lo) -> (raw, raw_lo, relu, relu_lo)."""
+def cbam_residual_split(x: torch.Tensor, x_lo: torch.Tensor, params: dict):
+    """(x + x_lo) + CBAM(x + x_lo) -> (raw, raw_lo, relu)."""
     b, h, w, c = x.shape
     r = params['w1'].shape[0]
     scratch = torch.empty((2 * CBAM_POOL_SPLIT + 1) * b * c + 2 * b * h * w, dtype=torch.float32, device=x.device)
     raw, raw_lo, relu = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
-    relu_lo = torch.empty_like(x) if want_relu_lo else None
     nat.cbam_split(x, x_lo, params['w1'], params['b1'], params['w2'], params['b2'], params['ws'], params['bs'], scratch,
-                   raw, raw_lo, relu, b, h, w, c, r, relu_lo=relu_lo, pool_lo=CBAM_POOL_LO)
-    return raw, raw_lo, relu, relu_lo
-
-
-def gru(values: torch.Tensor, h: torch.Tensor) -> torch.Tensor:
-    """values fp16 [B,H,W,3C], h fp16 [B,H,W,C] -> new h."""
-    out = torch.empty_like(h)
-    nat.gru(values, h, out, h.numel() // h.shape[-1], h.shape[-1])
-    return out
+                   raw, raw_lo, relu, b, h, w, c, r)
+    return raw, raw_lo, relu
