@@ -27,7 +27,9 @@
 extern "C" {
 #endif
 
-/* v18: dropped conv split_mode 1, the split twins' relu_lo and hi-only pooling, gru, nhwc_to_nchw, enable_peer_access.
+/* v19: deva_b200_mask_stats(_workspace_bytes), deva_b200_mask_scored_argmax and deva_b200_mask_last_cover (detector
+ * masks -> detection id map).
+ * v18: dropped conv split_mode 1, the split twins' relu_lo and hi-only pooling, gru, nhwc_to_nchw, enable_peer_access.
  * v16: deva_b200_label_areas and deva_b200_label_to_index (unsupervised DAVIS 2017 object limit).
  * v15: deva_b200_pano_joint_hist and deva_b200_pano_remap (video panoptic metrics and stuff merging).
  * v14: deva_b200_prob_to_scores and deva_b200_scores_to_ids (multi-scale / flip score export and merge).
@@ -35,10 +37,11 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 18
+#define DEVA_B200_ABI_VERSION 19
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
+#define DEVA_B200_MASK_SMEM_COUNTERS 8192 /* per-mask counters of one mask call kept in shared memory, else global */
 
 typedef void* deva_stream_t; /* cudaStream_t */
 
@@ -371,6 +374,31 @@ DEVA_B200_API int deva_b200_label_areas(const uint8_t* frame, int h, int w, int 
  * sorted ascending (distinct), index int32 [n]; 2 n entries take at most 200 KiB (shared memory). */
 DEVA_B200_API int deva_b200_label_to_index(const uint8_t* frame, int h, int w, int channels, const int32_t* labels,
                                            const int32_t* index, int n, uint8_t* out, deva_stream_t stream);
+
+/* ---- detector masks -> detection id map (deva/ext/automatic_sam.py auto_segment, deva/ext/grounding_dino.py
+ * segment_with_text) ------------------------------------------------------------------------------------------------
+ * masks u8 [n, h, w] (a bool or uint8 mask stack's bytes).  Mask k's value v_k at an output pixel of [out_h, out_w] is
+ * the bilinear resize (align_corners = False, F.interpolate's arithmetic; a copy when the sizes are equal) of the bytes
+ * as floats.  Any n >= 0; per-mask counters live in shared memory up to DEVA_B200_MASK_SMEM_COUNTERS, in global memory
+ * beyond.  The calls initialise their outputs.
+ *
+ * area float [n]: fp32 sum of v_k over the output, deterministic (fixed partial slots added in a fixed order, no float
+ * atomics: equal masks get equal areas).  covered int32 [n]: pixels with v_k > 0.5.  Either may be null.  workspace:
+ * deva_b200_mask_stats_workspace_bytes(n, out_h, out_w) bytes. */
+DEVA_B200_API size_t deva_b200_mask_stats_workspace_bytes(int n, int out_h, int out_w);
+DEVA_B200_API int deva_b200_mask_stats(const uint8_t* masks, int n, int h, int w, int out_h, int out_w, void* workspace,
+                                       float* area, int32_t* covered, deva_stream_t stream);
+/* slot int32 [out_h, out_w]: slot of the first maximum of [0.1, v_0 * score[0], ..., v_{n-1} * score[n-1]] (0 = the
+ * 0.1 background, k + 1 = mask k); with kept_only, 0 wherever the winner's v < 0.5.  won / kept int32 [n + 1]: pixels
+ * each slot wins / wins with v >= 0.5.  score float [n]. */
+DEVA_B200_API int deva_b200_mask_scored_argmax(const uint8_t* masks, int n, int h, int w, int out_h, int out_w,
+                                               const float* score, int kept_only, int32_t* slot, int32_t* won,
+                                               int32_t* kept, deva_stream_t stream);
+/* slot int32 [out_h, out_w]: k + 1 for the last mask k of order int32 [n] (a permutation of 0..n-1, the paint order)
+ * with v_k > 0.5, 0 where there is none.  covered int32 [n]: pixels with v_k > 0.5, indexed by mask. */
+DEVA_B200_API int deva_b200_mask_last_cover(const uint8_t* masks, int n, int h, int w, int out_h, int out_w,
+                                            const int32_t* order, int32_t* slot, int32_t* covered,
+                                            deva_stream_t stream);
 
 #ifdef __cplusplus
 }

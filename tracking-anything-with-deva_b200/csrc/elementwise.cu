@@ -941,11 +941,16 @@ __device__ __forceinline__ ResizeTaps resize_taps(int h, int w, int out_h, int o
   return t;
 }
 // Value of one channel plane at the output pixel of `t`.  Every egress kernel reads its values through this one
-// function, so their id maps and scores come from the same float, bit for bit.
-__device__ __forceinline__ float resized_value(const float* __restrict__ plane, const ResizeTaps& t) {
-  const float* q = plane + t.off;
-  if (t.same) return q[0];
-  return t.ly0 * (t.lx0 * q[0] + t.lx1 * q[t.dx]) + t.ly1 * (t.lx0 * q[t.dy] + t.lx1 * q[t.dy + t.dx]);
+// function, so their id maps and scores come from the same float, bit for bit.  A uint8 plane (bool or byte masks) is
+// read as bytes and each tap converted to float, which is what resizing `masks.float()` computes.  For 0 / 1 masks the
+// compiled form (source index fma(r, o + 0.5, -0.5), row blend fma(ly0, top, ly1 * bot)) makes the same > 0.5 decisions
+// as torch's CPU resize, which segment_with_text's reference thresholds (tests/test_detector_masks_cpu.py).
+template <typename T>
+__device__ __forceinline__ float resized_value(const T* __restrict__ plane, const ResizeTaps& t) {
+  const T* q = plane + t.off;
+  if (t.same) return (float)q[0];
+  return t.ly0 * (t.lx0 * (float)q[0] + t.lx1 * (float)q[t.dx]) +
+         t.ly1 * (t.lx0 * (float)q[t.dy] + t.lx1 * (float)q[t.dy + t.dx]);
 }
 
 // Channel of the first maximum of prob [c, h, w] resized to [out_h, out_w], at output pixel (oy, ox); channels
@@ -1167,6 +1172,147 @@ mask_gather_kernel(const unsigned char* __restrict__ src, int w, int out_h, int 
   const int oy = (int)(i / out_w), ox = (int)(i - (long long)oy * out_w);
   dst[i] = src[(long long)y_idx[oy] * w + x_idx[flip ? out_w - 1 - ox : ox]];
 }
+
+// ---------------------------------------------------------------- detector masks -> detection id map
+// (deva/ext/automatic_sam.py auto_segment, deva/ext/grounding_dino.py segment_with_text).  Masks are uint8 [n, h, w]
+// (a bool tensor's bytes), resized to [out_h, out_w] on the fly through resize_taps / resized_value.
+constexpr int kMaskStatsPix = 8192;  // output pixels per statistics block: fixes which pixels each partial sum holds
+constexpr int kMaskSmemCounters = DEVA_B200_MASK_SMEM_COUNTERS;
+
+// Statistics, pass 1: block (chunk p, mask k) sums the resized values of mask k over output pixels
+// [p * kMaskStatsPix, (p + 1) * kMaskStatsPix) in a fixed order (per thread, then a fixed shared-memory tree) and counts
+// those > 0.5.  The partial sums land in fixed slots, so a mask's area is the same float on every call.
+__global__ void __launch_bounds__(256)
+mask_stats_partial_kernel(const unsigned char* __restrict__ masks, int n_masks, int h, int w, int out_h, int out_w,
+                          float rh, float rw, int chunks, float* __restrict__ part_area, int* __restrict__ part_cov) {
+  __shared__ float ss[256];
+  __shared__ int sc[256];
+  const long long n = (long long)out_h * out_w, plane = (long long)h * w;
+  const long long i0 = (long long)blockIdx.x * kMaskStatsPix, i1 = min(n, i0 + kMaskStatsPix);
+  for (int k = blockIdx.y; k < n_masks; k += gridDim.y) {
+    const unsigned char* m = masks + k * plane;
+    float s = 0.f;
+    int c = 0;
+    for (long long i = i0 + threadIdx.x; i < i1; i += 256) {
+      const int oy = (int)(i / out_w), ox = (int)(i - (long long)oy * out_w);
+      const float v = resized_value(m, resize_taps(h, w, out_h, out_w, rh, rw, oy, ox));
+      s += v;
+      c += v > 0.5f;
+    }
+    ss[threadIdx.x] = s;
+    sc[threadIdx.x] = c;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+      if (threadIdx.x < o) {
+        ss[threadIdx.x] += ss[threadIdx.x + o];
+        sc[threadIdx.x] += sc[threadIdx.x + o];
+      }
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+      part_area[(long long)k * chunks + blockIdx.x] = ss[0];
+      part_cov[(long long)k * chunks + blockIdx.x] = sc[0];
+    }
+    __syncthreads();
+  }
+}
+// Statistics, pass 2: area[k] = the partial sums of mask k added in chunk order; covered[k] likewise.
+__global__ void __launch_bounds__(256)
+mask_stats_reduce_kernel(const float* __restrict__ part_area, const int* __restrict__ part_cov, int n_masks, int chunks,
+                         float* __restrict__ area, int* __restrict__ covered) {
+  const int k = blockIdx.x * 256 + threadIdx.x;
+  if (k >= n_masks) return;
+  float s = 0.f;
+  int c = 0;
+  for (int p = 0; p < chunks; ++p) {
+    s += part_area[(long long)k * chunks + p];
+    c += part_cov[(long long)k * chunks + p];
+  }
+  if (area) area[k] = s;
+  if (covered) covered[k] = c;
+}
+
+// Adds 1 to counter[key] for every active lane of the warp: one atomic per distinct key (the background slot is what
+// most pixels of a block share).  key < 0 adds nothing.
+__device__ __forceinline__ void warp_count(int* counter, int key) {
+  const unsigned peers = __match_any_sync(__activemask(), key);
+  if (key >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&counter[key], __popc(peers));
+}
+
+// Scored argmax: per output pixel the slot of the first maximum of [0.1, v_0 * s_0, ..., v_{n-1} * s_{n-1}] (slot 0 is
+// the background, slot k + 1 mask k).  won[slot] counts the pixels each slot wins, kept[slot] those where the winner's
+// own value is >= 0.5.  slot_out gets the winning slot, or with kept_only the winning slot where it is kept and 0
+// elsewhere.  Counters in shared memory when 2 (n + 1) fit in kMaskSmemCounters, in global memory otherwise.
+__global__ void __launch_bounds__(256)
+mask_scored_argmax_kernel(const unsigned char* __restrict__ masks, int n_masks, int h, int w, int out_h, int out_w,
+                          float rh, float rw, const float* __restrict__ score, int kept_only, int* __restrict__ slot_out,
+                          int* __restrict__ won, int* __restrict__ kept, int smem_counters) {
+  extern __shared__ int counters[];
+  const int slots = n_masks + 1;
+  int* cw = smem_counters ? counters : won;
+  int* ck = smem_counters ? counters + slots : kept;
+  if (smem_counters) {
+    for (int k = threadIdx.x; k < 2 * slots; k += 256) counters[k] = 0;
+    __syncthreads();
+  }
+  const long long n = (long long)out_h * out_w, plane = (long long)h * w;
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+    const int oy = (int)(i / out_w), ox = (int)(i - (long long)oy * out_w);
+    const ResizeTaps t = resize_taps(h, w, out_h, out_w, rh, rw, oy, ox);
+    int best = 0;
+    float best_s = 0.1f, best_v = 0.f;
+    for (int k = 0; k < n_masks; ++k) {
+      const float v = resized_value(masks + k * plane, t);
+      const float s = __fmul_rn(v, __ldg(score + k));
+      if (s > best_s) { best_s = s; best = k + 1; best_v = v; }
+    }
+    const bool keep = best > 0 && best_v >= 0.5f;
+    slot_out[i] = (kept_only && !keep) ? 0 : best;
+    warp_count(cw, best);
+    warp_count(ck, keep ? best : -1);
+  }
+  if (smem_counters) {
+    __syncthreads();
+    for (int k = threadIdx.x; k < slots; k += 256) {
+      if (counters[k]) atomicAdd(&won[k], counters[k]);
+      if (counters[slots + k]) atomicAdd(&kept[k], counters[slots + k]);
+    }
+  }
+}
+
+// Last cover: per output pixel the slot (k + 1) of the last mask k in `order` whose resized value is > 0.5, 0 when
+// none; covered[k] counts the pixels where mask k is > 0.5.  Counters as in mask_scored_argmax_kernel (n of them).
+__global__ void __launch_bounds__(256)
+mask_last_cover_kernel(const unsigned char* __restrict__ masks, int n_masks, int h, int w, int out_h, int out_w,
+                       float rh, float rw, const int* __restrict__ order, int* __restrict__ slot_out,
+                       int* __restrict__ covered, int smem_counters) {
+  extern __shared__ int counters[];
+  int* cc = smem_counters ? counters : covered;
+  if (smem_counters) {
+    for (int k = threadIdx.x; k < n_masks; k += 256) counters[k] = 0;
+    __syncthreads();
+  }
+  const long long n = (long long)out_h * out_w, plane = (long long)h * w;
+  for (long long i = blockIdx.x * 256ll + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+    const int oy = (int)(i / out_w), ox = (int)(i - (long long)oy * out_w);
+    const ResizeTaps t = resize_taps(h, w, out_h, out_w, rh, rw, oy, ox);
+    const unsigned active = __activemask();
+    int last = 0;
+    for (int j = 0; j < n_masks; ++j) {
+      const int k = __ldg(order + j);
+      const bool on = resized_value(masks + k * plane, t) > 0.5f;
+      const unsigned b = __ballot_sync(active, on);
+      if (b && (threadIdx.x & 31) == __ffs(active) - 1) atomicAdd(&cc[k], __popc(b));
+      if (on) last = k + 1;
+    }
+    slot_out[i] = last;
+  }
+  if (smem_counters) {
+    __syncthreads();
+    for (int k = threadIdx.x; k < n_masks; k += 256)
+      if (counters[k]) atomicAdd(&covered[k], counters[k]);
+  }
+}
 }  // namespace ew
 
 }  // namespace b200
@@ -1263,6 +1409,61 @@ DEVA_B200_API int deva_b200_prob_to_segments(const float* prob, int c, int h, in
   ew::prob_to_segments_kernel<<<(unsigned)blocks, 256, smem, s>>>(prob, c, h, w, out_h, out_w, (float)h / out_h,
                                                                    (float)w / out_w, lut, rgb, frame, out_u8, out_rgb,
                                                                    out_overlay, counts_u64, boxes);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+DEVA_B200_API size_t deva_b200_mask_stats_workspace_bytes(int n, int out_h, int out_w) {
+  const long long chunks = ((long long)out_h * out_w + ew::kMaskStatsPix - 1) / ew::kMaskStatsPix;
+  return (size_t)(n < 0 ? 0 : n) * (size_t)chunks * (sizeof(float) + sizeof(int));
+}
+DEVA_B200_API int deva_b200_mask_stats(const uint8_t* masks, int n, int h, int w, int out_h, int out_w, void* workspace,
+                                       float* area, int32_t* covered, deva_stream_t stream) {
+  B200_REQUIRE(n >= 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0 && (n == 0 || (masks && workspace && (area || covered))),
+               "mask_stats: bad arguments");
+  if (n == 0) return 0;
+  const cudaStream_t s = S(stream);
+  const int chunks = ceil_div((long long)out_h * out_w, ew::kMaskStatsPix);
+  float* part_area = reinterpret_cast<float*>(workspace);
+  int* part_cov = reinterpret_cast<int*>(part_area + (long long)n * chunks);
+  ew::mask_stats_partial_kernel<<<dim3(chunks, std::min(n, 65535)), 256, 0, s>>>(
+      masks, n, h, w, out_h, out_w, (float)h / out_h, (float)w / out_w, chunks, part_area, part_cov);
+  B200_LAUNCH_CHECK();
+  ew::mask_stats_reduce_kernel<<<ceil_div(n, 256), 256, 0, s>>>(part_area, part_cov, n, chunks, area, covered);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+DEVA_B200_API int deva_b200_mask_scored_argmax(const uint8_t* masks, int n, int h, int w, int out_h, int out_w,
+                                               const float* score, int kept_only, int32_t* slot, int32_t* won,
+                                               int32_t* kept, deva_stream_t stream) {
+  B200_REQUIRE(n >= 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0 && slot && won && kept && (n == 0 || (masks && score)),
+               "mask_scored_argmax: bad arguments");
+  const cudaStream_t s = S(stream);
+  B200_CUDA(cudaMemsetAsync(won, 0, (n + 1) * sizeof(int32_t), s));
+  B200_CUDA(cudaMemsetAsync(kept, 0, (n + 1) * sizeof(int32_t), s));
+  const long long pixels = (long long)out_h * out_w;
+  const bool smem = 2ll * (n + 1) <= ew::kMaskSmemCounters;
+  // with shared counters, fewer and longer-lived blocks amortise zeroing and flushing them
+  const long long blocks = smem ? std::min(ceil_div(pixels, 256), 4 * sm_count()) : ceil_div(pixels, 256);
+  const size_t bytes = smem ? 2ull * (n + 1) * sizeof(int) : 0;  // at most 32 KiB: no opt-in needed
+  ew::mask_scored_argmax_kernel<<<(unsigned)blocks, 256, bytes, s>>>(masks, n, h, w, out_h, out_w, (float)h / out_h,
+                                                                      (float)w / out_w, score, kept_only, slot, won, kept,
+                                                                      smem);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+DEVA_B200_API int deva_b200_mask_last_cover(const uint8_t* masks, int n, int h, int w, int out_h, int out_w,
+                                            const int32_t* order, int32_t* slot, int32_t* covered,
+                                            deva_stream_t stream) {
+  B200_REQUIRE(n >= 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0 && slot && (n == 0 || (masks && order && covered)),
+               "mask_last_cover: bad arguments");
+  const cudaStream_t s = S(stream);
+  if (n > 0) B200_CUDA(cudaMemsetAsync(covered, 0, n * sizeof(int32_t), s));
+  const long long pixels = (long long)out_h * out_w;
+  const bool smem = n <= ew::kMaskSmemCounters;
+  const long long blocks = smem ? std::min(ceil_div(pixels, 256), 4 * sm_count()) : ceil_div(pixels, 256);
+  const size_t bytes = smem ? (size_t)n * sizeof(int) : 0;
+  ew::mask_last_cover_kernel<<<(unsigned)blocks, 256, bytes, s>>>(masks, n, h, w, out_h, out_w, (float)h / out_h,
+                                                                   (float)w / out_w, order, slot, covered, smem);
   B200_LAUNCH_CHECK();
   return 0;
 }

@@ -12,10 +12,11 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 18
+ABI_VERSION = 19
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
+MASK_SMEM_COUNTERS = 8192
 
 _lib = None
 
@@ -111,6 +112,13 @@ _SIGNATURES = {
     'deva_b200_label_areas': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'deva_b200_label_to_index': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
                                          c_void_p]),
+    'deva_b200_mask_stats_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
+    'deva_b200_mask_stats': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                     c_void_p]),
+    'deva_b200_mask_scored_argmax': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                             c_void_p, c_void_p, c_void_p]),
+    'deva_b200_mask_last_cover': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                          c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -450,6 +458,55 @@ def label_to_index(frame, labels, index, out):
     assert out.dtype == torch.uint8 and out.shape == (h, w) and out.is_contiguous(), (out.dtype, out.shape)
     _check(lib().deva_b200_label_to_index(_ptr(frame), h, w, c, _ptr(labels), _ptr(index), labels.numel(), _ptr(out),
                                           _stream()), 'label_to_index')
+
+
+def _mask_stack(masks):
+    """uint8 view [n, h, w] of a contiguous bool / uint8 CUDA mask stack (no copy)."""
+    assert masks.is_cuda and masks.dim() == 3 and masks.is_contiguous(), (masks.device, masks.shape)
+    if masks.dtype == torch.bool:
+        masks = masks.view(torch.uint8)
+    if masks.dtype != torch.uint8:
+        raise TypeError(f'deva_b200: mask stacks are bool or uint8, not {masks.dtype}')
+    return masks
+
+
+def _i32(t, n):
+    assert t.dtype == torch.int32 and t.is_cuda and t.is_contiguous() and t.numel() == n, (t.dtype, t.shape, n)
+    return t
+
+
+def mask_stats(masks, out_h, out_w, area=None, covered=None):
+    """masks bool / uint8 [n, h, w] -> area float32 [n] (deterministic fp32 sums of the resized values) and / or covered
+    int32 [n] (resized values > 0.5), written into the given tensors."""
+    m = _mask_stack(masks)
+    n, h, w = m.shape
+    if area is not None:
+        assert _f32(area).numel() == n and area.is_contiguous()
+    if covered is not None:
+        _i32(covered, n)
+    ws = torch.empty(int(lib().deva_b200_mask_stats_workspace_bytes(n, out_h, out_w)), dtype=torch.uint8,
+                     device=m.device)
+    _check(lib().deva_b200_mask_stats(_ptr(m), n, h, w, out_h, out_w, _ptr(ws), _ptr(area), _ptr(covered), _stream()),
+           'mask_stats')
+
+
+def mask_scored_argmax(masks, out_h, out_w, score, kept_only, slot, won, kept):
+    """slot int32 [out_h, out_w]; won / kept int32 [n + 1]; score float32 [n] (see include/deva_b200.h)."""
+    m = _mask_stack(masks)
+    n, h, w = m.shape
+    assert _f32(score).numel() == n and score.is_contiguous()
+    _i32(slot, out_h * out_w), _i32(won, n + 1), _i32(kept, n + 1)
+    _check(lib().deva_b200_mask_scored_argmax(_ptr(m), n, h, w, out_h, out_w, _ptr(score), int(bool(kept_only)),
+                                              _ptr(slot), _ptr(won), _ptr(kept), _stream()), 'mask_scored_argmax')
+
+
+def mask_last_cover(masks, out_h, out_w, order, slot, covered):
+    """order int32 [n] (paint order); slot int32 [out_h, out_w]; covered int32 [n] (see include/deva_b200.h)."""
+    m = _mask_stack(masks)
+    n, h, w = m.shape
+    _i32(order, n), _i32(slot, out_h * out_w), _i32(covered, n)
+    _check(lib().deva_b200_mask_last_cover(_ptr(m), n, h, w, out_h, out_w, _ptr(order), _ptr(slot), _ptr(covered),
+                                           _stream()), 'mask_last_cover')
 
 
 def transpose_append(src, dst, ld_dst, n, c):
