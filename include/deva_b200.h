@@ -89,7 +89,10 @@ DEVA_B200_API int deva_b200_append_values(const float* src, int64_t ld_src, void
  *   affinity (optional): [q, ld_affinity] fp16 dense rows (zero-filled, top_k non-zeros per row) for
  *                        deva_b200_readout;
  *   use_cnt/life_cnt (optional): [n_window] fp32 counters; slots < n_long are long-term memory;
- *   count_long/count_work: which region(s) receive usage (+= affinity row sums) and life (+= 1). */
+ *   count_long/count_work: which region(s) receive usage (+= affinity row sums) and life (+= 1).
+ * Ties: the selection is the top_k of the window's slots [n_lead, n_window) under the order (similarity descending,
+ * slot ascending), where the similarity is the kernel's fp32 value; of bit-identical keys the lower slots are kept.
+ * The result is deterministic and the same with or without prev_idx. */
 DEVA_B200_API size_t deva_b200_simtopk_workspace_bytes(int q);
 DEVA_B200_API int deva_b200_sim_topk(const void* k_hi, const void* k_lo, const float* neg_s, int n_window, int n_lead,
                        const void* q_hi, const void* q_lo, const float* bsq, int q, int ck, int top_k,
@@ -99,7 +102,9 @@ DEVA_B200_API int deva_b200_sim_topk(const void* k_hi, const void* k_lo, const f
 /* prev_idx (optional, with thr_ws: [q] fp32 scratch): out_idx of the PREVIOUS read of the same window (same slot numbering;
  * may alias out_idx).  Temporal warm start: the similarities of those top_k slots to the current queries bound every
  * query's k-th best from below, so the streaming top-k inserts only the few candidates above that bound - the result
- * is unchanged (exact), the epilogue work drops several-fold.  Pass NULL after any compaction / re-numbering. */
+ * is unchanged (exact), the epilogue work drops several-fold.  Pass NULL after any compaction / re-numbering.  A row
+ * whose first top_k entries hold a slot outside [n_lead, n_window) or repeat a slot gives that query no bound (it is
+ * read cold), since fewer than top_k distinct slots bound nothing. */
 /* out_sim (optional): fp32 [q, 32] raw similarities of the selected slots (descending; -inf beyond top_k) - what a
  * bank-sharded read exchanges between ranks.
  *

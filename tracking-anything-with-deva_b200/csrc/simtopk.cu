@@ -73,19 +73,26 @@ __device__ __forceinline__ float pick32(const float (&v)[32], int j) {
 }
 
 // Per-thread running top-k: kListCap (32) candidate slots in a shared-memory column (entries >= top_k hold
-// +inf), tracked as 4 groups of 8 with the group minima (value, position) in registers.  Replacing the global
-// minimum re-scans only its group: 8 shared loads + a handful of selects per insertion.
+// +inf), tracked as 4 groups of 8 with the group minima (value, slot, position) in registers.  Replacing the global
+// minimum re-scans only its group: 16 shared loads + a handful of selects per insertion.
+// Entries are ranked by (similarity descending, slot ascending): of two equal similarities the higher slot is the
+// minimum and is evicted first.  A list scans its columns in ascending slot order and admits a column only above its
+// k-th best, so it always holds exactly the top-k of the columns it has seen under that order, whatever the history
+// of insertions (cold or warm-started).
 struct TopK {
   float gmin[4];
+  int gidx[4];
   int gpos[4];
   float thr;
   int minpos;
+  // (v, n) ranks below (u, m)
+  static __device__ __forceinline__ bool below(float v, int n, float u, int m) { return v < u || (v == u && n > m); }
   __device__ __forceinline__ void refresh() {
-    float m01 = gmin[0]; int p01 = gpos[0];
-    if (gmin[1] < m01) { m01 = gmin[1]; p01 = gpos[1]; }
-    float m23 = gmin[2]; int p23 = gpos[2];
-    if (gmin[3] < m23) { m23 = gmin[3]; p23 = gpos[3]; }
-    const bool c = m23 < m01;
+    float m01 = gmin[0]; int i01 = gidx[0], p01 = gpos[0];
+    if (below(gmin[1], gidx[1], m01, i01)) { m01 = gmin[1]; i01 = gidx[1]; p01 = gpos[1]; }
+    float m23 = gmin[2]; int i23 = gidx[2], p23 = gpos[2];
+    if (below(gmin[3], gidx[3], m23, i23)) { m23 = gmin[3]; i23 = gidx[3]; p23 = gpos[3]; }
+    const bool c = below(m23, i23, m01, i01);
     thr = c ? m23 : m01;
     minpos = c ? p23 : p01;
   }
@@ -94,17 +101,19 @@ struct TopK {
     li[minpos * BQ + row] = n;
     const int g = minpos >> 3;
     const float* base = lv + (g * 8) * BQ + row;
+    const int* ibase = li + (g * 8) * BQ + row;
     float x[8];
+    int y[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) x[e] = base[e * BQ];
-    float m = x[0]; int mp = 0;
+    for (int e = 0; e < 8; ++e) { x[e] = base[e * BQ]; y[e] = ibase[e * BQ]; }
+    float m = x[0]; int mi = y[0], mp = 0;
 #pragma unroll
     for (int e = 1; e < 8; ++e)
-      if (x[e] < m) { m = x[e]; mp = e; }
+      if (below(x[e], y[e], m, mi)) { m = x[e]; mi = y[e]; mp = e; }
     mp += g * 8;
 #pragma unroll
     for (int i = 0; i < 4; ++i)
-      if (i == g) { gmin[i] = m; gpos[i] = mp; }
+      if (i == g) { gmin[i] = m; gidx[i] = mi; gpos[i] = mp; }
     refresh();
   }
 };
@@ -192,13 +201,16 @@ simtopk_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       tk.gmin[i] = (i * 8 < top_k) ? -CUDART_INF_F : CUDART_INF_F;
+      tk.gidx[i] = -1;
       tk.gpos[i] = i * 8;
     }
     tk.refresh();
     // The two halves scan disjoint columns of the SAME queries into separate lists.  Each publishes its running k-th
     // best; the other's value is a valid lower bound of the query's global k-th best (its list holds k real candidates
     // at least that large), so gating on it keeps every global top-k member while cutting the insertions of two
-    // half-length lists to about those of one full-length list.  Stale reads are fine: the bound only grows.
+    // half-length lists to about those of one full-length list.  Stale reads are fine: the bound only grows.  A column
+    // EQUAL to the other list's k-th best is still admitted: it may be a global top-k member that wins the tie by its
+    // lower slot, and whether the other list has published that value yet depends on timing.
     thr_pub[list * BQ + row] = -CUDART_INF_F;
     named_bar_sync(3, GROUPS * 128);
   }
@@ -267,9 +279,10 @@ simtopk_kernel(const __grid_constant__ CUtensorMap map_qh, const __grid_constant
       // pending candidates in lock-step (1st of every lane, 2nd of every lane, ...): the warp pays for
       // max-per-lane insertions per tile, not for every distinct column position.
       uint32_t pending = 0;
-      const float gate = fmaxf(fmaxf(tk.thr, floor_thr), *thr_other);
+      const float gate = fmaxf(tk.thr, floor_thr);
+      const float gate_other = *thr_other;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) pending |= (v[j] > gate) ? (1u << j) : 0u;
+      for (int j = 0; j < 32; ++j) pending |= (v[j] > gate && v[j] >= gate_other) ? (1u << j) : 0u;
       while (__any_sync(0xffffffffu, pending != 0)) {
         if (pending) {
           const int j = __ffs(pending) - 1;
@@ -406,7 +419,8 @@ namespace simtopk {
 // CURRENT query, minus a margin.  The k-th best of the whole window is >= the k-th best of any k of its slots, so this is
 // a valid lower bound; consecutive frames share most of their top-k, so it is tight.  One warp per query, one lane per
 // slot; operands are the hi parts of the packed rows the GEMM uses, evaluated in fp32 with a rigorous allowance for the
-// dropped low-order parts.  Any invalid slot -> -inf (no bound).
+// dropped low-order parts.  Any invalid slot -> -inf (no bound); so is a repeated slot, since the minimum over fewer
+// than k distinct slots does not bound the k-th best.
 __global__ void __launch_bounds__(256)
 thr_floor_kernel(const int* __restrict__ prev_idx, int top_k, int q, int n_lead, int n_window, int kdim,
                  const __half* __restrict__ k_hi, const float* __restrict__ neg_s, const __half* __restrict__ q_hi,
@@ -421,8 +435,11 @@ thr_floor_kernel(const int* __restrict__ prev_idx, int top_k, int q, int n_lead,
   __syncwarp();
   float sim = CUDART_INF_F;
   bool bad = false;
+  const int n = (lane < top_k) ? prev_idx[(long long)qi * kListCap + lane] : -1;
+  const unsigned in_list = (top_k >= 32) ? 0xffffffffu : (1u << top_k) - 1u;
+  const unsigned same = __match_any_sync(0xffffffffu, n) & in_list;  // every lane takes part
+  if (lane < top_k && __popc(same) > 1) bad = true;
   if (lane < top_k) {
-    const int n = prev_idx[(long long)qi * kListCap + lane];
     if (n < n_lead || n >= n_window) {
       bad = true;
     } else {
