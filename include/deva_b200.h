@@ -27,7 +27,9 @@
 extern "C" {
 #endif
 
-/* v19: deva_b200_mask_stats(_workspace_bytes), deva_b200_mask_scored_argmax and deva_b200_mask_last_cover (detector
+/* v20: dropped deva_b200_up2_add and deva_b200_cbam (single-fp16 residual stream); deva_b200_up2_add_split requires skip_lo
+ * and raw / raw_lo.
+ * v19: deva_b200_mask_stats(_workspace_bytes), deva_b200_mask_scored_argmax and deva_b200_mask_last_cover (detector
  * masks -> detection id map).
  * v18: dropped conv split_mode 1, the split twins' relu_lo and hi-only pooling, gru, nhwc_to_nchw, enable_peer_access.
  * v16: deva_b200_label_areas and deva_b200_label_to_index (unsupervised DAVIS 2017 object limit).
@@ -37,7 +39,7 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 19
+#define DEVA_B200_ABI_VERSION 20
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -241,21 +243,15 @@ DEVA_B200_API int deva_b200_nchw_to_nhwc(const float* src, void* dst, int b, int
 /* 3x3 stride-2 max pool (resnet.py:123); x_lo / y_lo: optional low-order parts (pooling acts on x + x_lo) */
 DEVA_B200_API int deva_b200_maxpool(const void* x, const void* x_lo, void* y, void* y_lo, int b, int h, int w, int c,
                                     deva_stream_t stream);
-/* bilinear x2 (align_corners=False) + broadcast skip add -> raw and/or ReLU'd (modules.py:88-91) */
-DEVA_B200_API int deva_b200_up2_add(const void* g, const void* skip, void* raw, void* relu, int b, int h, int w, int c,
-                                    deva_stream_t stream);
 /* F.interpolate(mode='area') by an integer ratio r (group_modules.py:33-38), fp16 NHWC and fp32 planes */
 DEVA_B200_API int deva_b200_area_down(const void* x, void* y, int b, int h, int w, int c, int r, deva_stream_t stream);
 DEVA_B200_API int deva_b200_area_down_plane(const float* x, float* y, int b, int h, int w, int r, deva_stream_t stream);
-/* x + CBAM(x) (cbam.py:21-77 inside group_modules.py:146-150); scratch: fp32 [129*b*c + 2*b*h*w] (2 x 64 pooling slices + the gate, then the per-pixel statistics); c = 8 x a divisor of 256 */
-DEVA_B200_API int deva_b200_cbam(const void* x, const float* w1, const float* b1, const float* w2, const float* b2,
-                                 const float* ws, const float* bs, float* scratch, void* raw, void* relu, int b, int h,
-                                 int w, int c, int r, deva_stream_t stream);
-/* Split-precision twins for a residual stream carried as fp16 (hi, lo) pairs (the default "parity" precision plan): the
- * input is g + g_lo (x + x_lo) [+ skip_lo, optional], the raw result is written as (raw, raw_lo) (both NULL = not
- * wanted), the ReLU'd copy (an MMA operand) as hi.  relu_lo8 (optional): u8 NHWC, e4m3 of (relu - fp16(relu)) * 4096 -
- * the low-order operand of a conv with split_mode 3.  cbam_split takes the gate statistics (channel pooling, per-pixel
- * max / mean) over x + x_lo. */
+/* Bilinear x2 (align_corners=False) + broadcast skip add (modules.py:88-91) and x + CBAM(x) (cbam.py:21-77 inside
+ * group_modules.py:146-150) on a residual stream carried as fp16 (hi, lo) pairs (the "parity" precision plan): the input
+ * is g + g_lo + skip + skip_lo (x + x_lo), the raw result is written as (raw, raw_lo), the ReLU'd copy (an MMA operand) as
+ * hi.  relu_lo8 (optional): u8 NHWC, e4m3 of (relu - fp16(relu)) * 4096 - the low-order operand of a conv with
+ * split_mode 3.  cbam_split takes the gate statistics (channel pooling, per-pixel max / mean) over x + x_lo; scratch: fp32
+ * [129*b*c + 2*b*h*w] (2 x 64 pooling slices + the gate, then the per-pixel statistics); c = 8 x a divisor of 256. */
 DEVA_B200_API int deva_b200_up2_add_split(const void* g, const void* g_lo, const void* skip, const void* skip_lo,
                                           void* raw, void* raw_lo, void* relu, void* relu_lo8, int b, int h, int w, int c,
                                           deva_stream_t stream);

@@ -232,11 +232,6 @@ def test_helpers_match_torch():
     xh = _nhwc(x)
     xf = xh.float().permute(0, 3, 1, 2)
     torch.testing.assert_close(_nchw(ops.maxpool(xh)), F.max_pool2d(xf, 3, 2, 1))
-    skip = torch.randn(1, 64, 36, 52, device='cuda', generator=g)
-    raw, relu = ops.up2_add(xh, _nhwc(skip))
-    want = F.interpolate(xf, scale_factor=2, mode='bilinear', align_corners=False) + _nhwc(skip).float().permute(0, 3, 1, 2)
-    assert float((_nchw(raw) - want).abs().max()) < 4e-3
-    assert float((_nchw(relu) - want.clamp_min(0)).abs().max()) < 4e-3
     y = torch.randn(2, 64, 16, 24, device='cuda', generator=g)
     yh = _nhwc(y)
     for r in (2, 4):
@@ -244,25 +239,6 @@ def test_helpers_match_torch():
         assert float((_nchw(ops.area_down(yh, r)) - want).abs().max()) < 2e-3
     plane = torch.rand(3, 32, 48, device='cuda', generator=g)
     torch.testing.assert_close(ops.area_down_plane(plane, 16), F.interpolate(plane.unsqueeze(0), size=(2, 3), mode='area')[0])
-    # CBAM residual
-    c = 512
-    x = torch.randn(2, c, 6, 9, device='cuda', generator=g)
-    xh = _nhwc(x)
-    xf = xh.float().permute(0, 3, 1, 2)
-    p = dict(w1=torch.randn(32, c, device='cuda', generator=g) / c**0.5, b1=torch.randn(32, device='cuda', generator=g) * 0.1,
-             w2=torch.randn(c, 32, device='cuda', generator=g) / 32**0.5, b2=torch.randn(c, device='cuda', generator=g) * 0.1,
-             ws=torch.randn(98, device='cuda', generator=g) * 0.1, bs=torch.randn(1, device='cuda', generator=g) * 0.1)
-
-    def mlp(v):
-        return F.linear(F.relu(F.linear(v, p['w1'], p['b1'])), p['w2'], p['b2'])
-
-    gate = torch.sigmoid(mlp(xf.mean((2, 3))) + mlp(xf.amax((2, 3))))
-    xg = xf * gate[:, :, None, None]
-    pooled = torch.cat([xg.amax(1, keepdim=True), xg.mean(1, keepdim=True)], 1)
-    want = xf + xg * torch.sigmoid(F.conv2d(pooled, p['ws'].view(1, 2, 7, 7), p['bs'], padding=3))
-    raw, relu = ops.cbam_residual(xh, p)
-    assert float((_nchw(raw) - want).abs().max()) < 1e-2
-    assert float((_nchw(relu) - want.clamp_min(0)).abs().max()) < 1e-2
     # output tail
     k, hq, wq = 3, 6, 10
     logits = torch.randn(k, hq, wq, device='cuda', generator=g) * 3

@@ -330,27 +330,6 @@ def test_cbam_split(c, b, h, w):
     _check_relu_hi(raw, raw_lo, relu)
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize('c,b,h,w', CBAM_CASES)
-def test_cbam_fast(c, b, h, w):
-    """x + CBAM(x) on fp16 x (the fast plan): fp16 outputs within one fp16 ulp of fp64, plus fp32 epsilon."""
-    nat = _nat()
-    x, p = _cbam_inputs(c, b, h, w, 200 + c + b)
-    xh = x.half()
-    outs = Outputs()
-    raw, relu = (outs.new((b, h, w, c), torch.float16) for _ in range(2))
-    nat.cbam(xh, p['w1'], p['b1'], p['w2'], p['b2'], p['ws'], p['bs'], _cbam_scratch(b, h, w, c), raw, relu, b, h, w, c,
-             CBAM_R)
-    torch.cuda.synchronize()
-    outs.check()
-    ref = _cbam_residual_ref(_cbam_sd(p), xh.double())
-    slack = 8 * EPS32 * float(ref.abs().max())
-    _report(f'cbam C={c} {b}x{h}x{w}: raw / (ulp16 + 8 eps32 max|ref|)', _ulp_ratio(raw, ref, slack), 1.0)
-    _report(f'cbam C={c} {b}x{h}x{w}: relu / (ulp16 + 8 eps32 max|ref|)', _ulp_ratio(relu, ref.clamp_min(0), slack), 1.0)
-    pos = raw > 0
-    assert torch.equal(relu[pos], raw[pos]) and not bool(relu[~pos].any())
-
-
 # ------------------------------------------------------------------------------------------------- split-K finish
 SUM_OUTPUTS = ['raw', 'raw+lo', 'relu', 'relu+lo', 'all']
 SUM_SHAPE = (2, 30, 54, 64)
@@ -521,25 +500,6 @@ def test_up2_add_split_outputs(b, h, w, c, variant):
         got = relu_lo8.view(torch.float8_e4m3fn).double()
         bound = 0.07 * float(rem.abs().max()) + 2 ** -9 + 0.1
         _report(f'up2_add_split {shape}: e4m3 remainder abs', float((got - rem).abs().max()), bound)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('b,h,w,c', UP2_CASES)
-def test_up2_add(b, h, w, c):
-    """fp16 g bilinear x2 + fp16 skip -> fp16 raw / relu within one fp16 ulp of fp64, plus fp32 epsilon."""
-    nat = _nat()
-    x, skip = _up2_inputs(b, h, w, c, 700 + b + h + c)
-    xh, sh = x.half(), skip.half()
-    outs = Outputs()
-    shape = (b, 2 * h, 2 * w, c)
-    raw, relu = outs.new(shape, torch.float16), outs.new(shape, torch.float16)
-    nat.up2_add(xh, sh, raw, relu, b, h, w, c)
-    torch.cuda.synchronize()
-    outs.check()
-    ref = _up2_ref(xh.double(), sh.double())
-    slack = 8 * EPS32 * float(ref.abs().max())
-    _report(f'up2_add {shape}: raw / (ulp16 + 8 eps32 max|ref|)', _ulp_ratio(raw, ref, slack), 1.0)
-    _report(f'up2_add {shape}: relu / (ulp16 + 8 eps32 max|ref|)', _ulp_ratio(relu, ref.clamp_min(0), slack), 1.0)
 
 
 # ------------------------------------------------------------------------------------------------- max pool

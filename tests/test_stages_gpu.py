@@ -19,16 +19,13 @@ def _rel(a, b):
     return err, err / max(float(b.abs().max()), 1e-30)
 
 
-@pytest.mark.parametrize('precision', ['parity', 'fast'])
-def test_native_engine_stages_match_reference(golden_dir, synthetic_sd, precision, monkeypatch):
+def test_native_engine_stages_match_reference(golden_dir, synthetic_sd):
     from deva.model.native_engine import NativeEngine
-    monkeypatch.setenv('DEVA_B200_PRECISION', precision)
     g = {k: torch.from_numpy(v).cuda() for k, v in np.load(os.path.join(golden_dir, 'network_stages.npz')).items()}
     eng = NativeEngine({k: v.cuda() for k, v in synthetic_sd.items()})
-    assert eng.precision == precision
     report = {}
 
-    # ---- key encoder (split precision in both plans): a10, a11
+    # ---- key encoder (split precision): a10, a11
     ms, feat = eng.encode_image(g['image'])
     for name, got, want in (('f16', ms[0], g['f16']), ('f8', ms[1], g['f8']), ('f4', ms[2], g['f4']), ('feat', feat, g['feat'])):
         report[name] = _rel(got, want)
@@ -53,9 +50,9 @@ def test_native_engine_stages_match_reference(golden_dir, synthetic_sd, precisio
     report['logits'] = _rel(full, g['logits'])
     report['prob'] = _rel(prob, g['prob'])
     torch.cuda.synchronize()
-    print(f'[{precision}] stage errors (max abs, relative to max |ref|):')
+    print('stage errors (max abs, relative to max |ref|):')
     for k, (e, r) in report.items():
         print(f'    {k:10s} {e:.3e}  {r:.3e}')
     assert report['sensory2'][0] < 2e-2, report['sensory2']
-    assert report['logits'][0] < (8e-3 if precision == 'parity' else 1.6e-2), report['logits']
-    assert report['prob'][0] < (1e-3 if precision == 'parity' else 2.5e-3), report['prob']
+    assert report['logits'][0] < 8e-3, report['logits']
+    assert report['prob'][0] < 1e-3, report['prob']

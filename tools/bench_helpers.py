@@ -30,10 +30,16 @@ def main():
     def rec(name, ms, bytes_moved):
         res.append(dict(kernel=name, ms=round(ms, 4), GBps=round(bytes_moved / ms / 1e6, 1), MB=round(bytes_moved / 1e6, 1)))
 
-    p16 = torch.randn(K, h, w, 512, device=dev).half(); skip8 = torch.randn(1, 2 * h, 2 * w, 512, device=dev).half()
-    rec('up2_add 1/16->1/8 (512ch)', timeit(lambda: ops.up2_add(p16, skip8)), p16.numel() * 2 + skip8.numel() * 2 + 2 * K * 4 * h * w * 512 * 2)
-    p8 = torch.randn(K, 2 * h, 2 * w, 256, device=dev).half(); skip4 = torch.randn(1, 4 * h, 4 * w, 256, device=dev).half()
-    rec('up2_add 1/8->1/4 (256ch)', timeit(lambda: ops.up2_add(p8, skip4)), p8.numel() * 2 + skip4.numel() * 2 + 2 * K * 16 * h * w * 256 * 2)
+    # the decoder's residual stream is a fp16 (hi, lo) pair: 4 bytes per element read, raw + raw_lo + relu written
+    def pair(*shape):
+        return torch.randn(*shape, device=dev).half(), (torch.randn(*shape, device=dev) * 1e-3).half()
+    p16, p16_lo = pair(K, h, w, 512); skip8, skip8_lo = pair(1, 2 * h, 2 * w, 512)
+    rec('up2_add_split 1/16->1/8 (512ch)', timeit(lambda: ops.up2_add_split(p16, p16_lo, skip8, skip8_lo)),
+        p16.numel() * 4 + skip8.numel() * 4 + 3 * K * 4 * h * w * 512 * 2)
+    p8, p8_lo = pair(K, 2 * h, 2 * w, 256); skip4, skip4_lo = pair(1, 4 * h, 4 * w, 256)
+    rec('up2_add_split 1/8->1/4 (256ch, + e4m3 relu remainder)',
+        timeit(lambda: ops.up2_add_split(p8, p8_lo, skip4, skip4_lo, want_relu_lo8=True)),
+        p8.numel() * 4 + skip4.numel() * 4 + 7 * K * 16 * h * w * 256)
     p4 = torch.randn(K, 4 * h, 4 * w, 256, device=dev).half()
     rec('area_down x4 (256ch @1/4)', timeit(lambda: ops.area_down(p4, 4)), p4.numel() * 2 * (1 + 1 / 16))
     rec('area_down x2 (256ch @1/8)', timeit(lambda: ops.area_down(p8, 2)), p8.numel() * 2 * 1.25)
@@ -45,7 +51,8 @@ def main():
     rec('maxpool 3x3s2 (64ch @1/2)', timeit(lambda: ops.maxpool(x2)), x2.numel() * 2 * 1.25)
     cb = dict(w1=torch.randn(32, 512, device=dev), b1=torch.randn(32, device=dev), w2=torch.randn(512, 32, device=dev),
               b2=torch.randn(512, device=dev), ws=torch.randn(98, device=dev), bs=torch.randn(1, device=dev))
-    rec('cbam_residual (512ch @1/16)', timeit(lambda: ops.cbam_residual(p16, cb)), p16.numel() * 2 * 5)
+    # (hi, lo) read by the pooling, the statistics and the apply pass; raw + raw_lo + relu written
+    rec('cbam_residual_split (512ch @1/16)', timeit(lambda: ops.cbam_residual_split(p16, p16_lo, cb)), p16.numel() * 2 * 9)
     logits = torch.randn(K, 4 * h, 4 * w, device=dev); agg = torch.empty(K + 1, 4 * h, 4 * w, device=dev)
     prob = torch.empty(K + 1, H, W, device=dev)
     rec('aggregate + x4 + softmax', timeit(lambda: nat.output_tail(logits, agg, prob, None, K, 4 * h, 4 * w)), logits.numel() * 4 * 2 + agg.numel() * 4 + prob.numel() * 4)

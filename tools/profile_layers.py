@@ -42,8 +42,7 @@ def main():
             return orig_conv(x, pc, **kw)
         return timed('conv:' + names.get(id(pc), '?') + (f' [{passes} passes]' if passes > 1 else ''), fl, orig_conv, x, pc, **kw)
     ops.conv_ex = conv_ex
-    for fn in ('maxpool', 'up2_add', 'up2_add_split', 'area_down', 'area_down_plane', 'cbam_residual', 'cbam_residual_split',
-               'stem_columns'):
+    for fn in ('maxpool', 'up2_add_split', 'area_down', 'area_down_plane', 'cbam_residual_split', 'stem_columns'):
         o = getattr(ops, fn)
         setattr(ops, fn, (lambda o, fn: lambda *aa, **kw: timed('ew:' + fn, 0, o, *aa, **kw))(o, fn))
     for fn in ('pack_query', 'sim_topk', 'readout', 'output_tail', 'key_tail', 'pack_keys', 'transpose_append', 'nchw_to_nhwc', 'readout_sparse', 'head_gather3x3'):

@@ -205,46 +205,10 @@ __global__ void maxpool_kernel(const __half* __restrict__ x, const __half* __res
   }
 }
 
-// out = bilinear_x2(g) + skip (skip is one image broadcast over the batch); writes raw and/or relu
-// (MaskUpsampleBlock: upsample_groups + distributor 'add', modules.py:88-91)
-__global__ void __launch_bounds__(256)
-up2_add_kernel(const __half* __restrict__ g, const __half* __restrict__ skip, __half* __restrict__ raw,
-               __half* __restrict__ relu, int B, int h, int w, int C) {
-  // blockIdx.y = (image, output row): the two source rows and their weights are uniform per block
-  const int H = 2 * h, W = 2 * w, C8 = C / 8;
-  const int b = blockIdx.y / H, Y = blockIdx.y - b * H;
-  const float sy = fmaxf((Y + 0.5f) * 0.5f - 0.5f, 0.f);  // align_corners=False: src = (dst + 0.5)/2 - 0.5, clamped
-  const int y0 = (int)sy, y1 = min(y0 + 1, h - 1);
-  const float wy = sy - y0;
-  const __half* r0 = g + ((long long)b * h + y0) * w * C;
-  const __half* r1 = g + ((long long)b * h + y1) * w * C;
-  const __half* sk = skip + (long long)Y * W * C;
-  const long long obase = ((long long)b * H + Y) * W * C;
-  const int row_vecs = W * C8;
-  for (int i = blockIdx.x * 256 + threadIdx.x; i < row_vecs; i += gridDim.x * 256) {
-    const int X = i / C8, c = (i - X * C8) * 8;
-    const float sx = fmaxf((X + 0.5f) * 0.5f - 0.5f, 0.f);
-    const int x0 = (int)sx, x1 = min(x0 + 1, w - 1);
-    const float wx = sx - x0;
-    float a[8], bq[8], cq[8], d[8], o[8], s_[8];
-    ld8(r0 + x0 * C + c, a);
-    ld8(r0 + x1 * C + c, bq);
-    ld8(r1 + x0 * C + c, cq);
-    ld8(r1 + x1 * C + c, d);
-    ld8(sk + X * C + c, s_);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const float top = a[e] + (bq[e] - a[e]) * wx, bot = cq[e] + (d[e] - cq[e]) * wx;
-      o[e] = top + (bot - top) * wy + s_[e];
-    }
-    const long long off = obase + X * C + c;
-    if (raw) st8(raw + off, o, false);
-    if (relu) st8(relu + off, o, true);
-  }
-}
-
-// Split-precision twin (residual stream carried as fp16 hi/lo pairs, DESIGN section 4 "precision plan"): g = g + g_lo on
-// input; the raw sum is written as (hi, lo), the ReLU'd copy - an MMA operand only - as hi.
+// out = bilinear_x2(g) + skip (skip is one image broadcast over the batch; MaskUpsampleBlock: upsample_groups +
+// distributor 'add', modules.py:88-91) on the residual stream carried as fp16 hi/lo pairs (DESIGN section 4 "precision
+// plan"): g = g + g_lo and skip = skip + skip_lo on input; the raw sum is written as (hi, lo), the ReLU'd copy - an MMA
+// operand only - as hi.
 __device__ __forceinline__ void st8_split(__half* hi, __half* lo, const float (&f)[8]) {
   uint4 vh, vl;
   __half2* h2 = reinterpret_cast<__half2*>(&vh);
@@ -300,18 +264,16 @@ up2_add_split_kernel(const __half* __restrict__ g, const __half* __restrict__ g_
         const float wx = dx ? 0.75f : 0.25f;
         float o[8], s_[8];
         ld8(skip + ((long long)Y * W + X) * C + c, s_);
-        if (skip_lo) {
-          ld8(skip_lo + ((long long)Y * W + X) * C + c, l);
+        ld8(skip_lo + ((long long)Y * W + X) * C + c, l);
 #pragma unroll
-          for (int e = 0; e < 8; ++e) s_[e] += l[e];
-        }
+        for (int e = 0; e < 8; ++e) s_[e] += l[e];
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
           const float top = qa[e] + (qb[e] - qa[e]) * wx, bot = qc[e] + (qd[e] - qc[e]) * wx;
           o[e] = top + (bot - top) * wy + s_[e];
         }
         const long long off = (((long long)b * H + Y) * W + X) * C + c;
-        if (raw) st8_split(raw + off, raw_lo + off, o);
+        st8_split(raw + off, raw_lo + off, o);
         if (relu_lo8) {  // low-order part as e4m3 of (x - fp16(x)) * 4096: operand of an fp8 correction pass
           uint32_t w8[2];
 #pragma unroll
@@ -396,14 +358,11 @@ cbam_pool_kernel(const __half* __restrict__ x, const __half* __restrict__ x_lo, 
   for (int e = 0; e < 8; ++e) { s[e] = 0.f; m[e] = -CUDART_INF_F; }
   for (int i = i0 + pl; i < i1; i += lanes) {
     const long long o = ((long long)b * HW + i) * C + cv * 8;
-    float v[8];
+    float v[8], l[8];
     ld8(x + o, v);
-    if (x_lo) {
-      float l[8];
-      ld8(x_lo + o, l);
+    ld8(x_lo + o, l);
 #pragma unroll
-      for (int e = 0; e < 8; ++e) v[e] += l[e];
-    }
+    for (int e = 0; e < 8; ++e) v[e] += l[e];
 #pragma unroll
     for (int e = 0; e < 8; ++e) { s[e] += v[e]; m[e] = fmaxf(m[e], v[e]); }
   }
@@ -466,18 +425,15 @@ __global__ void cbam_stats_kernel(const __half* __restrict__ x, const __half* __
   if (pix >= (long long)B * HW) return;
   const int b = (int)(pix / HW);
   const __half* p = x + pix * C;
-  const __half* pl = x_lo ? x_lo + pix * C : nullptr;
+  const __half* pl = x_lo + pix * C;
   const float* g = gate + b * C;
   float s = 0.f, m = -CUDART_INF_F;
   for (int c = lane * 8; c < C; c += 256) {
-    float v[8];
+    float v[8], l[8];
     ld8(p + c, v);
-    if (pl) {
-      float l[8];
-      ld8(pl + c, l);
+    ld8(pl + c, l);
 #pragma unroll
-      for (int e = 0; e < 8; ++e) v[e] += l[e];
-    }
+    for (int e = 0; e < 8; ++e) v[e] += l[e];
     const float4 g0 = *reinterpret_cast<const float4*>(g + c), g1 = *reinterpret_cast<const float4*>(g + c + 4);
     const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
 #pragma unroll
@@ -493,36 +449,8 @@ __global__ void cbam_stats_kernel(const __half* __restrict__ x, const __half* __
   }
   if (lane == 0) { stats[pix * 2] = m; stats[pix * 2 + 1] = s / C; }
 }
-// out = x + x * gate * sigmoid(conv7x7(stats))   (FeatureFusion: g + attention(g)); one warp per pixel
-__global__ void cbam_apply_kernel(const __half* __restrict__ x, const float* __restrict__ gate, const float* __restrict__ stats,
-                                  const float* __restrict__ ws, const float* __restrict__ bs, __half* __restrict__ raw,
-                                  __half* __restrict__ relu, int B, int H, int W, int C) {
-  const long long pix = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (pix >= (long long)B * H * W) return;
-  const int b = (int)(pix / ((long long)H * W));
-  const int rem = (int)(pix - (long long)b * H * W);
-  const int y = rem / W, xq = rem - y * W;
-  float a = 0.f;
-  for (int t = lane; t < 98; t += 32) {
-    const int ch = t / 49, k = t % 49, dy = k / 7 - 3, dx = k % 7 - 3;
-    const int yy = y + dy, xx = xq + dx;
-    if (yy >= 0 && yy < H && xx >= 0 && xx < W) a += ws[t] * stats[(((long long)b * H + yy) * W + xx) * 2 + ch];
-  }
-  for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-  const float sg = sigmoidf_(a + bs[0]);
-  const float* g = gate + b * C;
-  for (int c = lane * 8; c < C; c += 256) {
-    float v[8], o[8];
-    ld8(x + pix * C + c, v);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) o[e] = v[e] + v[e] * g[c + e] * sg;
-    if (raw) st8(raw + pix * C + c, o, false);
-    if (relu) st8(relu + pix * C + c, o, true);
-  }
-}
-
-// split-precision twin of cbam_apply_kernel: x = x + x_lo on input, raw written as (hi, lo), relu as hi
+// out = x + x * gate * sigmoid(conv7x7(stats))   (FeatureFusion: g + attention(g)); one warp per pixel.  x = x + x_lo on
+// input, raw written as (hi, lo), relu as hi
 __global__ void cbam_apply_split_kernel(const __half* __restrict__ x, const __half* __restrict__ x_lo,
                                         const float* __restrict__ gate, const float* __restrict__ stats,
                                         const float* __restrict__ ws, const float* __restrict__ bs,
@@ -782,19 +710,11 @@ DEVA_B200_API int deva_b200_maxpool(const void* x, const void* x_lo, void* y, vo
   B200_LAUNCH_CHECK();
   return 0;
 }
-DEVA_B200_API int deva_b200_up2_add(const void* g, const void* skip, void* raw, void* relu, int b, int h, int w, int c,
-                                    deva_stream_t stream) {
-  B200_REQUIRE(c % 8 == 0, "up2_add: C %% 8");
-  ew::up2_add_kernel<<<dim3(ceil_div(2 * w * (c / 8), 256 * 2), b * 2 * h), 256, 0, S(stream)>>>(H(g), H(skip), H(raw),
-                                                                                                H(relu), b, h, w, c);
-  B200_LAUNCH_CHECK();
-  return 0;
-}
 DEVA_B200_API int deva_b200_up2_add_split(const void* g, const void* g_lo, const void* skip, const void* skip_lo,
                                           void* raw, void* raw_lo, void* relu, void* relu_lo8, int b, int h, int w, int c,
                                           deva_stream_t stream) {
-  B200_REQUIRE(c % 8 == 0 && g_lo && (raw != nullptr) == (raw_lo != nullptr) && (raw || relu) && (!relu_lo8 || relu),
-               "up2_add_split: C %% 8, g_lo, and raw/raw_lo (both or neither) with at least one output are required");
+  B200_REQUIRE(c % 8 == 0 && g_lo && skip_lo && raw && raw_lo && (!relu_lo8 || relu),
+               "up2_add_split: C %% 8, g_lo, skip_lo, raw and raw_lo are required, and relu with relu_lo8");
   ew::up2_add_split_kernel<<<dim3(ceil_div((w + 1) * (c / 8), 256), b * (h + 1)), 256, 0, S(stream)>>>(
       H(g), H(g_lo), H(skip), H(skip_lo), H(raw), H(raw_lo), H(relu), reinterpret_cast<unsigned char*>(relu_lo8), b, h, w,
       c);
@@ -814,29 +734,6 @@ DEVA_B200_API int deva_b200_area_down_plane(const float* x, float* y, int b, int
   B200_LAUNCH_CHECK();
   return 0;
 }
-DEVA_B200_API int deva_b200_cbam(const void* x, const float* w1, const float* b1, const float* w2, const float* b2,
-                                 const float* ws, const float* bs, float* scratch, void* raw, void* relu, int b, int h,
-                                 int w, int c, int r, deva_stream_t stream) {
-  const __half* xh = H(x);
-  const cudaStream_t s = S(stream);
-  // scratch: psum[B*16*C] | pmax[B*16*C] | gate[B*C] | stats[B*H*W*2]
-  float* psum = scratch;
-  float* pmax = psum + (long long)b * ew::kPoolSplit * c;
-  float* gate = pmax + (long long)b * ew::kPoolSplit * c;
-  float* stats = gate + (long long)b * c;
-  const int HW = h * w;
-  B200_REQUIRE(c % 8 == 0 && c / 8 <= 256 && 256 % (c / 8) == 0, "cbam: C = %d must be 8 x a divisor of 256", c);
-  ew::cbam_pool_kernel<<<dim3(b, ew::kPoolSplit), 256, 0, s>>>(xh, nullptr, psum, pmax, HW, c);
-  B200_LAUNCH_CHECK();
-  ew::cbam_mlp_kernel<<<b, 256, (2 * c + 2 * r) * sizeof(float), s>>>(psum, pmax, HW, w1, b1, w2, b2, gate, c, r);
-  B200_LAUNCH_CHECK();
-  const long long warps = (long long)b * HW;
-  ew::cbam_stats_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(xh, nullptr, gate, stats, b, HW, c);
-  B200_LAUNCH_CHECK();
-  ew::cbam_apply_kernel<<<ceil_div(warps * 32, 256), 256, 0, s>>>(xh, gate, stats, ws, bs, H(raw), H(relu), b, h, w, c);
-  B200_LAUNCH_CHECK();
-  return 0;
-}
 DEVA_B200_API int deva_b200_cbam_split(const void* x, const void* x_lo, const float* w1, const float* b1, const float* w2,
                                        const float* b2, const float* ws, const float* bs, float* scratch, void* raw,
                                        void* raw_lo, void* relu, int b, int h, int w, int c, int r, deva_stream_t stream) {
@@ -846,6 +743,7 @@ DEVA_B200_API int deva_b200_cbam_split(const void* x, const void* x_lo, const fl
   const __half* xh = H(x);
   const __half* xl = H(x_lo);
   const cudaStream_t s = S(stream);
+  // scratch: psum[B*kPoolSplit*C] | pmax[B*kPoolSplit*C] | gate[B*C] | stats[B*H*W*2]
   float* psum = scratch;
   float* pmax = psum + (long long)b * ew::kPoolSplit * c;
   float* gate = pmax + (long long)b * ew::kPoolSplit * c;

@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 19
+ABI_VERSION = 20
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -75,11 +75,8 @@ _SIGNATURES = {
     'deva_b200_stem_im2col': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_nchw_to_nhwc': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_maxpool': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    'deva_b200_up2_add': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_area_down': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_area_down_plane': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    'deva_b200_cbam': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                               c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_up2_add_split': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                         c_int, c_int, c_int, c_int, c_void_p]),
     'deva_b200_cbam_split': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -318,10 +315,6 @@ def maxpool(x, y, b, h, w, c, x_lo=None, y_lo=None):
     _check(lib().deva_b200_maxpool(_ptr(x), _ptr(x_lo), _ptr(y), _ptr(y_lo), b, h, w, c, _stream()), 'maxpool')
 
 
-def up2_add(g, skip, raw, relu, b, h, w, c):
-    _check(lib().deva_b200_up2_add(_ptr(g), _ptr(skip), _ptr(raw), _ptr(relu), b, h, w, c, _stream()), 'up2_add')
-
-
 def area_down(x, y, b, h, w, c, r):
     _check(lib().deva_b200_area_down(_ptr(x), _ptr(y), b, h, w, c, r, _stream()), 'area_down')
 
@@ -330,12 +323,7 @@ def area_down_plane(x, y, b, h, w, r):
     _check(lib().deva_b200_area_down_plane(_ptr(x), _ptr(y), b, h, w, r, _stream()), 'area_down_plane')
 
 
-def cbam(x, w1, b1, w2, b2, ws, bs, scratch, raw, relu, b, h, w, c, r):
-    _check(lib().deva_b200_cbam(_ptr(x), _ptr(w1), _ptr(b1), _ptr(w2), _ptr(b2), _ptr(ws), _ptr(bs), _ptr(scratch),
-                                _ptr(raw), _ptr(relu), b, h, w, c, r, _stream()), 'cbam')
-
-
-def up2_add_split(g, g_lo, skip, raw, raw_lo, relu, b, h, w, c, skip_lo=None, relu_lo8=None):
+def up2_add_split(g, g_lo, skip, raw, raw_lo, relu, b, h, w, c, *, skip_lo, relu_lo8=None):
     _check(lib().deva_b200_up2_add_split(_ptr(g), _ptr(g_lo), _ptr(skip), _ptr(skip_lo), _ptr(raw), _ptr(raw_lo),
                                          _ptr(relu), _ptr(relu_lo8), b, h, w, c, _stream()), 'up2_add_split')
 

@@ -9,10 +9,10 @@ csrc/elementwise.cu.  No cuDNN / cuBLAS on this path.
 
 Tensors crossing the public API keep the reference's [B, C, H, W] / [1, K, C, h, w] *shapes* but are
 permuted views of NHWC fp16 storage, so they flow through ``DEVAInferenceCore`` / ``MemoryManager``
-without conversion.
+without conversion.  The key path, the decoder's residual stream and the layers next to the logits run at more than
+fp16 precision (the precision plan in ``NativeEngine.__init__``), which keeps the probabilities within 1e-3 of fp32.
 """
-import os
-from typing import Dict, Tuple
+from typing import Dict
 
 import torch
 
@@ -42,19 +42,14 @@ def _api(t_nhwc: torch.Tensor) -> torch.Tensor:
 
 class NativeEngine:
     prefers_nhwc = True
+    precision = 'parity'  # the name of the precision plan below, reported in bench.py's result line
 
     def __init__(self, sd: Dict[str, torch.Tensor]):
         # Precision plan (DESIGN "precision plan"; tools/precision_layers.py / precision_plan.py rank the rounding sources):
-        #   'parity' (default): the decoder's residual / skip stream travels as fp16 (hi, lo) pairs, the 1x1 shortcut /
-        #       skip convolutions that consume the raw stream run in split precision (three MMA passes, they are cheap),
-        #       sensory_compress takes (hi, lo) weights, and the two 3x3 convs of the last decoder block (up_8_4, next to
-        #       the logits) add an fp8 correction pass over their activations' low-order part (half a pass).
-        #       max |prob - fp32 reference| < 1e-3.
-        #   'fast': every operand and every stored activation is a single fp16 (1.7e-3 on the golden clip).
-        self.precision = os.environ.get('DEVA_B200_PRECISION', 'parity')
-        if self.precision not in ('parity', 'fast'):
-            raise RuntimeError(f"deva_b200: DEVA_B200_PRECISION must be 'parity' or 'fast', got {self.precision!r}")
-        self.parity = self.precision == 'parity'
+        # the decoder's residual / skip stream travels as fp16 (hi, lo) pairs, the 1x1 shortcut / skip convolutions that
+        # consume the raw stream run in split precision (three MMA passes, they are cheap), sensory_compress takes (hi, lo)
+        # weights, and the two 3x3 convs of the last decoder block (up_8_4, next to the logits) add an fp8 correction pass
+        # over their activations' low-order part (half a pass).  max |prob - fp32 reference| < 1e-3.
         self.device = next(iter(sd.values())).device
         # fold BatchNorm and pack the operands on the host (a few hundred tiny device launches otherwise), upload once
         t = LayerTable({k: v.detach().to('cpu', torch.float32) if v.is_floating_point() else v.cpu() for k, v in sd.items()})
@@ -66,11 +61,10 @@ class NativeEngine:
             # accuracy): the top-k read is discontinuous in the keys, and the path is < 3 % of the frame's FLOPs.
             precise = name.startswith('pixel_encoder') or name.startswith('key_proj')
             tail = name.rsplit('.', 1)[-1]
-            if self.parity:
-                if tail in ('skip8', 'skip4', 'ds_x', 'ds_g') or name.endswith('up_16_8.out_conv.ds'):
-                    precise = True
-            act_lo8 = self.parity and 'up_8_4.out_conv' in name  # the low-order activation pass on the fp8 path
-            w_lo = self.parity and name.endswith('.sensory_compress')
+            if tail in ('skip8', 'skip4', 'ds_x', 'ds_g') or name.endswith('up_16_8.out_conv.ds'):
+                precise = True
+            act_lo8 = 'up_8_4.out_conv' in name  # the low-order activation pass on the fp8 path
+            w_lo = name.endswith('.sensory_compress')
             if name.endswith('.pred'):  # folded into up_8_4.c2's epilogue as a fp32 9-tap head (see decode)
                 self.pred_w = spec.weight[0].permute(1, 2, 0).reshape(9, -1).float().contiguous().to(self.device)  # [tap, cin]
                 self.pred_b = float(spec.bias[0])
@@ -119,7 +113,7 @@ class NativeEngine:
                 x = self._bottleneck(x, f'{p}.{stage}.{i}')
             feats.append(x)
         f4, f8, f16 = feats
-        o1 = ops.conv_ex(f16[0], P[p + '.proj1'], x_lo=f16[1], want_raw=True, want_relu=True, want_lo=self.parity)
+        o1 = ops.conv_ex(f16[0], P[p + '.proj1'], x_lo=f16[1], want_raw=True, want_relu=True, want_lo=True)
         o2 = ops.conv_ex(f16[0], P[p + '.proj2'], x_lo=f16[1], want_raw=True, want_lo=True)
         f16_api = _api(o1.raw)
         f16_api._b200_relu = o1.relu  # ReLU twin for the fusers' shared half (kept alive with the view)
@@ -151,13 +145,6 @@ class NativeEngine:
                 sel.view(1, h, w, ck).permute(0, 3, 1, 2) if need_ek else None)
 
     # ------------------------------------------------------------------ shared blocks
-    def _shared_pair(self, x_api: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-        raw = _to_nhwc(x_api)
-        relu = getattr(x_api, '_b200_relu', None)
-        if relu is None:
-            relu = torch.relu(raw)
-        return raw, relu
-
     @staticmethod
     def _lo_of(x_api: torch.Tensor, like: torch.Tensor) -> torch.Tensor:
         """Low-order part riding on an API view (zeros when the tensor came from elsewhere, e.g. a user's own features)."""
@@ -165,18 +152,6 @@ class NativeEngine:
         if lo is None or lo.shape != like.shape:
             lo = torch.zeros_like(like)
         return lo
-
-    def _fuse(self, p, x_raw, x_relu, g_raw, g_relu):
-        """GroupFeatureFusionBlock (group_modules.py:133-152): returns the raw block output [K,h,w,C]."""
-        P = self.P
-        sx = ops.conv(x_relu, P[p + '.b1.c1_x'], want_raw=True)           # shared half of conv1 (+bias)
-        dx = ops.conv(x_raw, P[p + '.b1.ds_x'], want_raw=True)            # shared half of the 1x1 shortcut (+bias)
-        y = ops.conv(g_relu, P[p + '.b1.c1_g'], res=sx, want_relu=True)
-        short = ops.conv(g_raw, P[p + '.b1.ds_g'], res=dx, want_raw=True)
-        g = ops.conv(y, P[p + '.b1.c2'], res=short, want_raw=True)
-        gr_raw, gr_relu = ops.cbam_residual(g, self.cbam[p])              # g + CBAM(g)
-        y = ops.conv(gr_relu, P[p + '.b2.c1'], want_relu=True)
-        return ops.conv(y, P[p + '.b2.c2'], res=gr_raw, want_raw=True)
 
     def _C(self, name, x, lo=None, **kw) -> ops.ConvOut:
         """Conv `name` on (x, lo): the low-order part is consumed only when the layer's precision mode takes it."""
@@ -190,11 +165,11 @@ class NativeEngine:
     def _tl(self, name) -> bool:
         return self.P[name].takes_lo
 
-    def _fuse_split(self, p, X, g_raw, g_lo, g_relu, g_relu_lo=None):
-        """_fuse of the parity plan: the block's residual stream (shortcut, block outputs, CBAM residual) is carried as
-        (hi, lo) pairs and the two 1x1 shortcut convs - they map the raw stream straight onto the output - run in split
-        precision; every MMA operand gets its low-order part when its layer's mode takes one.  X = the shared feature
-        (raw, raw_lo, relu, relu_lo).  Returns (raw, raw_lo)."""
+    def _fuse(self, p, X, g_raw, g_lo, g_relu, g_relu_lo=None):
+        """GroupFeatureFusionBlock (group_modules.py:133-152): the block's residual stream (shortcut, block outputs, CBAM
+        residual) is carried as (hi, lo) pairs and the two 1x1 shortcut convs - they map the raw stream straight onto the
+        output - run in split precision; every MMA operand gets its low-order part when its layer's mode takes one.
+        X = the shared feature (raw, raw_lo, relu, relu_lo).  Returns the block output [K,h,w,C] as (raw, raw_lo)."""
         x_raw, x_lo, x_relu, x_relu_lo = X
         q = p + '.b1'
         sx = self._C(q + '.c1_x', x_relu, x_relu_lo, want_raw=True, want_lo=True)
@@ -208,7 +183,10 @@ class NativeEngine:
         return out.raw, out.raw_lo
 
     def _shared_quad(self, x_api: torch.Tensor):
-        raw, relu = self._shared_pair(x_api)
+        raw = _to_nhwc(x_api)
+        relu = getattr(x_api, '_b200_relu', None)
+        if relu is None:
+            relu = torch.relu(raw)
         relu_lo = getattr(x_api, '_b200_relu_lo', None)
         return raw, self._lo_of(x_api, raw), relu, relu_lo
 
@@ -225,7 +203,7 @@ class NativeEngine:
         return ops.conv(y, P[q + '.c2'], res=short, want_relu=True)
 
     def _basic_pair(self, x, lo, q):
-        """BasicBlock on a post-ReLU (hi, lo) pair (parity plan): returns the output pair."""
+        """BasicBlock on a post-ReLU (hi, lo) pair: returns the output pair."""
         y = self._C(q + '.c1', x, lo, want_relu=True, want_lo=self._tl(q + '.c2'))
         if (q + '.ds') in self.P:
             s_ = self._C(q + '.ds', x, lo, want_raw=True, want_lo=True)
@@ -242,32 +220,22 @@ class NativeEngine:
         step = k if chunk_size < 1 or chunk_size >= k else chunk_size
         img_pc, msk_pc = P[p + '.stem_img'], P[p + '.stem_mask']
         shared = ops.conv(ops.stem_columns(image.float(), img_pc.cin_pad), img_pc, want_raw=True)
-        if self.parity:
-            X = self._shared_quad(ms_features[0])
-        else:
-            x_raw, x_relu = self._shared_pair(ms_features[0])
+        X = self._shared_quad(ms_features[0])
         h_all = _to_nhwc(sensory[0])
         planes = masks[0].float().contiguous().unsqueeze(1)  # [K,1,H,W]
         values, hiddens = [], []
         for i in range(0, k, step):
             cols = ops.stem_columns(planes[i:i + step], msk_pc.cin_pad)
-            if self.parity:  # single-fp16 trunk; its last block hands the fuser a (hi, lo) pair
-                x = ops.conv(cols, msk_pc, res=shared, want_relu=True)
-                x = ops.maxpool(x)
-                for stage in ('layer1', 'layer2', 'layer3'):
-                    for b in range(2):
-                        if stage == 'layer3' and b == 1:
-                            x, lo = self._basic_pair(x, None, f'{p}.{stage}.{b}')
-                        else:
-                            x = self._basic(x, f'{p}.{stage}.{b}')
-                g16, _ = self._fuse_split(p + '.fuser', X, x, lo, x, lo)
-            else:
-                x = ops.conv(cols, msk_pc, res=shared, want_relu=True)
-                x = ops.maxpool(x)  # ReLU and max-pool commute (quirk Q6)
-                for stage in ('layer1', 'layer2', 'layer3'):
-                    for b in range(2):
+            # single-fp16 trunk; its last block hands the fuser a (hi, lo) pair
+            x = ops.conv(cols, msk_pc, res=shared, want_relu=True)
+            x = ops.maxpool(x)  # ReLU and max-pool commute (quirk Q6)
+            for stage in ('layer1', 'layer2', 'layer3'):
+                for b in range(2):
+                    if stage == 'layer3' and b == 1:
+                        x, lo = self._basic_pair(x, None, f'{p}.{stage}.{b}')
+                    else:
                         x = self._basic(x, f'{p}.{stage}.{b}')
-                g16 = self._fuse(p + '.fuser', x_raw, x_relu, x, x)
+            g16, _ = self._fuse(p + '.fuser', X, x, lo, x, lo)
             values.append(g16)
             if deep_update:
                 hiddens.append(self._gru(p + '.gru', g16, h_all[i:i + step].contiguous()))
@@ -287,15 +255,10 @@ class NativeEngine:
         k = readout.shape[1]
         step = k if chunk_size < 1 or chunk_size >= k else chunk_size
         f8n, f4n = _to_nhwc(f8), _to_nhwc(f4)
-        if self.parity:
-            X = self._shared_quad(f16)
-            s8 = self._C(p + '.skip8', f8n, self._lo_of(f8, f8n), want_raw=True, want_lo=True)
-            s4 = self._C(p + '.skip4', f4n, self._lo_of(f4, f4n), want_raw=True, want_lo=True)
-            skip8, skip8_lo, skip4, skip4_lo = s8.raw, s8.raw_lo, s4.raw, s4.raw_lo
-        else:
-            x_raw, x_relu = self._shared_pair(f16)
-            skip8 = ops.conv(f8n, P[p + '.skip8'], want_raw=True)
-            skip4 = ops.conv(f4n, P[p + '.skip4'], want_raw=True)
+        X = self._shared_quad(f16)
+        s8 = self._C(p + '.skip8', f8n, self._lo_of(f8, f8n), want_raw=True, want_lo=True)
+        s4 = self._C(p + '.skip4', f4n, self._lo_of(f4, f4n), want_raw=True, want_lo=True)
+        skip8, skip8_lo, skip4, skip4_lo = s8.raw, s8.raw_lo, s4.raw, s4.raw_lo
         ro_all = _to_nhwc(readout[0])
         h_all = _to_nhwc(sensory[0])
         hh, ww = ro_all.shape[1:3]
@@ -305,40 +268,23 @@ class NativeEngine:
         logits_all, hiddens = [], []
         for i in range(0, k, step):
             h = h_all[i:i + step].contiguous()
-            if self.parity:
-                tl = self._tl
-                c16 = self._C(p + '.sensory_compress', h, rank1_x=last[i:i + step].contiguous(),
-                              res=ro_all[i:i + step].contiguous(), want_raw=True, want_relu=True, want_lo=True)
-                p16, p16_lo = self._fuse_split(p + '.fuser', X, c16.raw, c16.raw_lo, c16.relu, c16.relu_lo)
-                q = p + '.up_16_8.out_conv'
-                g8_raw, g8_lo, g8_relu, _ = ops.up2_add_split(p16, p16_lo, skip8, skip8_lo)
-                y = self._C(q + '.c1', g8_relu, want_relu=True, want_lo=tl(q + '.c2'))
-                short = self._C(q + '.ds', g8_raw, g8_lo, want_raw=True, want_lo=True)
-                o8 = self._C(q + '.c2', y.relu, y.relu_lo, res=short.raw, res_lo=short.raw_lo, want_raw=True, want_lo=True)
-                p8 = o8.raw
-                q = p + '.up_8_4.out_conv'
-                g4_raw, g4_lo, g4_relu, g4_relu_lo8 = ops.up2_add_split(p8, o8.raw_lo, skip4, skip4_lo, want_relu_lo8=True)
-                y4 = self._C(q + '.c1', g4_relu, g4_relu_lo8, want_relu=True, want_relu_lo8=True)
-                # p4 = c2(...) + g4; the logit conv pred(relu(p4)) (big_modules.py:189-190) is folded in: the epilogue
-                # emits the 9 per-tap dot products in fp32, a 3x3 gather finishes the convolution.  p4 itself is only
-                # read 4x4-pooled by su.g4_conv, so the epilogue writes that pool instead of p4.
-                o4 = self._C(q + '.c2', y4.relu, y4.relu_lo8, res=g4_raw, res_lo=g4_lo, want_pool4=update_sensory,
-                             head_w=self.pred_w)
-            else:
-                p16_raw, p16_relu = ops.conv(h, P[p + '.sensory_compress'], rank1_x=last[i:i + step].contiguous(),
-                                             res=ro_all[i:i + step].contiguous(), want_raw=True, want_relu=True)
-                p16 = self._fuse(p + '.fuser', x_raw, x_relu, p16_raw, p16_relu)
-                g8_raw, g8_relu = ops.up2_add(p16, skip8)
-                q = p + '.up_16_8.out_conv'
-                y = ops.conv(g8_relu, P[q + '.c1'], want_relu=True)
-                short = ops.conv(g8_raw, P[q + '.ds'], want_raw=True)
-                p8 = ops.conv(y, P[q + '.c2'], res=short, want_raw=True)
-                g4_raw, g4_relu = ops.up2_add(p8, skip4)
-                q = p + '.up_8_4.out_conv'
-                y = ops.conv(g4_relu, P[q + '.c1'], want_relu=True)
-                # p4 = c2(...) + g4; the logit conv pred(relu(p4)) (big_modules.py:189-190) is folded in: the epilogue
-                # emits the 9 per-tap dot products in fp32, a 3x3 gather finishes the convolution.
-                o4 = ops.conv_ex(y, P[q + '.c2'], res=g4_raw, want_pool4=update_sensory, head_w=self.pred_w)
+            c16 = self._C(p + '.sensory_compress', h, rank1_x=last[i:i + step].contiguous(),
+                          res=ro_all[i:i + step].contiguous(), want_raw=True, want_relu=True, want_lo=True)
+            p16, p16_lo = self._fuse(p + '.fuser', X, c16.raw, c16.raw_lo, c16.relu, c16.relu_lo)
+            q = p + '.up_16_8.out_conv'
+            g8_raw, g8_lo, g8_relu, _ = ops.up2_add_split(p16, p16_lo, skip8, skip8_lo)
+            y = self._C(q + '.c1', g8_relu, want_relu=True, want_lo=self._tl(q + '.c2'))
+            short = self._C(q + '.ds', g8_raw, g8_lo, want_raw=True, want_lo=True)
+            o8 = self._C(q + '.c2', y.relu, y.relu_lo, res=short.raw, res_lo=short.raw_lo, want_raw=True, want_lo=True)
+            p8 = o8.raw
+            q = p + '.up_8_4.out_conv'
+            g4_raw, g4_lo, g4_relu, g4_relu_lo8 = ops.up2_add_split(p8, o8.raw_lo, skip4, skip4_lo, want_relu_lo8=True)
+            y4 = self._C(q + '.c1', g4_relu, g4_relu_lo8, want_relu=True, want_relu_lo8=True)
+            # p4 = c2(...) + g4; the logit conv pred(relu(p4)) (big_modules.py:189-190) is folded in: the epilogue
+            # emits the 9 per-tap dot products in fp32, a 3x3 gather finishes the convolution.  p4 itself is only
+            # read 4x4-pooled by su.g4_conv, so the epilogue writes that pool instead of p4.
+            o4 = self._C(q + '.c2', y4.relu, y4.relu_lo8, res=g4_raw, res_lo=g4_lo, want_pool4=update_sensory,
+                         head_w=self.pred_w)
             logits = torch.empty(o4.head.shape[0], 4 * hh, 4 * ww, 1, dtype=torch.float32, device=o4.head.device)
             nat.head_gather3x3(o4.head, logits, self.pred_b, o4.head.shape[0], 4 * hh, 4 * ww)
             logits_all.append(logits)

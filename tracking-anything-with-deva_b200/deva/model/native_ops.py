@@ -278,25 +278,14 @@ def maxpool(x: torch.Tensor, x_lo: Optional[torch.Tensor] = None):
     return (y, y_lo) if x_lo is not None else y
 
 
-def up2_add(g: torch.Tensor, skip: torch.Tensor, want_raw=True, want_relu=True):
-    b, h, w, c = g.shape
-    assert skip.shape == (1, 2 * h, 2 * w, c)
-    raw = torch.empty(b, 2 * h, 2 * w, c, dtype=torch.float16, device=g.device) if want_raw else None
-    relu = torch.empty(b, 2 * h, 2 * w, c, dtype=torch.float16, device=g.device) if want_relu else None
-    nat.up2_add(g, skip, raw, relu, b, h, w, c)
-    return raw, relu
-
-
-def up2_add_split(g: torch.Tensor, g_lo: torch.Tensor, skip: torch.Tensor, skip_lo: Optional[torch.Tensor] = None,
-                  want_raw: bool = True, want_relu_lo8: bool = False):
+def up2_add_split(g: torch.Tensor, g_lo: torch.Tensor, skip: torch.Tensor, skip_lo: torch.Tensor,
+                  want_relu_lo8: bool = False):
     """(g + g_lo) bilinear x2 + (skip + skip_lo) -> (raw, raw_lo, relu, relu_lo8): the residual stream stays a fp16
     hi/lo pair; relu_lo8 (the e4m3 remainder of relu) only when the consumer runs the fp8 correction pass."""
     b, h, w, c = g.shape
-    assert skip.shape == (1, 2 * h, 2 * w, c) and g_lo.shape == g.shape
-    assert skip_lo is None or skip_lo.shape == skip.shape
+    assert skip.shape == (1, 2 * h, 2 * w, c) and g_lo.shape == g.shape and skip_lo.shape == skip.shape
     new = lambda: torch.empty(b, 2 * h, 2 * w, c, dtype=torch.float16, device=g.device)  # noqa: E731
-    raw, raw_lo = (new(), new()) if want_raw else (None, None)
-    relu = new()
+    raw, raw_lo, relu = new(), new(), new()
     relu_lo8 = torch.empty(b, 2 * h, 2 * w, c, dtype=torch.uint8, device=g.device) if want_relu_lo8 else None
     nat.up2_add_split(g, g_lo, skip, raw, raw_lo, relu, b, h, w, c, skip_lo=skip_lo, relu_lo8=relu_lo8)
     return raw, raw_lo, relu, relu_lo8
@@ -317,20 +306,9 @@ def area_down_plane(x: torch.Tensor, r: int) -> torch.Tensor:
     return y
 
 
-def cbam_residual(x: torch.Tensor, params: dict, want_raw=True, want_relu=True):
-    """x + CBAM(x) on fp16 NHWC; params: w1,b1,w2,b2 (channel MLP), ws [2*49], bs [1] (fp32)."""
-    b, h, w, c = x.shape
-    r = params['w1'].shape[0]
-    scratch = torch.empty((2 * CBAM_POOL_SPLIT + 1) * b * c + 2 * b * h * w, dtype=torch.float32, device=x.device)
-    raw = torch.empty_like(x) if want_raw else None
-    relu = torch.empty_like(x) if want_relu else None
-    nat.cbam(x, params['w1'], params['b1'], params['w2'], params['b2'], params['ws'], params['bs'], scratch, raw, relu,
-             b, h, w, c, r)
-    return raw, relu
-
-
 def cbam_residual_split(x: torch.Tensor, x_lo: torch.Tensor, params: dict):
-    """(x + x_lo) + CBAM(x + x_lo) -> (raw, raw_lo, relu)."""
+    """(x + x_lo) + CBAM(x + x_lo) -> (raw, raw_lo, relu) on fp16 NHWC; params: w1,b1,w2,b2 (channel MLP), ws [2*49],
+    bs [1] (fp32)."""
     b, h, w, c = x.shape
     r = params['w1'].shape[0]
     scratch = torch.empty((2 * CBAM_POOL_SPLIT + 1) * b * c + 2 * b * h * w, dtype=torch.float32, device=x.device)
