@@ -27,7 +27,8 @@
 extern "C" {
 #endif
 
-/* v20: dropped deva_b200_up2_add and deva_b200_cbam (single-fp16 residual stream); deva_b200_up2_add_split requires skip_lo
+/* v21: deva_b200_png_bound, deva_b200_png_workspace_bytes and deva_b200_png_encode (result PNGs encoded on the device).
+ * v20: dropped deva_b200_up2_add and deva_b200_cbam (single-fp16 residual stream); deva_b200_up2_add_split requires skip_lo
  * and raw / raw_lo.
  * v19: deva_b200_mask_stats(_workspace_bytes), deva_b200_mask_scored_argmax and deva_b200_mask_last_cover (detector
  * masks -> detection id map).
@@ -39,7 +40,7 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 20
+#define DEVA_B200_ABI_VERSION 21
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -400,6 +401,18 @@ DEVA_B200_API int deva_b200_mask_scored_argmax(const uint8_t* masks, int n, int 
 DEVA_B200_API int deva_b200_mask_last_cover(const uint8_t* masks, int n, int h, int w, int out_h, int out_w,
                                             const int32_t* order, int32_t* slot, int32_t* covered,
                                             deva_stream_t stream);
+
+/* ---- PNG image data (deva/utils/png_encode.py; the format is DESIGN §7) ------------------------------------------
+ * img u8 [h, w] (channels 1: an L or P image, at bits 1, 2, 4 or 8) or [h, w, 3] (channels 3, bits 8).  Writes the zlib
+ * stream of the PNG's IDAT to out and its byte length to out_len (int64 [1]), both on the device; the chunks around it
+ * are the caller's.  Rows are Up-filtered, tokenised greedily at distances 1 and bytes-per-pixel and coded with
+ * deflate's fixed Huffman codes, so the bytes are a function of the image alone.  out: deva_b200_png_bound(h, w,
+ * channels, bits) bytes (every filtered byte a 9-bit literal, rounded up to 4 bytes), 4-byte aligned; workspace:
+ * deva_b200_png_workspace_bytes(h) bytes, 8-byte aligned.  A row's bytes + 5 must fit in a block's shared memory. */
+DEVA_B200_API size_t deva_b200_png_bound(int h, int w, int channels, int bits);
+DEVA_B200_API size_t deva_b200_png_workspace_bytes(int h);
+DEVA_B200_API int deva_b200_png_encode(const uint8_t* img, int h, int w, int channels, int bits, void* workspace,
+                                       uint8_t* out, int64_t* out_len, deva_stream_t stream);
 
 #ifdef __cplusplus
 }

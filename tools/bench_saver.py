@@ -153,14 +153,15 @@ def encode_ms(n=5):
     return out
 
 
-def e2e(savers, steps, ref_steps, warmup=RING_SIZE + 1):
+def e2e(savers, steps, ref_steps, warmup=RING_SIZE + 1, impls=('none', 'ours', 'reference')):
+    """impls: 'none' (no saver) and keys of savers, in the order they run; 'reference' runs ref_steps steps."""
     from deva.inference.frame_io import frame_from_rgb8
     wl = dict(bench.WORKLOADS['c2'], w=853)  # frame_from_rgb8(size=480)'s output for a 1920x1080 frame
     g = torch.Generator().manual_seed(1)
     frames = [torch.randint(0, 256, (1080, 1920, 3), generator=g, dtype=torch.uint8).pin_memory() for _ in range(5)]
     images = [f.numpy() for f in frames]
     out = {}
-    for impl in ('none', 'ours', 'reference'):
+    for impl in impls:
         clip = bench.Clip(wl, torch.device('cuda', 0), seed=0)
         clip.core.object_manager.use_long_id = True
         n = ref_steps if impl == 'reference' else steps

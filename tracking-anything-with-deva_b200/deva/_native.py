@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 20
+ABI_VERSION = 21
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -116,6 +116,9 @@ _SIGNATURES = {
                                              c_void_p, c_void_p, c_void_p]),
     'deva_b200_mask_last_cover': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                           c_void_p]),
+    'deva_b200_png_bound': (c_size_t, [c_int, c_int, c_int, c_int]),
+    'deva_b200_png_workspace_bytes': (c_size_t, [c_int]),
+    'deva_b200_png_encode': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -495,6 +498,27 @@ def mask_last_cover(masks, out_h, out_w, order, slot, covered):
     _i32(order, n), _i32(slot, out_h * out_w), _i32(covered, n)
     _check(lib().deva_b200_mask_last_cover(_ptr(m), n, h, w, out_h, out_w, _ptr(order), _ptr(slot), _ptr(covered),
                                            _stream()), 'mask_last_cover')
+
+
+def png_bound(h, w, channels, bits) -> int:
+    return int(lib().deva_b200_png_bound(h, w, channels, bits))
+
+
+def png_workspace_bytes(h) -> int:
+    return int(lib().deva_b200_png_workspace_bytes(h))
+
+
+def png_encode(img, bits, workspace, out, out_len):
+    """img uint8 [h, w] or [h, w, 3]; out: png_bound bytes, 4-byte aligned; out_len int64 [1]; workspace:
+    png_workspace_bytes, 8-byte aligned (see include/deva_b200.h)."""
+    assert img.dtype == torch.uint8 and img.is_cuda and img.is_contiguous() and img.dim() in (2, 3), (img.dtype,
+                                                                                                      img.shape)
+    h, w = img.shape[:2]
+    channels = 1 if img.dim() == 2 else img.shape[2]
+    assert out.numel() * out.element_size() >= png_bound(h, w, channels, bits) and out_len.dtype == torch.int64
+    assert workspace.numel() * workspace.element_size() >= png_workspace_bytes(h)
+    _check(lib().deva_b200_png_encode(_ptr(img), h, w, channels, bits, _ptr(workspace), _ptr(out), _ptr(out_len),
+                                      _stream()), 'png_encode')
 
 
 def transpose_append(src, dst, ld_dst, n, c):

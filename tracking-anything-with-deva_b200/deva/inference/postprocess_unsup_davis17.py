@@ -15,8 +15,10 @@ Per video each file is decoded once on a pool of host threads and uploaded throu
 the device for both passes.  ``deva_b200_label_areas`` counts every frame's labels, and the per-frame lists come to the
 host once; the selection runs there, on lists of at most a few thousand entries.  The (label -> index) table goes back
 to the device, ``deva_b200_label_to_index`` rewrites every frame, and the index maps come back through pinned memory
-to be encoded on the thread pool.  Files are read in full before any of their video is written, so input_path ==
-output_path (as evaluation/eval_with_detections.py calls it) is safe.
+to be encoded on the thread pool.  With ``png_encoder='device'`` (or ``DEVA_B200_PNG_ENCODER=device``) they are encoded
+as PNGs on the device instead (deva/utils/png_encode.py), and only the compressed files come back.  Files are read in
+full before any of their video is written, so input_path == output_path (as evaluation/eval_with_detections.py calls
+it) is safe.
 
 Supported frames are P, L, RGB and RGBA uint8 images (everything the result saver writes); another mode raises
 ``ValueError`` naming the file, where the reference would read the frame.  Importing this module does not initialise
@@ -30,6 +32,7 @@ import numpy as np
 import torch
 from PIL import Image
 
+from deva.utils.png_encode import encode_png_async, resolve_encoder, write_png
 from deva.utils.png_pipeline import Decoder, Uploader
 
 CAPACITY = 1024  # label table entries per frame; a frame with more distinct labels is counted again with a larger table
@@ -104,7 +107,7 @@ def index_table(existing_objects):
     return labels, np.array([last[v] for v in labels.tolist()], np.int32)
 
 
-def _limit_video(decoder, upload, video_path, out_dir, max_num_objects, palette):
+def _limit_video(decoder, upload, video_path, out_dir, max_num_objects, palette, png_encoder):
     from deva import _native
     dev = upload.device
     frames = sorted(os.listdir(video_path))
@@ -133,25 +136,32 @@ def _limit_video(decoder, upload, video_path, out_dir, max_num_objects, palette)
     for f in on_dev:
         starts.append(starts[-1] + (f.shape[0] * f.shape[1] + 15) // 16 * 16)
     out = torch.empty(starts[-1], dtype=torch.uint8, device=dev)
-    for f, s in zip(on_dev, starts):
-        _native.label_to_index(f, labels, index, out[s:s + f.shape[0] * f.shape[1]].view(f.shape[0], f.shape[1]))
-    host = torch.empty(out.numel(), dtype=torch.uint8, pin_memory=True)
-    host.copy_(out, non_blocking=True)
-    torch.cuda.current_stream().synchronize()
-    host_np = host.numpy()
+    maps = [out[s:s + f.shape[0] * f.shape[1]].view(f.shape[0], f.shape[1]) for f, s in zip(on_dev, starts)]
+    for f, m in zip(on_dev, maps):
+        _native.label_to_index(f, labels, index, m)
     os.makedirs(out_dir, exist_ok=True)
-    writes = [decoder.pool.submit(_save, host_np[s:s + f.shape[0] * f.shape[1]].reshape(f.shape[0], f.shape[1]),
-                                  palette, path.join(out_dir, name))
-              for f, s, name in zip(on_dev, starts, frames)]
+    if png_encoder == 'device':
+        pngs = [encode_png_async(m, 'P', palette) for m in maps]
+        writes = [decoder.pool.submit(write_png, p, path.join(out_dir, name)) for p, name in zip(pngs, frames)]
+    else:
+        host = torch.empty(out.numel(), dtype=torch.uint8, pin_memory=True)
+        host.copy_(out, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        host_np = host.numpy()
+        writes = [decoder.pool.submit(_save, host_np[s:s + f.shape[0] * f.shape[1]].reshape(f.shape[0], f.shape[1]),
+                                      palette, path.join(out_dir, name))
+                  for f, s, name in zip(on_dev, starts, frames)]
     for w in writes:
         w.result()
     if unreadable is not None:
         raise unreadable  # the rewrite pass wrote the frames before it
 
 
-def limit_max_id(input_path, output_path, max_num_objects=20, *, palette=None, num_threads=None):
+def limit_max_id(input_path, output_path, max_num_objects=20, *, palette=None, num_threads=None, png_encoder=None):
     """palette: the PNGs' palette; None = DAVIS's (deva.utils.palette.davis_palette, which comes from the reference
-    checkout).  num_threads: host threads that decode and encode PNGs."""
+    checkout).  num_threads: host threads that decode and encode PNGs.  png_encoder: 'pil' or 'device'; None reads
+    DEVA_B200_PNG_ENCODER (default 'pil')."""
+    png_encoder = resolve_encoder(png_encoder)
     if palette is None:
         from deva.utils.palette import davis_palette as palette
     from deva import _native
@@ -161,7 +171,7 @@ def limit_max_id(input_path, output_path, max_num_objects=20, *, palette=None, n
     try:
         for video in sorted(os.listdir(input_path)):
             _limit_video(decoder, upload, path.join(input_path, video), path.join(output_path, video), max_num_objects,
-                         palette)
+                         palette, png_encoder)
     finally:
         decoder.close()
 

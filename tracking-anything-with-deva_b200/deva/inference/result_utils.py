@@ -7,6 +7,10 @@ records an event and queues the frame; it never synchronises the host.  The writ
 only what has to stay on the host: PIL images and PNG / JPEG encoding, the JSON entries, the gradio writer, and the two
 paths that need third-party code - ``supervision`` boxes and labels for prompts, and ``pycocotools`` RLE for burst (the
 one per-object host loop left; a device RLE would remove it).  Both libraries are imported only when those paths run.
+
+With ``png_encoder='device'`` (or ``DEVA_B200_PNG_ENCODER=device``) the id image is encoded as a PNG on the device too
+(deva/utils/png_encode.py), right after ``prob_to_segments`` on the same stream: only the compressed stream comes to the
+host, and the writer thread writes its bytes.  The files decode to the pixels, mode and palette Pillow's files decode to.
 """
 import copy
 import os
@@ -21,14 +25,19 @@ import torch
 from PIL import Image
 
 from deva.inference.frame_io import prob_to_ids, prob_to_segments
+from deva.utils.png_encode import PREFIX as PNG_PREFIX, PendingPng, encode_png_async, resolve_encoder, write_png
 
 QUEUE_SIZE = 10
 RING_SIZE = QUEUE_SIZE + 2  # the queued frames, the one the writer holds and the one save_mask is filling
 
 
 class ResultSaver:
-    def __init__(self, output_root: str, video_name: str, *, dataset: str, object_manager, palette=None):
+    def __init__(self, output_root: str, video_name: str, *, dataset: str, object_manager, palette=None,
+                 png_encoder: Optional[str] = None):
+        """png_encoder: 'pil' (Pillow on the writer thread) or 'device'; None reads DEVA_B200_PNG_ENCODER (default
+        'pil')."""
         self.output_root = output_root
+        self.png_encoder = resolve_encoder(png_encoder)
         self.video_name = video_name
         self.dataset = dataset.lower()
         self.palette = palette
@@ -108,9 +117,17 @@ class ResultSaver:
         seg = prob_to_segments(prob, self.object_manager, size, index=save_the_mask and not long_id,
                                rgb=save_the_mask and long_id, frame=frame,
                                stats=self.json_style is not None or self.visualize, remap=self.need_remapping)
+        png = None
+        if save_the_mask and self.png_encoder == 'device' and self.dataset != 'gradio':
+            png = encode_png_async(seg.rgb if long_id else seg.index,
+                                   'RGB' if long_id else 'L' if self.palette is None else 'P', self.palette,
+                                   host=_pinned(slot, 'png', (8 + PNG_PREFIX, ), torch.uint8))
         host = {}
         for name in ('index', 'rgb', 'overlay', 'counts', 'boxes'):
             t = getattr(seg, name)
+            # an encoded id image stays on the device; the host blend still needs the RGB ids
+            if png is not None and (name == 'index' or (name == 'rgb' and not (overlay and not on_device))):
+                continue
             if t is not None:
                 host[name] = _pinned(slot, name, t.shape, t.dtype)
                 host[name].copy_(t, non_blocking=True)
@@ -137,6 +154,7 @@ class ResultSaver:
             path_to_image=path_to_image,
             all_obj_ids=[int(o.id) for o in self.object_manager.obj_to_tmp_id],
             segments_info=copy.deepcopy(self.object_manager.get_current_segments_info()),
+            png=png,
         ))
 
     def end(self):
@@ -168,6 +186,7 @@ class ResultArgs:
     path_to_image: str
     all_obj_ids: List[int]
     segments_info: List[Dict]
+    png: Optional[PendingPng] = None  # the id image's PNG, encoded on the device
 
 
 def save_result(queue: Queue):
@@ -221,15 +240,17 @@ def _write(args: ResultArgs):
 
     if not args.save_the_mask:
         return
-    if args.long_id:
-        rgb_mask = host['rgb'].numpy()
-        out_img = Image.fromarray(rgb_mask)
+    if args.png is not None:
+        write_png(args.png, _path(saver, saver.output_postfix, frame_name[:-4] + '.png'))
     else:
-        out_img = Image.fromarray(host['index'].numpy())
-        if saver.palette is not None:
-            out_img.putpalette(saver.palette)
-    if saver.dataset != 'gradio':
-        _save(out_img, saver, saver.output_postfix, frame_name[:-4] + '.png')
+        if args.long_id:
+            out_img = Image.fromarray(host['rgb'].numpy())
+        else:
+            out_img = Image.fromarray(host['index'].numpy())
+            if saver.palette is not None:
+                out_img.putpalette(saver.palette)
+        if saver.dataset != 'gradio':
+            _save(out_img, saver, saver.output_postfix, frame_name[:-4] + '.png')
 
     if not (saver.visualize and args.long_id):
         return
@@ -241,7 +262,7 @@ def _write(args: ResultArgs):
             image_np = np.array(Image.open(args.path_to_image))
         # the reference's blend: alpha = 1 where the id is 0, else 0.5
         alpha = (host['ids'].numpy() == 0).astype(np.float32)[:, :, None] * 0.5 + 0.5
-        blend = (image_np * alpha + rgb_mask * (1 - alpha)).astype(np.uint8)
+        blend = (image_np * alpha + host['rgb'].numpy() * (1 - alpha)).astype(np.uint8)
 
     if args.prompts is not None and len(segments_info) > 0:
         import supervision as sv
@@ -258,9 +279,13 @@ def _write(args: ResultArgs):
         saver.writer.write(blend[:, :, ::-1])
 
 
-def _save(img: Image.Image, saver: ResultSaver, postfix: Optional[str], name: str):
+def _path(saver: ResultSaver, postfix: Optional[str], name: str) -> str:
     out = path.join(saver.output_root, postfix) if postfix is not None else saver.output_root
     if saver.video_name is not None:
         out = path.join(out, saver.video_name)
     os.makedirs(out, exist_ok=True)
-    img.save(path.join(out, name))
+    return path.join(out, name)
+
+
+def _save(img: Image.Image, saver: ResultSaver, postfix: Optional[str], name: str):
+    img.save(_path(saver, postfix, name))

@@ -5,7 +5,8 @@ Per video, IDPostprocessor's rules run on the host over the JSON entries alone: 
 new id, every stuff category maps to one id, and a collision draws from the global ``np.random`` as the reference does.
 That gives each frame a table -> output-id rewrite, which ``deva_b200_pano_remap`` applies per pixel while it writes the
 RGB of the new id and counts the pixels of every output id (the areas that decide which stuff entries are kept).  PNGs
-are decoded and encoded on a pool of host threads.
+are decoded and encoded on a pool of host threads; with ``png_encoder='device'`` (or ``DEVA_B200_PNG_ENCODER=device``)
+the rewritten maps are encoded on the device (deva/utils/png_encode.py) and only the compressed files come back.
 
 Videos are processed in order in this process.  The reference maps them over ``Pool(16)``, so its random draws depend on
 which worker handles which video; here they follow the order of ``pred.json``, as a serial run of the reference's
@@ -19,6 +20,7 @@ import numpy as np
 import torch
 from PIL import Image
 
+from deva.utils.png_encode import encode_png_async, resolve_encoder, write_png
 from deva.vps_metrics import scoring, video_pass
 
 
@@ -26,9 +28,11 @@ def _save(rgb: np.ndarray, file: str):
     Image.fromarray(rgb).save(file)
 
 
-def merge_stuff(input_path, output_path, isthing=None, num_threads=None):
+def merge_stuff(input_path, output_path, isthing=None, num_threads=None, *, png_encoder=None):
     """isthing: {category id: bool}; None = the VIPSeg category table (deva.utils.pano_utils.vipseg_cat_to_isthing,
-    which comes from the reference checkout)."""
+    which comes from the reference checkout).  png_encoder: 'pil' or 'device'; None reads DEVA_B200_PNG_ENCODER
+    (default 'pil')."""
+    png_encoder = resolve_encoder(png_encoder)
     if isthing is None:
         from deva.utils.pano_utils import vipseg_cat_to_isthing as isthing
     from deva import _native
@@ -56,13 +60,16 @@ def merge_stuff(input_path, output_path, isthing=None, num_threads=None):
                 _native.pano_remap(upload(mask), ids, torch.from_numpy(slot).to(dev, non_blocking=True),
                                    torch.from_numpy(out_ids).to(dev, non_blocking=True), out,
                                    counts[t, :len(out_ids)], unknown[t])
-                outs.append(out)
+                outs.append(encode_png_async(out, 'RGB') if png_encoder == 'device' else out)
             counts_h = counts.cpu().numpy()
             video_annotations = []
             for t, (ann, (slot, out_ids, things, stuff_to_id)) in enumerate(zip(vid_ann['annotations'], frames)):
                 segments = scoring.merged_segments(things, stuff_to_id, out_ids, counts_h[t, :len(out_ids)], isthing)
                 video_annotations.append({'file_name': ann['file_name'], 'segments_info': segments})
-                writes.append(decoder.pool.submit(_save, outs[t].cpu().numpy(), path.join(out_dir, names[t])))
+                if png_encoder == 'device':
+                    writes.append(decoder.pool.submit(write_png, outs[t], path.join(out_dir, names[t])))
+                else:
+                    writes.append(decoder.pool.submit(_save, outs[t].cpu().numpy(), path.join(out_dir, names[t])))
             output_annotations.append({'video_id': video_id, 'annotations': video_annotations})
         for w in writes:
             w.result()
