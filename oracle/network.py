@@ -4,7 +4,8 @@ Test infrastructure (see oracle/__init__.py).  Restates, layer for layer,
 deva/model/network.py:33-173, big_modules.py:23-212, modules.py:22-169,
 group_modules.py:17-152, cbam.py:21-77 and resnet.py:46-152 of the reference.  Nothing is
 folded or reordered: BatchNorm stays a separate eval-mode op so the result is the
-reference's fp32 arithmetic.
+reference's fp32 arithmetic.  Every function keeps the dtype it is given, so a state dict and inputs upcast to float64
+replay the same network in float64 (tests/test_engine_float64_gpu.py measures the native engine against that).
 
 Tensor conventions follow the reference: images [1,3,H,W]; per-object tensors
 [1,K,C,h,w]; ``sd`` is the flat checkpoint dict (``pixel_encoder.*``, ``mask_encoder.*``,
@@ -146,9 +147,14 @@ def encode_mask(sd: SD, image, ms_features, sensory, masks, deep_update=True):
 
 
 # ---------------------------------------------------------------------------------- decoder
+def _at_least_f32(x):
+    """The reference's ``.float()``, except that float64 stays float64 (a float64 replay of the network)."""
+    return x.to(torch.promote_types(x.dtype, torch.float32))
+
+
 def aggregate(prob, dim: int):
     """network.py:33-40."""
-    prob = prob.float()
+    prob = _at_least_f32(prob)
     full = torch.cat([torch.prod(1 - prob, dim=dim, keepdim=True), prob], dim).clamp(1e-7, 1 - 1e-7)
     return torch.log(full / (1 - full))
 
@@ -157,6 +163,17 @@ def segment(sd: SD, ms_features, readout, sensory, last_mask, update_sensory=Tru
     """network.py:94-173 (inference branch) -> big_modules.py:147-212.
 
     readout/sensory [1,K,512,h,w]; last_mask [1,K,H,W].  Returns (sensory, logits, prob).
+    """
+    sensory, logits = decode(sd, ms_features, readout, sensory, last_mask, update_sensory)
+    logits, prob = output_tail(logits)
+    return sensory, logits, prob
+
+
+def decode(sd: SD, ms_features, readout, sensory, last_mask, update_sensory=True):
+    """The decoder up to the logits, before the objects meet in ``aggregate``: every object's result depends on its own
+    readout / sensory / mask only (quirk Q11), so the objects can be run one at a time.
+
+    readout/sensory [1,K,512,h,w]; last_mask [1,K,H,W].  Returns (sensory, logits [1,K,H/4,W/4]).
     """
     p = 'mask_decoder'
     f16, f8, f4 = ms_features
@@ -169,7 +186,7 @@ def segment(sd: SD, ms_features, readout, sensory, last_mask, update_sensory=Tru
     p16 = _fusion(sd, p + '.fuser', f16, p16)
     p8 = _group_resblock(sd, p + '.up_16_8.out_conv', skip8.unsqueeze(1) + _resize_groups(p16, 2, 'bilinear'))
     p4 = _group_resblock(sd, p + '.up_8_4.out_conv', skip4.unsqueeze(1) + _resize_groups(p8, 2, 'bilinear'))
-    logits = _conv(sd, p + '.pred', F.relu(p4.flatten(0, 1).float()), pad=1)
+    logits = _conv(sd, p + '.pred', F.relu(_at_least_f32(p4.flatten(0, 1))), pad=1)
 
     if update_sensory:
         p4x = torch.cat([p4, logits.view(b, k, 1, *logits.shape[-2:])], 2)
@@ -179,9 +196,13 @@ def segment(sd: SD, ms_features, readout, sensory, last_mask, update_sensory=Tru
             _gconv(sd, su + '.g4_conv', _resize_groups(p4x, 1 / 4, 'area'))
         vals = _gconv(sd, su + '.transform', torch.cat([g, sensory], 2), pad=1)
         sensory = _gru(vals, sensory, sensory.shape[2])
+    return sensory, logits.view(b, k, *logits.shape[-2:])
 
-    logits = logits.view(b, k, *logits.shape[-2:])
+
+def output_tail(logits):
+    """network.py:144 and :164-168: per-object logits [1,K,h4,w4] -> soft aggregation over all K objects, x4 bilinear,
+    softmax.  Returns (aggregated logits [1,K+1,4*h4,4*w4], prob)."""
     prob = torch.sigmoid(logits)
     logits = aggregate(prob, dim=1)
     logits = F.interpolate(logits, scale_factor=4, mode='bilinear', align_corners=False)
-    return sensory, logits, F.softmax(logits, dim=1)
+    return logits, F.softmax(logits, dim=1)

@@ -59,6 +59,45 @@ def test_network_stages_match_reference(golden_dir, synthetic_sd):
     torch.testing.assert_close(logits, g['logits'], rtol=1e-4, atol=1e-4)
     torch.testing.assert_close(prob, g['prob'], rtol=1e-4, atol=1e-5)
     torch.testing.assert_close(net.aggregate(g['masks'][0] * 0.9, dim=0), g['aggregate'])
+    s2b, lg = net.decode(sd, ms, g['readout'], g['sensory1'], g['masks'])
+    assert torch.equal(s2b, s2) and torch.equal(net.output_tail(lg)[1], prob)
+
+
+def test_network_stages_float64_match_reference(golden_dir, synthetic_sd):
+    """The oracle replayed in float64 (the reference for tests/test_engine_float64_gpu.py) against the fp32 reference.
+
+    Measured (max abs error relative to max |fixture|): <= 1.6e-6 through the encoders, 5.0e-6 on sensory2, 1.7e-6 /
+    4.5e-6 on logits / prob when the output tail runs in fp32: the bound REL = 2e-5 leaves a 4x margin.  The float64
+    tail itself sits further from the fixture (1.8e-4 abs on the logits, 4.5e-5 on prob): the fixture's fp32
+    ``aggregate`` takes log(p / (1 - p)) with 1 - p cancelling where p nears 1, so the gap is the fp32 reference's own
+    rounding, bounded here at 4x what was measured."""
+    REL = 2e-5
+    g = _load(golden_dir, 'network_stages.npz')
+    sd = {k: v.double() if v.is_floating_point() else v for k, v in synthetic_sd.items()}
+    d = {k: v.double() for k, v in g.items()}
+
+    def rel(a, name):
+        assert a.dtype == torch.float64, (name, a.dtype)
+        return float((a - d[name]).abs().max()) / float(d[name].abs().max())
+
+    ms, feat = net.encode_image(sd, d['image'])
+    key, shr, sel = net.transform_key(sd, feat)
+    value, s1 = net.encode_mask(sd, d['image'], ms, d['sensory0'], d['masks'])
+    s2, lg = net.decode(sd, ms, d['readout'], d['sensory1'], d['masks'])
+    logits32, prob32 = net.output_tail(lg.float())
+    logits, prob = net.output_tail(lg)
+    errs = {name: rel(a, name) for name, a in (
+        ('f16', ms[0]), ('f8', ms[1]), ('f4', ms[2]), ('feat', feat), ('key', key), ('shrinkage', shr),
+        ('selection', sel), ('value', value), ('sensory1', s1), ('sensory2', s2))}
+    errs['logits (fp32 tail)'] = float((logits32 - g['logits']).abs().max()) / float(g['logits'].abs().max())
+    errs['prob (fp32 tail)'] = float((prob32 - g['prob']).abs().max()) / float(g['prob'].abs().max())
+    for name, e in errs.items():
+        print(f'float64 oracle {name:20s} rel {e:.3e}  bound {REL:.0e}')
+        assert e < REL, (name, e)
+    tail = {'logits': float((logits - d['logits']).abs().max()), 'prob': float((prob - d['prob']).abs().max())}
+    for name, e, bound in (('logits', tail['logits'], 7e-4), ('prob', tail['prob'], 2e-4)):
+        print(f'float64 oracle {name:20s} abs {e:.3e}  bound {bound:.0e}')
+        assert e < bound, (name, e)
 
 
 def test_vos_steps_match_reference(golden_dir, synthetic_sd):
