@@ -27,7 +27,9 @@
 extern "C" {
 #endif
 
-/* v21: deva_b200_png_bound, deva_b200_png_workspace_bytes and deva_b200_png_encode (result PNGs encoded on the device).
+/* v22: deva_b200_jpeg_bound, deva_b200_jpeg_workspace_bytes and deva_b200_jpeg_encode (result JPEGs encoded on the
+ * device).
+ * v21: deva_b200_png_bound, deva_b200_png_workspace_bytes and deva_b200_png_encode (result PNGs encoded on the device).
  * v20: dropped deva_b200_up2_add and deva_b200_cbam (single-fp16 residual stream); deva_b200_up2_add_split requires skip_lo
  * and raw / raw_lo.
  * v19: deva_b200_mask_stats(_workspace_bytes), deva_b200_mask_scored_argmax and deva_b200_mask_last_cover (detector
@@ -40,7 +42,7 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 21
+#define DEVA_B200_ABI_VERSION 22
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -413,6 +415,19 @@ DEVA_B200_API size_t deva_b200_png_bound(int h, int w, int channels, int bits);
 DEVA_B200_API size_t deva_b200_png_workspace_bytes(int h);
 DEVA_B200_API int deva_b200_png_encode(const uint8_t* img, int h, int w, int channels, int bits, void* workspace,
                                        uint8_t* out, int64_t* out_len, deva_stream_t stream);
+
+/* ---- baseline JPEG scan (deva/utils/jpeg_encode.py; the format is DESIGN §7) --------------------------------------
+ * img u8 [h, w, 3] RGB, 1 <= h, w <= 65535.  Writes the entropy-coded segment of a baseline 4:2:0 JPEG followed by EOI
+ * to out and its byte length to out_len (int64 [1]), both on the device; the marker segments before it (SOI .. SOS) are
+ * the caller's.  The arithmetic is libjpeg's (jccolor.c colour, h2v2 downsampling with libjpeg's edge padding, islow
+ * DCT, rounding quantisation, Annex K Huffman tables, 1-bit fill, 0x00 after every 0xFF), so the bytes are a function of
+ * the image and the tables alone and equal Pillow's default save.  quality_tables: HOST, 64 luma then 64 chroma
+ * quantisation values in zigzag order, each in [1, 255].  out: deva_b200_jpeg_bound(h, w) bytes (every block at its
+ * worst case, every byte stuffed, plus EOI); workspace: deva_b200_jpeg_workspace_bytes(h, w) bytes, 16-byte aligned. */
+DEVA_B200_API size_t deva_b200_jpeg_bound(int h, int w);
+DEVA_B200_API size_t deva_b200_jpeg_workspace_bytes(int h, int w);
+DEVA_B200_API int deva_b200_jpeg_encode(const uint8_t* img, int h, int w, const uint8_t* quality_tables, void* workspace,
+                                        uint8_t* out, int64_t* out_len, deva_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 21
+ABI_VERSION = 22
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -119,6 +119,9 @@ _SIGNATURES = {
     'deva_b200_png_bound': (c_size_t, [c_int, c_int, c_int, c_int]),
     'deva_b200_png_workspace_bytes': (c_size_t, [c_int]),
     'deva_b200_png_encode': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'deva_b200_jpeg_bound': (c_size_t, [c_int, c_int]),
+    'deva_b200_jpeg_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'deva_b200_jpeg_encode': (c_int, [c_void_p, c_int, c_int, c_char_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -519,6 +522,27 @@ def png_encode(img, bits, workspace, out, out_len):
     assert workspace.numel() * workspace.element_size() >= png_workspace_bytes(h)
     _check(lib().deva_b200_png_encode(_ptr(img), h, w, channels, bits, _ptr(workspace), _ptr(out), _ptr(out_len),
                                       _stream()), 'png_encode')
+
+
+def jpeg_bound(h, w) -> int:
+    return int(lib().deva_b200_jpeg_bound(h, w))
+
+
+def jpeg_workspace_bytes(h, w) -> int:
+    return int(lib().deva_b200_jpeg_workspace_bytes(h, w))
+
+
+def jpeg_encode(img, tables: bytes, workspace, out, out_len):
+    """img uint8 [h, w, 3]; tables: 128 bytes (luma then chroma quantisation, zigzag); out: jpeg_bound bytes; out_len
+    int64 [1]; workspace: jpeg_workspace_bytes, 16-byte aligned (see include/deva_b200.h)."""
+    assert img.dtype == torch.uint8 and img.is_cuda and img.is_contiguous() and img.dim() == 3 and img.shape[2] == 3, \
+        (img.dtype, img.shape)
+    h, w = img.shape[:2]
+    assert len(tables) == 128 and out_len.dtype == torch.int64
+    assert out.numel() * out.element_size() >= jpeg_bound(h, w)
+    assert workspace.numel() * workspace.element_size() >= jpeg_workspace_bytes(h, w)
+    _check(lib().deva_b200_jpeg_encode(_ptr(img), h, w, bytes(tables), _ptr(workspace), _ptr(out), _ptr(out_len),
+                                       _stream()), 'jpeg_encode')
 
 
 def transpose_append(src, dst, ld_dst, n, c):

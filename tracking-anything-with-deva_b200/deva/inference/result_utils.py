@@ -11,6 +11,11 @@ one per-object host loop left; a device RLE would remove it).  Both libraries ar
 With ``png_encoder='device'`` (or ``DEVA_B200_PNG_ENCODER=device``) the id image is encoded as a PNG on the device too
 (deva/utils/png_encode.py), right after ``prob_to_segments`` on the same stream: only the compressed stream comes to the
 host, and the writer thread writes its bytes.  The files decode to the pixels, mode and palette Pillow's files decode to.
+
+With ``jpeg_encoder='device'`` (or ``DEVA_B200_JPEG_ENCODER=device``) the demo overlay JPEG is encoded on the device
+(deva/utils/jpeg_encode.py), byte for byte Pillow's file.  An overlay blended on the device is encoded right after
+``prob_to_segments`` and only its scan comes to the host; an image finished on the host (prompt boxes and labels, or
+the host blend) is encoded by the writer thread.  The gradio writer is unchanged.
 """
 import copy
 import os
@@ -25,6 +30,8 @@ import torch
 from PIL import Image
 
 from deva.inference.frame_io import prob_to_ids, prob_to_segments
+from deva.utils.jpeg_encode import PREFIX as JPEG_PREFIX, PendingJpeg, encode_jpeg, encode_jpeg_async, write_jpeg
+from deva.utils.jpeg_encode import resolve_encoder as resolve_jpeg_encoder
 from deva.utils.png_encode import PREFIX as PNG_PREFIX, PendingPng, encode_png_async, resolve_encoder, write_png
 
 QUEUE_SIZE = 10
@@ -33,11 +40,12 @@ RING_SIZE = QUEUE_SIZE + 2  # the queued frames, the one the writer holds and th
 
 class ResultSaver:
     def __init__(self, output_root: str, video_name: str, *, dataset: str, object_manager, palette=None,
-                 png_encoder: Optional[str] = None):
+                 png_encoder: Optional[str] = None, jpeg_encoder: Optional[str] = None):
         """png_encoder: 'pil' (Pillow on the writer thread) or 'device'; None reads DEVA_B200_PNG_ENCODER (default
-        'pil')."""
+        'pil').  jpeg_encoder: the same for the overlay JPEG; None reads DEVA_B200_JPEG_ENCODER (default 'pil')."""
         self.output_root = output_root
         self.png_encoder = resolve_encoder(png_encoder)
+        self.jpeg_encoder = resolve_jpeg_encoder(jpeg_encoder)
         self.video_name = video_name
         self.dataset = dataset.lower()
         self.palette = palette
@@ -122,11 +130,16 @@ class ResultSaver:
             png = encode_png_async(seg.rgb if long_id else seg.index,
                                    'RGB' if long_id else 'L' if self.palette is None else 'P', self.palette,
                                    host=_pinned(slot, 'png', (8 + PNG_PREFIX, ), torch.uint8))
+        jpeg = None
+        if overlay and on_device and prompts is None and self.jpeg_encoder == 'device' and self.dataset != 'gradio':
+            jpeg = encode_jpeg_async(seg.overlay, host=_pinned(slot, 'jpeg', (8 + JPEG_PREFIX, ), torch.uint8))
         host = {}
         for name in ('index', 'rgb', 'overlay', 'counts', 'boxes'):
             t = getattr(seg, name)
             # an encoded id image stays on the device; the host blend still needs the RGB ids
             if png is not None and (name == 'index' or (name == 'rgb' and not (overlay and not on_device))):
+                continue
+            if jpeg is not None and name == 'overlay':  # an encoded overlay stays on the device
                 continue
             if t is not None:
                 host[name] = _pinned(slot, name, t.shape, t.dtype)
@@ -155,6 +168,7 @@ class ResultSaver:
             all_obj_ids=[int(o.id) for o in self.object_manager.obj_to_tmp_id],
             segments_info=copy.deepcopy(self.object_manager.get_current_segments_info()),
             png=png,
+            jpeg=jpeg,
         ))
 
     def end(self):
@@ -187,6 +201,7 @@ class ResultArgs:
     all_obj_ids: List[int]
     segments_info: List[Dict]
     png: Optional[PendingPng] = None  # the id image's PNG, encoded on the device
+    jpeg: Optional[PendingJpeg] = None  # the overlay's JPEG, encoded on the device
 
 
 def save_result(queue: Queue):
@@ -254,6 +269,9 @@ def _write(args: ResultArgs):
 
     if not (saver.visualize and args.long_id):
         return
+    if args.jpeg is not None:
+        write_jpeg(args.jpeg, _path(saver, saver.visualize_postfix, frame_name[:-4] + '.jpg'))
+        return
     if 'overlay' in host:
         blend = host['overlay'].numpy()
     else:
@@ -273,10 +291,14 @@ def _write(args: ResultArgs):
         blend = sv.BoundingBoxAnnotator().annotate(scene=blend, detections=detections)
         blend = sv.LabelAnnotator().annotate(scene=blend, detections=detections, labels=labels)
 
-    if saver.dataset != 'gradio':
-        _save(Image.fromarray(blend), saver, saver.visualize_postfix, frame_name[:-4] + '.jpg')
-    else:
+    if saver.dataset == 'gradio':
         saver.writer.write(blend[:, :, ::-1])
+    elif saver.jpeg_encoder == 'device':  # an image finished on the host
+        data = encode_jpeg(blend)
+        with open(_path(saver, saver.visualize_postfix, frame_name[:-4] + '.jpg'), 'wb') as f:
+            f.write(data)
+    else:
+        _save(Image.fromarray(blend), saver, saver.visualize_postfix, frame_name[:-4] + '.jpg')
 
 
 def _path(saver: ResultSaver, postfix: Optional[str], name: str) -> str:
