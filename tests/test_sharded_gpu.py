@@ -3,7 +3,9 @@
 * one rank (no process group): the sharded code path - candidate merge, scatter read-out into the peer buffer,
   object-partitioned decode, token-sliced append, distributed consolidation hooks - must reproduce the plain core;
 * two ranks over NCCL (skipped on a 1-GPU box): every rank must return the same probabilities as the unsharded run;
-  slots, objects and prototypes are really split (bank sizes are halves)."""
+  slots, objects and prototypes are really split (bank sizes are halves).  What this test adds is the NCCL transport and
+  peer memory on a second device; the multi-rank logic itself runs on ONE GPU, at 2, 3 and 4 ranks against float64 and
+  the plain core, in tests/test_sharded_ranks_gpu.py."""
 import json
 import os
 import socket

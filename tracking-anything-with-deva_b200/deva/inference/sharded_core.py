@@ -21,7 +21,8 @@ exactly its per-frame math (inference_core.py:55-113,200-290; memory_manager.py:
   ranks (the "pre-softmax max/sum" exchange), partial prototype values summed by all-reduce.
 
 ``world == 1`` (no process group) degenerates to the plain single-GPU math through the same code, which is how the
-1-GPU test-suite covers it; ``tests/test_sharded_gpu.py`` runs it on 2 ranks against the unsharded core.
+1-GPU test-suite covers it; ``tests/test_sharded_ranks_gpu.py`` runs 2, 3 and 4 ranks as processes on one GPU against float64
+and the unsharded core, ``tests/test_sharded_gpu.py`` 2 ranks over NCCL on 2 GPUs.
 """
 from typing import Dict, Iterable, List, Optional, Tuple
 
