@@ -27,7 +27,9 @@
 extern "C" {
 #endif
 
-/* v22: deva_b200_jpeg_bound, deva_b200_jpeg_workspace_bytes and deva_b200_jpeg_encode (result JPEGs encoded on the
+/* v23: deva_b200_rle_bound, deva_b200_rle_workspace_bytes and deva_b200_rle_encode (BURST's per-segment COCO RLE encoded
+ * on the device).
+ * v22: deva_b200_jpeg_bound, deva_b200_jpeg_workspace_bytes and deva_b200_jpeg_encode (result JPEGs encoded on the
  * device).
  * v21: deva_b200_png_bound, deva_b200_png_workspace_bytes and deva_b200_png_encode (result PNGs encoded on the device).
  * v20: dropped deva_b200_up2_add and deva_b200_cbam (single-fp16 residual stream); deva_b200_up2_add_split requires skip_lo
@@ -42,7 +44,7 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 22
+#define DEVA_B200_ABI_VERSION 23
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -428,6 +430,19 @@ DEVA_B200_API size_t deva_b200_jpeg_bound(int h, int w);
 DEVA_B200_API size_t deva_b200_jpeg_workspace_bytes(int h, int w);
 DEVA_B200_API int deva_b200_jpeg_encode(const uint8_t* img, int h, int w, const uint8_t* quality_tables, void* workspace,
                                         uint8_t* out, int64_t* out_len, deva_stream_t stream);
+
+/* ---- COCO compressed RLE (deva/utils/rle_encode.py; the format is DESIGN §7) --------------------------------------
+ * ids i64 [h, w] row-major, 1 <= h, w and h * w < 2^31; seg_ids i64 [n], 1 <= n <= DEVA_B200_MAX_SEGMENT_CHANNELS, both
+ * on the device.  For every j < n, out[offsets[j] : offsets[j + 1]] is the counts string pycocotools' rleToString
+ * writes for the column-major RLE of the mask ids == seg_ids[j]; offsets: i64 [n + 1] on the device, offsets[0] = 0.  A
+ * repeated seg id gets the same string again; an id absent from the map gets the string of [h * w].  The bytes are a
+ * function of the inputs alone.  out: deva_b200_rle_bound(h, w, n) bytes = n * (h * w + 1), the longest string (a mask
+ * that changes at every pixel) for every entry; workspace: deva_b200_rle_workspace_bytes(h, w, n) bytes, 16-byte
+ * aligned.  Neither depends on the map's content. */
+DEVA_B200_API size_t deva_b200_rle_bound(int h, int w, int n);
+DEVA_B200_API size_t deva_b200_rle_workspace_bytes(int h, int w, int n);
+DEVA_B200_API int deva_b200_rle_encode(const int64_t* ids, int h, int w, const int64_t* seg_ids, int n, void* workspace,
+                                       uint8_t* out, int64_t* offsets, deva_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 22
+ABI_VERSION = 23
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -122,6 +122,9 @@ _SIGNATURES = {
     'deva_b200_jpeg_bound': (c_size_t, [c_int, c_int]),
     'deva_b200_jpeg_workspace_bytes': (c_size_t, [c_int, c_int]),
     'deva_b200_jpeg_encode': (c_int, [c_void_p, c_int, c_int, c_char_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'deva_b200_rle_bound': (c_size_t, [c_int, c_int, c_int]),
+    'deva_b200_rle_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
+    'deva_b200_rle_encode': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -543,6 +546,28 @@ def jpeg_encode(img, tables: bytes, workspace, out, out_len):
     assert workspace.numel() * workspace.element_size() >= jpeg_workspace_bytes(h, w)
     _check(lib().deva_b200_jpeg_encode(_ptr(img), h, w, bytes(tables), _ptr(workspace), _ptr(out), _ptr(out_len),
                                        _stream()), 'jpeg_encode')
+
+
+def rle_bound(h, w, n) -> int:
+    return int(lib().deva_b200_rle_bound(h, w, n))
+
+
+def rle_workspace_bytes(h, w, n) -> int:
+    return int(lib().deva_b200_rle_workspace_bytes(h, w, n))
+
+
+def rle_encode(ids, seg_ids, workspace, out, offsets):
+    """ids int64 [h, w]; seg_ids int64 [n]; out: rle_bound bytes; offsets int64 [n + 1]; workspace:
+    rle_workspace_bytes, 16-byte aligned (see include/deva_b200.h)."""
+    assert ids.dtype == torch.int64 and ids.is_cuda and ids.is_contiguous() and ids.dim() == 2, (ids.dtype, ids.shape)
+    assert seg_ids.dtype == torch.int64 and seg_ids.is_cuda and seg_ids.is_contiguous() and seg_ids.dim() == 1
+    h, w = ids.shape
+    n = seg_ids.numel()
+    assert offsets.dtype == torch.int64 and offsets.is_contiguous() and offsets.numel() == n + 1
+    assert out.numel() * out.element_size() >= rle_bound(h, w, n)
+    assert workspace.numel() * workspace.element_size() >= rle_workspace_bytes(h, w, n)
+    _check(lib().deva_b200_rle_encode(_ptr(ids), h, w, _ptr(seg_ids), n, _ptr(workspace), _ptr(out), _ptr(offsets),
+                                      _stream()), 'rle_encode')
 
 
 def transpose_append(src, dst, ld_dst, n, c):

@@ -5,8 +5,9 @@ work runs on the device.
 overlay, per-channel areas and boxes in one kernel - starts the device-to-host copies into a ring of pinned buffers,
 records an event and queues the frame; it never synchronises the host.  The writer thread waits on the event and does
 only what has to stay on the host: PIL images and PNG / JPEG encoding, the JSON entries, the gradio writer, and the two
-paths that need third-party code - ``supervision`` boxes and labels for prompts, and ``pycocotools`` RLE for burst (the
-one per-object host loop left; a device RLE would remove it).  Both libraries are imported only when those paths run.
+paths that need third-party code - ``supervision`` boxes and labels for prompts, and ``pycocotools`` RLE for burst (a
+full-frame compare and encode per segment, from the downloaded id map).  Both libraries are imported only when those
+paths run.
 
 With ``png_encoder='device'`` (or ``DEVA_B200_PNG_ENCODER=device``) the id image is encoded as a PNG on the device too
 (deva/utils/png_encode.py), right after ``prob_to_segments`` on the same stream: only the compressed stream comes to the
@@ -16,6 +17,11 @@ With ``jpeg_encoder='device'`` (or ``DEVA_B200_JPEG_ENCODER=device``) the demo o
 (deva/utils/jpeg_encode.py), byte for byte Pillow's file.  An overlay blended on the device is encoded right after
 ``prob_to_segments`` and only its scan comes to the host; an image finished on the host (prompt boxes and labels, or
 the host blend) is encoded by the writer thread.  The gradio writer is unchanged.
+
+With ``rle_encoder='device'`` (or ``DEVA_B200_RLE_ENCODER=device``) burst's per-segment COCO RLE is encoded on the
+device (deva/utils/rle_encode.py), string for string pycocotools': every segment's string comes from one pass over the
+id map right after ``prob_to_segments``, and only the strings come to the host, not the id map.  The writer builds the
+same JSON entries from them, with no per-segment pixel work and no pycocotools.
 """
 import copy
 import os
@@ -33,6 +39,8 @@ from deva.inference.frame_io import prob_to_ids, prob_to_segments
 from deva.utils.jpeg_encode import PREFIX as JPEG_PREFIX, PendingJpeg, encode_jpeg, encode_jpeg_async, write_jpeg
 from deva.utils.jpeg_encode import resolve_encoder as resolve_jpeg_encoder
 from deva.utils.png_encode import PREFIX as PNG_PREFIX, PendingPng, encode_png_async, resolve_encoder, write_png
+from deva.utils.rle_encode import MAX_SEGMENT_CHANNELS, PendingRle, encode_rle_async, host_bytes as rle_host_bytes
+from deva.utils.rle_encode import resolve_encoder as resolve_rle_encoder
 
 QUEUE_SIZE = 10
 RING_SIZE = QUEUE_SIZE + 2  # the queued frames, the one the writer holds and the one save_mask is filling
@@ -40,12 +48,16 @@ RING_SIZE = QUEUE_SIZE + 2  # the queued frames, the one the writer holds and th
 
 class ResultSaver:
     def __init__(self, output_root: str, video_name: str, *, dataset: str, object_manager, palette=None,
-                 png_encoder: Optional[str] = None, jpeg_encoder: Optional[str] = None):
+                 png_encoder: Optional[str] = None, jpeg_encoder: Optional[str] = None,
+                 rle_encoder: Optional[str] = None):
         """png_encoder: 'pil' (Pillow on the writer thread) or 'device'; None reads DEVA_B200_PNG_ENCODER (default
-        'pil').  jpeg_encoder: the same for the overlay JPEG; None reads DEVA_B200_JPEG_ENCODER (default 'pil')."""
+        'pil').  jpeg_encoder: the same for the overlay JPEG; None reads DEVA_B200_JPEG_ENCODER (default 'pil').
+        rle_encoder: 'pycocotools' (on the writer thread) or 'device' for burst's RLE; None reads DEVA_B200_RLE_ENCODER
+        (default 'pycocotools')."""
         self.output_root = output_root
         self.png_encoder = resolve_encoder(png_encoder)
         self.jpeg_encoder = resolve_jpeg_encoder(jpeg_encoder)
+        self.rle_encoder = resolve_rle_encoder(rle_encoder)
         self.video_name = video_name
         self.dataset = dataset.lower()
         self.palette = palette
@@ -144,12 +156,18 @@ class ResultSaver:
             if t is not None:
                 host[name] = _pinned(slot, name, t.shape, t.dtype)
                 host[name].copy_(t, non_blocking=True)
+        segments_info = copy.deepcopy(self.object_manager.get_current_segments_info())
+        rle = None
         if self.json_style == 'burst' or (overlay and not on_device):
             # the full id map: burst's per-segment RLE and the host blend need ids, not colours
             lut = torch.tensor(seg.lut, dtype=torch.int32).pin_memory().to(prob.device, non_blocking=True)
             ids = prob_to_ids(prob, size=size, lut=lut)
-            host['ids'] = _pinned(slot, 'ids', ids.shape, ids.dtype)
-            host['ids'].copy_(ids, non_blocking=True)
+            if self.json_style == 'burst' and self.rle_encoder == 'device':
+                rle = encode_rle_async(ids, [s['id'] for s in segments_info],
+                                       host=_pinned(slot, 'rle', (rle_host_bytes(MAX_SEGMENT_CHANNELS), ), torch.uint8))
+            if rle is None or (overlay and not on_device):  # encoded RLE strings replace the id map's download
+                host['ids'] = _pinned(slot, 'ids', ids.shape, ids.dtype)
+                host['ids'].copy_(ids, non_blocking=True)
         done = torch.cuda.Event()
         done.record()
 
@@ -166,9 +184,10 @@ class ResultSaver:
             prompts=prompts,
             path_to_image=path_to_image,
             all_obj_ids=[int(o.id) for o in self.object_manager.obj_to_tmp_id],
-            segments_info=copy.deepcopy(self.object_manager.get_current_segments_info()),
+            segments_info=segments_info,
             png=png,
             jpeg=jpeg,
+            rle=rle,
         ))
 
     def end(self):
@@ -202,6 +221,7 @@ class ResultArgs:
     segments_info: List[Dict]
     png: Optional[PendingPng] = None  # the id image's PNG, encoded on the device
     jpeg: Optional[PendingJpeg] = None  # the overlay's JPEG, encoded on the device
+    rle: Optional[PendingRle] = None  # burst's RLE of every entry of segments_info, encoded on the device
 
 
 def save_result(queue: Queue):
@@ -235,14 +255,19 @@ def _write(args: ResultArgs):
         segments_info = [s for s in segments_info if s['area'] > 0]
         saver.all_annotations.append({'file_name': frame_name[:-4] + '.jpg', 'segments_info': segments_info})
     elif saver.json_style == 'burst':
-        import pycocotools.mask as mask_util
-        ids = host['ids'].numpy()
-        for seg in segments_info:
-            m = ids == seg['id']
-            seg['area'] = area.get(seg['id'], 0)
-            coco_mask = mask_util.encode(np.asfortranarray(m))
-            coco_mask['counts'] = coco_mask['counts'].decode('utf-8')
-            seg['rle_mask'] = coco_mask
+        if args.rle is not None:
+            for seg, rle in zip(segments_info, args.rle.result()):
+                seg['area'] = area.get(seg['id'], 0)
+                seg['rle_mask'] = rle
+        else:
+            import pycocotools.mask as mask_util
+            ids = host['ids'].numpy()
+            for seg in segments_info:
+                m = ids == seg['id']
+                seg['area'] = area.get(seg['id'], 0)
+                coco_mask = mask_util.encode(np.asfortranarray(m))
+                coco_mask['counts'] = coco_mask['counts'].decode('utf-8')
+                seg['rle_mask'] = coco_mask
         segments_info = [s for s in segments_info if s['area'] > 0]
         saver.all_annotations.append({
             'file_name': frame_name[:-4] + '.jpg',
