@@ -14,6 +14,7 @@
 #include <stdint.h>
 
 #include "common.h"
+#include "scan.cuh"
 
 namespace b200 {
 namespace jpeg {
@@ -258,51 +259,19 @@ __global__ void __launch_bounds__(32 * kWarps) huffman_kernel(const int16_t* __r
 }
 
 // ---- 3, 5. scans --------------------------------------------------------------------------------------------------------
-// Exclusive scan of one value per thread over the block; returns the value's offset and sets *chunk to the block total.
-__device__ __forceinline__ unsigned long long block_exclusive_scan(unsigned long long v, unsigned long long* warp_sums,
-                                                                   unsigned long long* chunk) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
-  unsigned long long x = v;
-  for (int m = 1; m < 32; m <<= 1) {
-    const unsigned long long t = __shfl_up_sync(kFull, x, m);
-    if (lane >= m) x += t;
-  }
-  if (lane == 31) warp_sums[warp] = x;
-  __syncthreads();
-  unsigned long long before = 0, all = 0;
-  for (int k = 0; k < warps; ++k) {
-    if (k < warp) before += warp_sums[k];
-    all += warp_sums[k];
-  }
-  __syncthreads();  // warp_sums is rewritten by the next call
-  *chunk = all;
-  return before + x - v;
-}
-
 // Exclusive scan of n counts into off, kScanItems consecutive counts per thread; returns the total on every thread.
 __device__ unsigned long long scan_counts(const uint32_t* __restrict__ counts, long long n,
                                           unsigned long long* __restrict__ off) {
   __shared__ unsigned long long warp_sums[kScanThreads / 32];
-  unsigned long long carry = 0;
-  for (long long base = 0; base < n; base += (long long)kScanThreads * kScanItems) {
-    const long long i0 = base + (long long)threadIdx.x * kScanItems;
-    uint32_t v[kScanItems];
-    unsigned long long sum = 0;
-#pragma unroll
-    for (int k = 0; k < kScanItems; ++k) {
-      v[k] = i0 + k < n ? counts[i0 + k] : 0;
-      sum += v[k];
-    }
-    unsigned long long chunk;
-    unsigned long long o = carry + block_exclusive_scan(sum, warp_sums, &chunk);
-#pragma unroll
-    for (int k = 0; k < kScanItems; ++k) {
-      if (i0 + k < n) off[i0 + k] = o;
-      o += v[k];
-    }
-    carry += chunk;
-  }
-  return carry;
+  return block_scan<kScanItems>(
+      n, 0ull, warp_sums, [&](long long i) { return counts[i]; },
+      [&](long long i, unsigned long long o, uint32_t) { off[i] = o; });
+}
+
+// The 0xFF bytes among the 16 of q
+__device__ __forceinline__ int count_ff(const uint4& q) {
+  return (__popc(__vcmpeq4(q.x, kFull)) + __popc(__vcmpeq4(q.y, kFull)) + __popc(__vcmpeq4(q.z, kFull)) +
+          __popc(__vcmpeq4(q.w, kFull))) >> 3;
 }
 
 // meta[0]: bytes of the scan before stuffing; the fill's 1-bits are ORed into its last byte.
@@ -326,10 +295,8 @@ __global__ void __launch_bounds__(kSegThreads) count_ff_kernel(const uint4* __re
   const unsigned long long n = meta[0];
   if ((unsigned long long)blockIdx.x * kSegBytes >= n) return;  // past the scan: whole blocks leave
   const uint4 q = bytes[(long long)blockIdx.x * kSegThreads + threadIdx.x];  // bytes past n are zero
-  const int ff = (__popc(__vcmpeq4(q.x, kFull)) + __popc(__vcmpeq4(q.y, kFull)) + __popc(__vcmpeq4(q.z, kFull)) +
-                  __popc(__vcmpeq4(q.w, kFull))) >> 3;
   unsigned long long total;
-  block_exclusive_scan(ff, warp_sums, &total);
+  block_exclusive_scan<unsigned long long>(count_ff(q), warp_sums, total);
   if (threadIdx.x == 0) seg_ff[blockIdx.x] = (uint32_t)total;
 }
 
@@ -354,10 +321,8 @@ __global__ void __launch_bounds__(kSegThreads) stuff_kernel(const uint4* __restr
   const unsigned long long n = meta[0];
   if ((unsigned long long)blockIdx.x * kSegBytes >= n) return;
   const uint4 q = bytes[(long long)blockIdx.x * kSegThreads + threadIdx.x];
-  const int ff = (__popc(__vcmpeq4(q.x, kFull)) + __popc(__vcmpeq4(q.y, kFull)) + __popc(__vcmpeq4(q.z, kFull)) +
-                  __popc(__vcmpeq4(q.w, kFull))) >> 3;
   unsigned long long total;
-  const unsigned long long before = block_exclusive_scan(ff, warp_sums, &total);
+  const unsigned long long before = block_exclusive_scan<unsigned long long>(count_ff(q), warp_sums, total);
   const unsigned long long p0 = (unsigned long long)blockIdx.x * kSegBytes + threadIdx.x * 16;
   uint8_t* dst = out + p0 + seg_off[blockIdx.x] + before;
   const uint32_t word[4] = {q.x, q.y, q.z, q.w};
@@ -373,33 +338,30 @@ __global__ void __launch_bounds__(kSegThreads) stuff_kernel(const uint4* __restr
 // ---- sizes --------------------------------------------------------------------------------------------------------------
 inline long long blocks_of(int h, int w) { return 6LL * ((h + 15) / 16) * ((w + 15) / 16); }
 inline long long segments_of(int h, int w) { return (blocks_of(h, w) * kMaxBlockBytes + 1 + kSegBytes - 1) / kSegBytes; }
-inline size_t align16(size_t n) { return (n + 15) / 16 * 16; }
-
-struct Workspace {
-  int16_t* coef;
-  uint32_t* block_bits;
-  unsigned long long* block_off;
-  uint32_t* seg_ff;
-  unsigned long long* seg_off;
-  unsigned long long* meta;
-  uint32_t* words;  // the scan before stuffing, segments * kSegBytes bytes
-  size_t bytes;
+// Workspace regions, each 16-byte aligned.
+struct Work {
+  int16_t* coef;                  // [blocks * 64]
+  uint32_t* block_bits;           // [blocks]
+  unsigned long long* block_off;  // [blocks]
+  uint32_t* seg_ff;               // [segments]
+  unsigned long long* seg_off;    // [segments]
+  unsigned long long* meta;       // [1]
+  uint32_t* words;                // the scan before stuffing, segments * kSegBytes bytes
 };
 
-inline Workspace carve(void* base, int h, int w) {
+inline size_t carve(int h, int w, void* base, Work* wk) {
   const long long nb = blocks_of(h, w), ns = segments_of(h, w);
-  char* p = static_cast<char*>(base);
-  Workspace ws{};
-  size_t o = 0;
-  ws.coef = reinterpret_cast<int16_t*>(p + o), o += align16((size_t)nb * 64 * 2);
-  ws.block_bits = reinterpret_cast<uint32_t*>(p + o), o += align16((size_t)nb * 4);
-  ws.block_off = reinterpret_cast<unsigned long long*>(p + o), o += align16((size_t)nb * 8);
-  ws.seg_ff = reinterpret_cast<uint32_t*>(p + o), o += align16((size_t)ns * 4);
-  ws.seg_off = reinterpret_cast<unsigned long long*>(p + o), o += align16((size_t)ns * 8);
-  ws.meta = reinterpret_cast<unsigned long long*>(p + o), o += 16;
-  ws.words = reinterpret_cast<uint32_t*>(p + o), o += (size_t)ns * kSegBytes;
-  ws.bytes = o;
-  return ws;
+  Carver<16> c{static_cast<char*>(base)};
+  Work t;
+  t.coef = c.take<int16_t>(nb * 64);
+  t.block_bits = c.take<uint32_t>(nb);
+  t.block_off = c.take<unsigned long long>(nb);
+  t.seg_ff = c.take<uint32_t>(ns);
+  t.seg_off = c.take<unsigned long long>(ns);
+  t.meta = c.take<unsigned long long>(1);
+  t.words = c.take<uint32_t>(ns * (kSegBytes / 4));
+  if (wk) *wk = t;
+  return c.bytes;
 }
 
 }  // namespace jpeg
@@ -413,7 +375,7 @@ DEVA_B200_API size_t deva_b200_jpeg_bound(int h, int w) {
   return (size_t)(2 * (jpeg::blocks_of(h, w) * jpeg::kMaxBlockBytes + 1) + 2);
 }
 
-DEVA_B200_API size_t deva_b200_jpeg_workspace_bytes(int h, int w) { return jpeg::carve(nullptr, h, w).bytes; }
+DEVA_B200_API size_t deva_b200_jpeg_workspace_bytes(int h, int w) { return jpeg::carve(h, w, nullptr, nullptr); }
 
 DEVA_B200_API int deva_b200_jpeg_encode(const uint8_t* img, int h, int w, const uint8_t* quality_tables,
                                         void* workspace, uint8_t* out, int64_t* out_len, deva_stream_t stream) {
@@ -425,7 +387,8 @@ DEVA_B200_API int deva_b200_jpeg_encode(const uint8_t* img, int h, int w, const 
     B200_REQUIRE(quality_tables[i] >= 1, "jpeg_encode: quantisation table entry %d is 0", i);
     tables.q[i / 64][i % 64] = quality_tables[i];
   }
-  const jpeg::Workspace ws = jpeg::carve(workspace, h, w);
+  jpeg::Work ws;
+  jpeg::carve(h, w, workspace, &ws);
   const int mcu_cols = (w + 15) / 16, mcus = ((h + 15) / 16) * mcu_cols;
   const long long blocks = jpeg::blocks_of(h, w), segs = jpeg::segments_of(h, w);
   cudaStream_t s = S(stream);

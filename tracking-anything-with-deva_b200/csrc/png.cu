@@ -13,6 +13,7 @@
 #include <stdint.h>
 
 #include "common.h"
+#include "scan.cuh"
 
 namespace b200 {
 namespace png {
@@ -202,37 +203,21 @@ __global__ void __launch_bounds__(kScanThreads) frame_kernel(int h, int seg, con
                                                              uint32_t* __restrict__ out, int64_t* __restrict__ out_len) {
   __shared__ unsigned long long warp_sums[kScanThreads / 32];
   __shared__ unsigned long long s1_total, s2_total;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const long long n = (long long)h * seg;
   if (tid == 0) s1_total = s2_total = 0;
-  unsigned long long carry = kFirstRowBit, s1 = 0, s2 = 0;
-  for (int base = 0; base < h; base += kScanThreads) {
-    const int r = base + tid;
-    const unsigned long long v = r < h ? row_bits[r] : 0;
-    unsigned long long x = v;  // inclusive scan within the warp
-    for (int m = 1; m < 32; m <<= 1) {
-      const unsigned long long t = __shfl_up_sync(kFull, x, m);
-      if (lane >= m) x += t;
-    }
-    if (lane == 31) warp_sums[warp] = x;
-    __syncthreads();
-    unsigned long long before = 0, chunk = 0;
-    for (int k = 0; k < kScanThreads / 32; ++k) {
-      if (k < warp) before += warp_sums[k];
-      chunk += warp_sums[k];
-    }
-    if (r < h) {
-      const unsigned long long off = carry + before + x - v;
-      row_off[r] = off;
-      out[off >> 5] = 0;  // the row's first and last words, shared with the neighbouring rows
-      out[(off + v - 1) >> 5] = 0;
-      const long long after = n - (long long)r * seg - seg;  // bytes of s after the row
-      s1 += row_sum[r];
-      s2 += row_weighted[r] + (unsigned long long)(after % kAdlerMod) * (row_sum[r] % kAdlerMod) % kAdlerMod;
-    }
-    carry += chunk;
-    __syncthreads();  // warp_sums is rewritten by the next chunk
-  }
+  unsigned long long s1 = 0, s2 = 0;
+  // end_bit follows the last row; end-of-block is seven 0 bits
+  const unsigned long long end_bit = block_scan(
+      h, (unsigned long long)kFirstRowBit, warp_sums, [&](long long r) { return row_bits[r]; },
+      [&](long long r, unsigned long long off, uint32_t v) {
+        row_off[r] = off;
+        out[off >> 5] = 0;  // the row's first and last words, shared with the neighbouring rows
+        out[(off + v - 1) >> 5] = 0;
+        const long long after = n - r * seg - seg;  // bytes of s after the row
+        s1 += row_sum[r];
+        s2 += row_weighted[r] + (unsigned long long)(after % kAdlerMod) * (row_sum[r] % kAdlerMod) % kAdlerMod;
+      });
   atomicAdd(&s1_total, s1);
   atomicAdd(&s2_total, s2);
   __syncthreads();
@@ -241,7 +226,6 @@ __global__ void __launch_bounds__(kScanThreads) frame_kernel(int h, int seg, con
   const uint32_t a = (uint32_t)((1 + s1_total) % kAdlerMod);
   const uint32_t b = (uint32_t)((n % kAdlerMod + s2_total) % kAdlerMod);
   out[0] |= 0x78u | (0x01u << 8) | (3u << 16);  // zlib CMF, FLG; then BFINAL = 1, BTYPE = 01
-  const unsigned long long end_bit = carry;  // after the last row; end-of-block is seven 0 bits
   const long long body = (long long)((end_bit + 7 + 7) >> 3);
   uint8_t* bytes = reinterpret_cast<uint8_t*>(out);
   for (long long k = (long long)((end_bit + 7) >> 3); k < body; ++k) bytes[k] = 0;
@@ -252,6 +236,21 @@ __global__ void __launch_bounds__(kScanThreads) frame_kernel(int h, int seg, con
 
 inline long long stream_bytes(int h, int w, int channels, int bits) {
   return (long long)h * (((long long)w * channels * bits + 7) / 8 + 1);
+}
+
+// Workspace regions, each 8-byte aligned.
+struct Work {
+  uint32_t* row_stats;          // [3 * h] row_bits, row_sum, row_weighted
+  unsigned long long* row_off;  // [h]
+};
+
+inline size_t carve(int h, void* base, Work* wk) {
+  Carver<8> c{static_cast<char*>(base)};
+  Work t;
+  t.row_stats = c.take<uint32_t>(3ll * h);
+  t.row_off = c.take<unsigned long long>(h);
+  if (wk) *wk = t;
+  return c.bytes;
 }
 
 }  // namespace png
@@ -267,9 +266,7 @@ DEVA_B200_API size_t deva_b200_png_bound(int h, int w, int channels, int bits) {
   return (size_t)((bound + 3) / 4 * 4);
 }
 
-DEVA_B200_API size_t deva_b200_png_workspace_bytes(int h) {
-  return ((size_t)12 * h + 7) / 8 * 8 + (size_t)8 * h;
-}
+DEVA_B200_API size_t deva_b200_png_workspace_bytes(int h) { return png::carve(h, nullptr, nullptr); }
 
 DEVA_B200_API int deva_b200_png_encode(const uint8_t* img, int h, int w, int channels, int bits, void* workspace,
                                        uint8_t* out, int64_t* out_len, deva_stream_t stream) {
@@ -286,10 +283,12 @@ DEVA_B200_API int deva_b200_png_encode(const uint8_t* img, int h, int w, int cha
   const int warps = (int)std::max(1, std::min(png::kMaxWarps, 48 * 1024 / stride));
   const size_t smem = (size_t)warps * stride;
   png::Shape g{img, w, channels, bits, (int)seg, std::max(1, channels * bits / 8)};
-  uint32_t* row_bits = reinterpret_cast<uint32_t*>(workspace);
+  png::Work wk;
+  png::carve(h, workspace, &wk);
+  uint32_t* row_bits = wk.row_stats;
   uint32_t* row_sum = row_bits + h;
   uint32_t* row_weighted = row_sum + h;
-  auto* row_off = reinterpret_cast<unsigned long long*>(static_cast<char*>(workspace) + ((size_t)12 * h + 7) / 8 * 8);
+  unsigned long long* row_off = wk.row_off;
   uint32_t* words = reinterpret_cast<uint32_t*>(out);
   cudaStream_t s = S(stream);
   const unsigned blocks = (unsigned)ceil_div(h, warps);

@@ -16,6 +16,7 @@
 #include <stdint.h>
 
 #include "common.h"
+#include "scan.cuh"
 
 namespace b200 {
 namespace rle {
@@ -41,8 +42,6 @@ inline Plan plan(int h, int w, int n) {
   return p;
 }
 
-inline size_t align16(size_t b) { return (b + 15) / 16 * 16; }
-
 // Workspace regions, each 16-byte aligned.
 struct Work {
   int* canon;           // [n] first entry with the same id
@@ -56,25 +55,20 @@ struct Work {
   int* bounds;          // [2 * pixels] boundary positions, grouped by slot, increasing within a slot
 };
 
-inline size_t carve(const Plan& p, int n, char* base, Work* w) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    char* at = base ? base + off : nullptr;
-    off += align16(bytes);
-    return at;
-  };
+inline size_t carve(const Plan& p, int n, void* base, Work* w) {
+  Carver<16> c{static_cast<char*>(base)};
   Work t;
-  t.canon = reinterpret_cast<int*>(take((size_t)n * 4));
-  t.entry_slot = reinterpret_cast<int*>(take((size_t)n * 4));
-  t.uniq = reinterpret_cast<long long*>(take((size_t)n * 8));
-  t.n_slots = reinterpret_cast<int*>(take(4));
-  t.chunk_count = reinterpret_cast<int*>(take((size_t)n * p.chunks * 4));
-  t.slot_count = reinterpret_cast<int*>(take((size_t)n * 4));
-  t.slot_start = reinterpret_cast<long long*>(take((size_t)n * 8));
-  t.slot_len = reinterpret_cast<long long*>(take((size_t)n * 8));
-  t.bounds = reinterpret_cast<int*>(take((size_t)p.pixels * 2 * 4));
+  t.canon = c.take<int>(n);
+  t.entry_slot = c.take<int>(n);
+  t.uniq = c.take<long long>(n);
+  t.n_slots = c.take<int>(1);
+  t.chunk_count = c.take<int>((long long)n * p.chunks);
+  t.slot_count = c.take<int>(n);
+  t.slot_start = c.take<long long>(n);
+  t.slot_len = c.take<long long>(n);
+  t.bounds = c.take<int>(p.pixels * 2);
   if (w) *w = t;
-  return off;
+  return c.bytes;
 }
 
 // ---- 1. distinct ids -----------------------------------------------------------------------------------------------
@@ -183,56 +177,23 @@ __global__ void __launch_bounds__(32 * kWarps) boundary_kernel(const int64_t* __
 }
 
 // ---- 3, 5. scans ---------------------------------------------------------------------------------------------------
-// Exclusive scan of v over the block (blockDim.x a multiple of 32, at most 1024); total: the block's sum.
-__device__ __forceinline__ long long block_exclusive_scan(long long v, long long* warp_sums, long long& total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
-  long long x = v;
-  for (int m = 1; m < 32; m <<= 1) {
-    const long long t = __shfl_up_sync(kFull, x, m);
-    if (lane >= m) x += t;
-  }
-  if (lane == 31) warp_sums[warp] = x;
-  __syncthreads();
-  long long before = 0;
-  total = 0;
-  for (int k = 0; k < warps; ++k) {
-    if (k < warp) before += warp_sums[k];
-    total += warp_sums[k];
-  }
-  __syncthreads();  // warp_sums is rewritten by the next call
-  return before + x - v;
-}
-
 // One block per slot: its chunks' counts -> the chunks' first index within the slot; the slot's total.
 __global__ void __launch_bounds__(kScanThreads) scan_chunks_kernel(Plan p, Work wk) {
   __shared__ long long warp_sums[kScanThreads / 32];
   const int s = blockIdx.x;
   if (s >= *wk.n_slots) return;
   int* row = wk.chunk_count + (size_t)s * p.chunks;
-  long long carry = 0;
-  for (int base = 0; base < p.chunks; base += kScanThreads) {
-    const int k = base + threadIdx.x;
-    const long long v = k < p.chunks ? row[k] : 0;
-    long long total;
-    const long long before = block_exclusive_scan(v, warp_sums, total);
-    if (k < p.chunks) row[k] = (int)(carry + before);
-    carry += total;
-  }
-  if (threadIdx.x == 0) wk.slot_count[s] = (int)carry;
+  const long long total = block_scan(
+      p.chunks, 0ll, warp_sums, [&](long long k) { return row[k]; },
+      [&](long long k, long long o, int) { row[k] = (int)o; });
+  if (threadIdx.x == 0) wk.slot_count[s] = (int)total;
 }
 
 __global__ void __launch_bounds__(kScanThreads) scan_slots_kernel(Work wk) {
   __shared__ long long warp_sums[kScanThreads / 32];
-  const int n_slots = *wk.n_slots;
-  long long carry = 0;
-  for (int base = 0; base < n_slots; base += kScanThreads) {
-    const int s = base + threadIdx.x;
-    const long long v = s < n_slots ? wk.slot_count[s] : 0;
-    long long total;
-    const long long before = block_exclusive_scan(v, warp_sums, total);
-    if (s < n_slots) wk.slot_start[s] = carry + before;
-    carry += total;
-  }
+  block_scan(
+      *wk.n_slots, 0ll, warp_sums, [&](long long s) { return wk.slot_count[s]; },
+      [&](long long s, long long o, int) { wk.slot_start[s] = o; });
 }
 
 // ---- 5. strings ----------------------------------------------------------------------------------------------------
@@ -286,16 +247,10 @@ __global__ void __launch_bounds__(kThreads) length_kernel(long long pixels, Work
 
 __global__ void __launch_bounds__(kScanThreads) offsets_kernel(int n, Work wk, int64_t* __restrict__ offsets) {
   __shared__ long long warp_sums[kScanThreads / 32];
-  long long carry = 0;
-  for (int base = 0; base < n; base += kScanThreads) {
-    const int j = base + threadIdx.x;
-    const long long v = j < n ? wk.slot_len[wk.entry_slot[j]] : 0;
-    long long total;
-    const long long before = block_exclusive_scan(v, warp_sums, total);
-    if (j < n) offsets[j] = carry + before;
-    carry += total;
-  }
-  if (threadIdx.x == 0) offsets[n] = carry;
+  const long long total = block_scan(
+      n, 0ll, warp_sums, [&](long long j) { return wk.slot_len[wk.entry_slot[j]]; },
+      [&](long long j, long long o, long long) { offsets[j] = o; });
+  if (threadIdx.x == 0) offsets[n] = total;
 }
 
 // One block per entry: its slot's string at offsets[j].
@@ -307,20 +262,14 @@ __global__ void __launch_bounds__(kThreads) write_kernel(long long pixels, Work 
   const int k = wk.slot_count[s];
   const int* b = wk.bounds + wk.slot_start[s];
   const long long end = offsets[j + 1];
-  long long at = offsets[j];
-  for (long long base = 0; base <= k; base += kThreads) {
-    const long long i = base + threadIdx.x;
-    long long x = 0;
-    int len = 0;
-    if (i <= k) {
-      x = coded(b, k, pixels, i);
-      len = chars(x);
-    }
-    long long total;
-    const long long before = block_exclusive_scan(len, warp_sums, total);
-    if (i <= k) emit(x, out, at + before, end);
-    at += total;
-  }
+  long long x = 0;  // the coded value the thread loaded last, written once its offset is known
+  block_scan(
+      k + 1ll, (long long)offsets[j], warp_sums,
+      [&](long long i) {
+        x = coded(b, k, pixels, i);
+        return chars(x);
+      },
+      [&](long long, long long at, int) { emit(x, out, at, end); });
 }
 
 }  // namespace rle
@@ -355,7 +304,7 @@ DEVA_B200_API int deva_b200_rle_encode(const int64_t* ids, int h, int w, const i
                "rle_encode: ids, seg_ids and offsets must be 8-byte and workspace 16-byte aligned");
   const rle::Plan p = rle::plan(h, w, n);
   rle::Work wk;
-  rle::carve(p, n, static_cast<char*>(workspace), &wk);
+  rle::carve(p, n, workspace, &wk);
   cudaStream_t s = S(stream);
   const unsigned entry_blocks = (unsigned)ceil_div(n, rle::kThreads);
   rle::canon_kernel<<<entry_blocks, rle::kThreads, 0, s>>>(seg_ids, n, wk.canon);

@@ -32,7 +32,8 @@ import numpy as np
 import torch
 from PIL import Image
 
-from deva.utils.png_encode import encode_png_async, resolve_encoder, write_png
+from deva.utils.device_download import write
+from deva.utils.png_encode import encode_png_async, resolve_encoder
 from deva.utils.png_pipeline import Decoder, Uploader
 
 CAPACITY = 1024  # label table entries per frame; a frame with more distinct labels is counted again with a larger table
@@ -142,7 +143,7 @@ def _limit_video(decoder, upload, video_path, out_dir, max_num_objects, palette,
     os.makedirs(out_dir, exist_ok=True)
     if png_encoder == 'device':
         pngs = [encode_png_async(m, 'P', palette) for m in maps]
-        writes = [decoder.pool.submit(write_png, p, path.join(out_dir, name)) for p, name in zip(pngs, frames)]
+        writes = [decoder.pool.submit(write, p, path.join(out_dir, name)) for p, name in zip(pngs, frames)]
     else:
         host = torch.empty(out.numel(), dtype=torch.uint8, pin_memory=True)
         host.copy_(out, non_blocking=True)

@@ -36,10 +36,11 @@ import torch
 from PIL import Image
 
 from deva.inference.frame_io import prob_to_ids, prob_to_segments
-from deva.utils.jpeg_encode import PREFIX as JPEG_PREFIX, PendingJpeg, encode_jpeg, encode_jpeg_async, write_jpeg
+from deva.utils.device_download import Pending, write
+from deva.utils.jpeg_encode import encode_jpeg_async, host_bytes as jpeg_host_bytes
 from deva.utils.jpeg_encode import resolve_encoder as resolve_jpeg_encoder
-from deva.utils.png_encode import PREFIX as PNG_PREFIX, PendingPng, encode_png_async, resolve_encoder, write_png
-from deva.utils.rle_encode import MAX_SEGMENT_CHANNELS, PendingRle, encode_rle_async, host_bytes as rle_host_bytes
+from deva.utils.png_encode import encode_png_async, host_bytes as png_host_bytes, resolve_encoder
+from deva.utils.rle_encode import MAX_SEGMENT_CHANNELS, encode_rle_async, host_bytes as rle_host_bytes
 from deva.utils.rle_encode import resolve_encoder as resolve_rle_encoder
 
 QUEUE_SIZE = 10
@@ -141,10 +142,10 @@ class ResultSaver:
         if save_the_mask and self.png_encoder == 'device' and self.dataset != 'gradio':
             png = encode_png_async(seg.rgb if long_id else seg.index,
                                    'RGB' if long_id else 'L' if self.palette is None else 'P', self.palette,
-                                   host=_pinned(slot, 'png', (8 + PNG_PREFIX, ), torch.uint8))
+                                   host=_pinned(slot, 'png', (png_host_bytes(), ), torch.uint8))
         jpeg = None
         if overlay and on_device and prompts is None and self.jpeg_encoder == 'device' and self.dataset != 'gradio':
-            jpeg = encode_jpeg_async(seg.overlay, host=_pinned(slot, 'jpeg', (8 + JPEG_PREFIX, ), torch.uint8))
+            jpeg = encode_jpeg_async(seg.overlay, host=_pinned(slot, 'jpeg', (jpeg_host_bytes(), ), torch.uint8))
         host = {}
         for name in ('index', 'rgb', 'overlay', 'counts', 'boxes'):
             t = getattr(seg, name)
@@ -219,9 +220,9 @@ class ResultArgs:
     path_to_image: str
     all_obj_ids: List[int]
     segments_info: List[Dict]
-    png: Optional[PendingPng] = None  # the id image's PNG, encoded on the device
-    jpeg: Optional[PendingJpeg] = None  # the overlay's JPEG, encoded on the device
-    rle: Optional[PendingRle] = None  # burst's RLE of every entry of segments_info, encoded on the device
+    png: Optional[Pending] = None  # the id image's PNG, encoded on the device
+    jpeg: Optional[Pending] = None  # the overlay's JPEG, encoded on the device
+    rle: Optional[Pending] = None  # burst's RLE of every entry of segments_info, encoded on the device
 
 
 def save_result(queue: Queue):
@@ -281,7 +282,7 @@ def _write(args: ResultArgs):
     if not args.save_the_mask:
         return
     if args.png is not None:
-        write_png(args.png, _path(saver, saver.output_postfix, frame_name[:-4] + '.png'))
+        write(args.png, _path(saver, saver.output_postfix, frame_name[:-4] + '.png'))
     else:
         if args.long_id:
             out_img = Image.fromarray(host['rgb'].numpy())
@@ -295,7 +296,7 @@ def _write(args: ResultArgs):
     if not (saver.visualize and args.long_id):
         return
     if args.jpeg is not None:
-        write_jpeg(args.jpeg, _path(saver, saver.visualize_postfix, frame_name[:-4] + '.jpg'))
+        write(args.jpeg, _path(saver, saver.visualize_postfix, frame_name[:-4] + '.jpg'))
         return
     if 'overlay' in host:
         blend = host['overlay'].numpy()
@@ -319,9 +320,7 @@ def _write(args: ResultArgs):
     if saver.dataset == 'gradio':
         saver.writer.write(blend[:, :, ::-1])
     elif saver.jpeg_encoder == 'device':  # an image finished on the host
-        data = encode_jpeg(blend)
-        with open(_path(saver, saver.visualize_postfix, frame_name[:-4] + '.jpg'), 'wb') as f:
-            f.write(data)
+        write(encode_jpeg_async(blend), _path(saver, saver.visualize_postfix, frame_name[:-4] + '.jpg'))
     else:
         _save(Image.fromarray(blend), saver, saver.visualize_postfix, frame_name[:-4] + '.jpg')
 

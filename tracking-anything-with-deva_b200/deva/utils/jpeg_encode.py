@@ -13,17 +13,18 @@ libjpeg(-turbo), because every step is libjpeg's integer arithmetic (oracle/jpeg
   * markers SOI, APP0 (JFIF 1.01, no units, density 1x1), DQT 0, DQT 1, SOF0, DHT DC0 AC0 DC1 AC1, SOS, scan, EOI.
 
 The device writes the scan, EOI and its length; the marker segments are built here.  ``encode_jpeg_async`` enqueues
-the encode and a copy of the scan's first ``PREFIX`` bytes on the current stream without synchronising, and
-``PendingJpeg.result()`` waits for them (and fetches the rest of a longer scan).  Importing this module does not
-initialise CUDA.
+the encode and a copy of the scan's first ``PREFIX`` bytes on the current stream without synchronising, and the
+returned ``Pending``'s ``result()`` waits for them (and fetches the rest of a longer scan;
+deva/utils/device_download.py).  Importing this module does not initialise CUDA.
 """
 import functools
-import os
 import struct
 from typing import Optional
 
 import numpy as np
 import torch
+
+from deva.utils import device_download
 
 ENCODERS = ('pil', 'device')
 ENV = 'DEVA_B200_JPEG_ENCODER'
@@ -56,10 +57,7 @@ _DHT = (
 
 def resolve_encoder(jpeg_encoder: Optional[str] = None) -> str:
     """``jpeg_encoder``, or the environment's ``DEVA_B200_JPEG_ENCODER`` when it is None ('pil' when that is unset)."""
-    value = os.environ.get(ENV, 'pil') if jpeg_encoder is None else jpeg_encoder
-    if value not in ENCODERS:
-        raise ValueError(f'jpeg_encoder must be one of {ENCODERS}, not {value!r}')
-    return value
+    return device_download.resolve(jpeg_encoder, 'jpeg_encoder', ENV, ENCODERS, 'pil')
 
 
 @functools.lru_cache(maxsize=128)
@@ -87,20 +85,9 @@ def headers(h: int, w: int, quality: int = 75) -> bytes:
     return out + _segment(0xda, bytes([3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0]))
 
 
-class PendingJpeg:
-    """An encode enqueued by ``encode_jpeg_async``; ``result()`` -> the JPEG file's bytes."""
-
-    def __init__(self, head: bytes, dev: torch.Tensor, host: torch.Tensor, prefix: int, done: torch.cuda.Event):
-        self.head, self.dev, self.host, self.prefix, self.done = head, dev, host, prefix, done
-
-    def result(self) -> bytes:
-        self.done.synchronize()
-        n = int(self.host[:8].view(torch.int64)[0])
-        scan = self.host[8:8 + min(n, self.prefix)].numpy().tobytes()
-        if n > self.prefix:
-            scan += self.dev[8 + self.prefix:8 + n].cpu().numpy().tobytes()
-        self.dev = None  # the device buffer is free once the scan is on the host
-        return self.head + scan
+def host_bytes() -> int:
+    """Bytes of the pinned buffer ``encode_jpeg_async`` needs: the scan's length and its first ``PREFIX`` bytes."""
+    return 8 + PREFIX
 
 
 def _as_device_image(img):
@@ -108,7 +95,7 @@ def _as_device_image(img):
         if not (img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3):
             raise ValueError(f'a JPEG image is uint8 RGB [h, w, 3], not {img.dtype} {img.shape}')
         _check_sides(img.shape)
-        return torch.from_numpy(np.ascontiguousarray(img)).pin_memory().cuda(non_blocking=True)
+        return device_download.upload(img)
     if not (isinstance(img, torch.Tensor) and img.is_cuda and img.dtype == torch.uint8 and img.dim() == 3 and
             img.shape[2] == 3):
         desc = f'{img.dtype} {tuple(img.shape)} on {img.device}' if isinstance(img, torch.Tensor) else type(img)
@@ -122,36 +109,22 @@ def _check_sides(shape):
         raise ValueError(f'a JPEG image has sides in [1, {MAX_SIDE}], not {shape[0]} x {shape[1]}')
 
 
-def encode_jpeg_async(img, quality: int = 75, host: Optional[torch.Tensor] = None) -> PendingJpeg:
+def encode_jpeg_async(img, quality: int = 75, host: Optional[torch.Tensor] = None) -> device_download.Pending:
     """Enqueues the encode of uint8 RGB ``img`` [h, w, 3] (a CUDA tensor, or a numpy array that is uploaded) on the
-    current stream; never synchronises the host.  host: optional pinned uint8 buffer of at least 8 + PREFIX bytes that
-    receives the scan's length and first bytes (one is allocated otherwise); it must stay untouched until ``result()``
-    returns."""
+    current stream; never synchronises the host.  host: optional pinned uint8 buffer of at least ``host_bytes()`` bytes
+    that receives the scan's length and first bytes (one is allocated otherwise); it must stay untouched until
+    ``result()`` returns, which gives the JPEG file's bytes."""
     from deva import _native
     tables = quant_tables(quality)
     img = _as_device_image(img)
     h, w = img.shape[:2]
     bound = _native.jpeg_bound(h, w)
-    ws_at = (8 + bound + 15) // 16 * 16
-    dev = torch.empty(ws_at + _native.jpeg_workspace_bytes(h, w), dtype=torch.uint8, device=img.device)
-    _native.jpeg_encode(img, tables, dev[ws_at:], dev[8:8 + bound], dev[:8].view(torch.int64))  # [length | scan | ws]
-    prefix = min(PREFIX, bound)
-    if host is None:
-        host = torch.empty(8 + prefix, dtype=torch.uint8, pin_memory=True)
-    assert host.is_pinned() and host.dtype == torch.uint8 and host.numel() >= 8 + prefix
-    host[:8 + prefix].copy_(dev[:8 + prefix], non_blocking=True)
-    done = torch.cuda.Event()
-    done.record()
-    return PendingJpeg(headers(h, w, quality), dev, host, prefix, done)
+    dev, out, ws = device_download.buffer(8, bound, _native.jpeg_workspace_bytes(h, w), img.device)
+    _native.jpeg_encode(img, tables, ws, out, dev[:8].view(torch.int64))
+    head = headers(h, w, quality)
+    return device_download.enqueue(lambda _, scan: head + scan, dev, (0, 8), bound, PREFIX, host)
 
 
 def encode_jpeg(img, quality: int = 75) -> bytes:
     """The JPEG file of uint8 RGB ``img`` (see ``encode_jpeg_async``); waits for the device."""
     return encode_jpeg_async(img, quality).result()
-
-
-def write_jpeg(jpeg: PendingJpeg, file: str):
-    """Writes the file of an enqueued encode; waits for it."""
-    data = jpeg.result()
-    with open(file, 'wb') as f:
-        f.write(data)

@@ -21,17 +21,18 @@ Every literal takes at most 9 bits, which bounds the stream at ``ceil((3 + 9 len
 
 The device writes the zlib stream and its length; the chunks and their CRCs are built here around the downloaded
 stream.  ``encode_png_async`` enqueues the encode and a copy of the stream's first ``PREFIX`` bytes on the current
-stream without synchronising, and ``PendingPng.result()`` waits for them (and fetches the rest of a larger stream).
-Importing this module does not initialise CUDA.
+stream without synchronising, and the returned ``Pending``'s ``result()`` waits for them (and fetches the rest of a
+larger stream; deva/utils/device_download.py).  Importing this module does not initialise CUDA.
 """
 import functools
-import os
 import struct
 import zlib
 from typing import Optional
 
 import numpy as np
 import torch
+
+from deva.utils import device_download
 
 ENCODERS = ('pil', 'device')
 ENV = 'DEVA_B200_PNG_ENCODER'
@@ -42,10 +43,7 @@ _COLOUR_TYPE = {'L': 0, 'RGB': 2, 'P': 3}
 
 def resolve_encoder(png_encoder: Optional[str] = None) -> str:
     """``png_encoder``, or the environment's ``DEVA_B200_PNG_ENCODER`` when it is None ('pil' when that is unset)."""
-    value = os.environ.get(ENV, 'pil') if png_encoder is None else png_encoder
-    if value not in ENCODERS:
-        raise ValueError(f'png_encoder must be one of {ENCODERS}, not {value!r}')
-    return value
+    return device_download.resolve(png_encoder, 'png_encoder', ENV, ENCODERS, 'pil')
 
 
 @functools.lru_cache(maxsize=64)
@@ -74,25 +72,14 @@ def _chunk(kind: bytes, data: bytes) -> bytes:
     return struct.pack('>I', len(data)) + kind + data + struct.pack('>I', zlib.crc32(kind + data))
 
 
-class PendingPng:
-    """An encode enqueued by ``encode_png_async``; ``result()`` -> the PNG file's bytes."""
-
-    def __init__(self, head: bytes, dev: torch.Tensor, host: torch.Tensor, prefix: int, done: torch.cuda.Event):
-        self.head, self.dev, self.host, self.prefix, self.done = head, dev, host, prefix, done
-
-    def result(self) -> bytes:
-        self.done.synchronize()
-        n = int(self.host[:8].view(torch.int64)[0])
-        idat = self.host[8:8 + min(n, self.prefix)].numpy().tobytes()
-        if n > self.prefix:
-            idat += self.dev[8 + self.prefix:8 + n].cpu().numpy().tobytes()
-        self.dev = None  # the device buffer is free once the stream is on the host
-        return self.head + _chunk(b'IDAT', idat) + _chunk(b'IEND', b'')
+def host_bytes() -> int:
+    """Bytes of the pinned buffer ``encode_png_async`` needs: the stream's length and its first ``PREFIX`` bytes."""
+    return 8 + PREFIX
 
 
 def _as_device_image(img, mode):
     if isinstance(img, np.ndarray):
-        img = torch.from_numpy(np.ascontiguousarray(img)).cuda()
+        img = device_download.upload(img)
     want = 3 if mode == 'RGB' else 2
     if not (img.is_cuda and img.dtype == torch.uint8 and img.dim() == want and (mode != 'RGB' or img.shape[2] == 3)):
         raise ValueError(f'a {mode} image is a CUDA uint8 tensor [h, w{", 3" if mode == "RGB" else ""}], not '
@@ -100,40 +87,26 @@ def _as_device_image(img, mode):
     return img.contiguous()
 
 
-def encode_png_async(img, mode: str, palette=None, host: Optional[torch.Tensor] = None) -> PendingPng:
+def encode_png_async(img, mode: str, palette=None, host: Optional[torch.Tensor] = None) -> device_download.Pending:
     """Enqueues the encode of uint8 ``img`` ([h, w] for 'L' / 'P', [h, w, 3] for 'RGB'; a CUDA tensor, or a numpy
     array that is uploaded) on the current stream; never synchronises the host.  host: optional pinned uint8 buffer of
-    at least 8 + PREFIX bytes that receives the stream's length and first bytes (one is allocated otherwise); it must
-    stay untouched until ``result()`` returns."""
+    at least ``host_bytes()`` bytes that receives the stream's length and first bytes (one is allocated otherwise); it
+    must stay untouched until ``result()`` returns, which gives the PNG file's bytes."""
     from deva import _native
     bits, plte = pillow_png_layout(mode, palette)
     img = _as_device_image(img, mode)
     h, w = img.shape[:2]
     channels = 3 if mode == 'RGB' else 1
-    bound = (_native.png_bound(h, w, channels, bits) + 7) // 8 * 8
-    ws = _native.png_workspace_bytes(h)
-    dev = torch.empty(8 + bound + ws, dtype=torch.uint8, device=img.device)  # [length | stream | workspace]
-    _native.png_encode(img, bits, dev[8 + bound:], dev[8:8 + bound], dev[:8].view(torch.int64))
-    prefix = min(PREFIX, bound)
-    if host is None:
-        host = torch.empty(8 + prefix, dtype=torch.uint8, pin_memory=True)
-    assert host.is_pinned() and host.dtype == torch.uint8 and host.numel() >= 8 + prefix
-    host[:8 + prefix].copy_(dev[:8 + prefix], non_blocking=True)
-    done = torch.cuda.Event()
-    done.record()
+    bound = _native.png_bound(h, w, channels, bits)
+    dev, out, ws = device_download.buffer(8, bound, _native.png_workspace_bytes(h), img.device)
+    _native.png_encode(img, bits, ws, out, dev[:8].view(torch.int64))
     head = SIGNATURE + _chunk(b'IHDR', struct.pack('>IIBBBBB', w, h, bits, _COLOUR_TYPE[mode], 0, 0, 0))
     if plte is not None:
         head += _chunk(b'PLTE', plte)
-    return PendingPng(head, dev, host, prefix, done)
+    return device_download.enqueue(lambda _, idat: head + _chunk(b'IDAT', idat) + _chunk(b'IEND', b''), dev, (0, 8),
+                                   bound, PREFIX, host)
 
 
 def encode_png(img, mode: str, palette=None) -> bytes:
     """The PNG file of uint8 ``img`` (see ``encode_png_async``); waits for the device."""
     return encode_png_async(img, mode, palette).result()
-
-
-def write_png(png: PendingPng, file: str):
-    """Writes the file of an enqueued encode; waits for it."""
-    data = png.result()
-    with open(file, 'wb') as f:
-        f.write(data)

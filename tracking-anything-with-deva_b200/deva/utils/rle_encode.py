@@ -11,16 +11,18 @@ All segments come from one pass over the map; a repeated id gets the same string
 the string of ``[h * w]``.
 
 ``encode_rle_async`` uploads the seg ids and enqueues the encode and one copy of the offsets and the strings' first
-``PREFIX`` bytes on the current stream without synchronising; ``PendingRle.result()`` waits for them (and fetches the
-rest of longer strings).  Importing this module neither imports pycocotools nor initialises CUDA.
+``PREFIX`` bytes on the current stream without synchronising; the returned ``Pending``'s ``result()`` waits for them
+(and fetches the rest of longer strings; deva/utils/device_download.py).  Importing this module neither imports
+pycocotools nor initialises CUDA.
 """
-import os
+import functools
 from typing import List, Optional
 
 import numpy as np
 import torch
 
 from deva._native import MAX_SEGMENT_CHANNELS
+from deva.utils import device_download
 
 ENCODERS = ('pycocotools', 'device')
 ENV = 'DEVA_B200_RLE_ENCODER'
@@ -31,10 +33,7 @@ _INT_DTYPES = (torch.bool, torch.uint8, torch.int8, torch.int16, torch.int32, to
 
 def resolve_encoder(rle_encoder: Optional[str] = None) -> str:
     """``rle_encoder``, or the environment's ``DEVA_B200_RLE_ENCODER`` when it is None ('pycocotools' when unset)."""
-    value = os.environ.get(ENV, 'pycocotools') if rle_encoder is None else rle_encoder
-    if value not in ENCODERS:
-        raise ValueError(f'rle_encoder must be one of {ENCODERS}, not {value!r}')
-    return value
+    return device_download.resolve(rle_encoder, 'rle_encoder', ENV, ENCODERS, 'pycocotools')
 
 
 def host_bytes(n: int) -> int:
@@ -42,28 +41,9 @@ def host_bytes(n: int) -> int:
     return 16 * n + 8 + PREFIX
 
 
-class PendingRle:
-    """An encode enqueued by ``encode_rle_async``; ``result()`` -> one ``{'size': [h, w], 'counts': str}`` per seg id."""
-
-    def __init__(self, size, n: int, dev: Optional[torch.Tensor], host: Optional[torch.Tensor], prefix: int,
-                 done: Optional[torch.cuda.Event]):
-        self.size, self.n, self.dev, self.host, self.prefix, self.done = size, n, dev, host, prefix, done
-
-    def result(self) -> List[dict]:
-        n = self.n
-        if n == 0:
-            return []
-        self.done.synchronize()
-        offsets = self.host[8 * n:16 * n + 8].view(torch.int64).tolist()
-        total = offsets[n]
-        at = 16 * n + 8  # the strings, in the host and the device buffer alike
-        data = self.host[at:at + min(total, self.prefix)].numpy().tobytes()
-        if total > self.prefix:
-            data += self.dev[at + self.prefix:at + total].cpu().numpy().tobytes()
-        self.dev = None  # the device buffer is free once the strings are on the host
-        text = data.decode('ascii')
-        h, w = self.size
-        return [{'size': [h, w], 'counts': text[offsets[j]:offsets[j + 1]]} for j in range(n)]
+def _strings(h: int, w: int, offsets: List[int], data: bytes) -> List[dict]:
+    text = data.decode('ascii')
+    return [{'size': [h, w], 'counts': text[offsets[j]:offsets[j + 1]]} for j in range(len(offsets) - 1)]
 
 
 def _as_device_ids(ids) -> torch.Tensor:
@@ -72,7 +52,7 @@ def _as_device_ids(ids) -> torch.Tensor:
                                    ids.dtype in (np.uint8, np.uint16, np.uint32))):
             raise ValueError(f'an id map is an integer array [h, w], not {ids.dtype} {ids.shape}')
         _check_shape(ids.shape)
-        return torch.from_numpy(np.ascontiguousarray(ids, dtype=np.int64)).pin_memory().cuda(non_blocking=True)
+        return device_download.upload(ids, np.int64)
     if not (isinstance(ids, torch.Tensor) and ids.is_cuda and ids.dtype in _INT_DTYPES and ids.dim() == 2):
         desc = f'{ids.dtype} {tuple(ids.shape)} on {ids.device}' if isinstance(ids, torch.Tensor) else type(ids)
         raise ValueError(f'an id map is a CUDA integer tensor [h, w] or a numpy array, not {desc}')
@@ -103,35 +83,27 @@ def _as_id_list(seg_ids) -> List[int]:
     return out
 
 
-def encode_rle_async(ids, seg_ids, host: Optional[torch.Tensor] = None) -> PendingRle:
+def encode_rle_async(ids, seg_ids, host: Optional[torch.Tensor] = None) -> device_download.Pending:
     """Enqueues the RLE of ``ids == i`` for every ``i`` in ``seg_ids`` on the current stream; never synchronises the
     host.  ids: integer [h, w] (a CUDA tensor, or a numpy array that is uploaded); seg_ids: host integers.  host:
     optional pinned uint8 buffer of at least ``host_bytes(len(seg_ids))`` bytes through which the seg ids go up and the
     offsets and the strings' first bytes come back (one is allocated otherwise); it must stay untouched until
-    ``result()`` returns."""
+    ``result()`` returns, which gives one ``{'size': [h, w], 'counts': str}`` per seg id."""
     seg = _as_id_list(seg_ids)
     ids = _as_device_ids(ids)
     h, w = int(ids.shape[0]), int(ids.shape[1])
     n = len(seg)
     if n == 0:
-        return PendingRle((h, w), 0, None, None, 0, None)
+        return device_download.Pending(lambda *_: [])
     from deva import _native
     bound = _native.rle_bound(h, w, n)
     at = 16 * n + 8  # [seg ids | offsets | strings | workspace], the first three as in the host buffer
-    ws_at = (at + bound + 15) // 16 * 16
-    dev = torch.empty(ws_at + _native.rle_workspace_bytes(h, w, n), dtype=torch.uint8, device=ids.device)
-    prefix = min(PREFIX, bound)
-    if host is None:
-        host = torch.empty(at + prefix, dtype=torch.uint8, pin_memory=True)
-    assert host.is_pinned() and host.dtype == torch.uint8 and host.numel() >= at + prefix
+    dev, out, ws = device_download.buffer(at, bound, _native.rle_workspace_bytes(h, w, n), ids.device)
+    host = device_download.pinned(host, at + min(PREFIX, bound))
     host[:8 * n].view(torch.int64).numpy()[:] = seg
     dev[:8 * n].copy_(host[:8 * n], non_blocking=True)
-    _native.rle_encode(ids, dev[:8 * n].view(torch.int64), dev[ws_at:], dev[at:at + bound],
-                       dev[8 * n:at].view(torch.int64))
-    host[8 * n:at + prefix].copy_(dev[8 * n:at + prefix], non_blocking=True)
-    done = torch.cuda.Event()
-    done.record()
-    return PendingRle((h, w), n, dev, host, prefix, done)
+    _native.rle_encode(ids, dev[:8 * n].view(torch.int64), ws, out, dev[8 * n:at].view(torch.int64))
+    return device_download.enqueue(functools.partial(_strings, h, w), dev, (8 * n, at), bound, PREFIX, host)
 
 
 def encode_rle(ids, seg_ids) -> List[dict]:

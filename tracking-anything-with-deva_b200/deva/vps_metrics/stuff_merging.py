@@ -20,7 +20,8 @@ import numpy as np
 import torch
 from PIL import Image
 
-from deva.utils.png_encode import encode_png_async, resolve_encoder, write_png
+from deva.utils.device_download import write
+from deva.utils.png_encode import encode_png_async, resolve_encoder
 from deva.vps_metrics import scoring, video_pass
 
 
@@ -67,7 +68,7 @@ def merge_stuff(input_path, output_path, isthing=None, num_threads=None, *, png_
                 segments = scoring.merged_segments(things, stuff_to_id, out_ids, counts_h[t, :len(out_ids)], isthing)
                 video_annotations.append({'file_name': ann['file_name'], 'segments_info': segments})
                 if png_encoder == 'device':
-                    writes.append(decoder.pool.submit(write_png, outs[t], path.join(out_dir, names[t])))
+                    writes.append(decoder.pool.submit(write, outs[t], path.join(out_dir, names[t])))
                 else:
                     writes.append(decoder.pool.submit(_save, outs[t].cpu().numpy(), path.join(out_dir, names[t])))
             output_annotations.append({'video_id': video_id, 'annotations': video_annotations})
