@@ -27,7 +27,9 @@
 extern "C" {
 #endif
 
-/* v23: deva_b200_rle_bound, deva_b200_rle_workspace_bytes and deva_b200_rle_encode (BURST's per-segment COCO RLE encoded
+/* v24: deva_b200_png_decode_workspace_bytes and deva_b200_png_decode (the post-processing passes' PNGs decoded on the
+ * device).
+ * v23: deva_b200_rle_bound, deva_b200_rle_workspace_bytes and deva_b200_rle_encode (BURST's per-segment COCO RLE encoded
  * on the device).
  * v22: deva_b200_jpeg_bound, deva_b200_jpeg_workspace_bytes and deva_b200_jpeg_encode (result JPEGs encoded on the
  * device).
@@ -44,7 +46,7 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 23
+#define DEVA_B200_ABI_VERSION 24
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -443,6 +445,21 @@ DEVA_B200_API size_t deva_b200_rle_bound(int h, int w, int n);
 DEVA_B200_API size_t deva_b200_rle_workspace_bytes(int h, int w, int n);
 DEVA_B200_API int deva_b200_rle_encode(const int64_t* ids, int h, int w, const int64_t* seg_ids, int n, void* workspace,
                                        uint8_t* out, int64_t* offsets, deva_stream_t stream);
+
+/* ---- PNG decode (deva/utils/png_decode.py; the format rules are DESIGN §7) ----------------------------------------
+ * A batch of n files: streams holds their zlib streams (the concatenated IDAT data of each), desc int64 [n, 8] per file
+ * {stream offset, stream length, h, w, colour type, bit depth, output offset, workspace offset}, all on the device.  A
+ * supported file is grey at 2, 4 or 8 bits, palette at 1, 2, 4 or 8, RGB 8 or RGBA 8, non-interlaced.  For each file
+ * whose stream is one well-formed zlib stream that inflates to exactly h * (rowbytes + 1) bytes with a matching
+ * Adler-32, nothing after it, and every row's filter type <= 4, out[output offset ..] receives Pillow's array ([h, w]
+ * or [h, w, 3 | 4] uint8; 2- and 4-bit grey scaled by 85 and 17, palette indices unscaled) and status[i] = 0; any other
+ * file gets a nonzero int32 status and its output bytes are undefined.  Every read of a stream is bounded by its length
+ * and every write by the file's shape.  workspace + workspace offset: deva_b200_png_decode_workspace_bytes(h, w, colour
+ * type, bit depth) bytes per file (its filtered stream), 0 for an unsupported shape.  Enqueued on stream without
+ * synchronising the host; allocates nothing. */
+DEVA_B200_API size_t deva_b200_png_decode_workspace_bytes(int h, int w, int colour_type, int bits);
+DEVA_B200_API int deva_b200_png_decode(const uint8_t* streams, const int64_t* desc, int n, uint8_t* out, void* workspace,
+                                       int32_t* status, deva_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -135,7 +135,10 @@ def main():
     ap.add_argument('--videos', type=int, default=4)
     ap.add_argument('--max-objects', type=int, default=20)
     ap.add_argument('--seed', type=int, default=0)
+    ap.add_argument('--png-decoder', choices=('pil', 'device', 'both'), default='pil',
+                    help="the input decoder of limit_max_id; 'both' times the two, alternating, in one run")
     args = ap.parse_args()
+    decoders = ('pil', 'device') if args.png_decoder == 'both' else (args.png_decoder,)
     from deva import _native as nat
     nat.require_device()
     ref = load_reference()
@@ -146,18 +149,27 @@ def main():
         src = os.path.join(root, 'in')
         n = make_dataset(src, args.videos, args.seed)
         m = args.max_objects
-        limit_max_id(src, os.path.join(root, 'warm'), m)  # CUDA context, module load, pinned pool
-        t = {'ours': timed(lambda: limit_max_id(src, os.path.join(root, 'ours'), m)),
-             'reference': timed(lambda: ref.limit_max_id(src, os.path.join(root, 'ref'), m))}
-        ours, want = us.snapshot(os.path.join(root, 'ours')), us.snapshot(os.path.join(root, 'ref'))
-        equal = sorted(ours) == sorted(want) and all(
-            ours[k][:2] == want[k][:2] and np.array_equal(ours[k][2], want[k][2]) for k in want)
+        for d in decoders:  # CUDA context, module load, pinned pool
+            limit_max_id(src, os.path.join(root, 'warm'), m, png_decoder=d)
+        runs = {d: [] for d in decoders}
+        for _ in range(2 if len(decoders) > 1 else 1):  # alternating, so both paths see the same machine state
+            for d in decoders:
+                runs[d].append(timed(lambda: limit_max_id(src, os.path.join(root, 'ours_' + d), m, png_decoder=d)))
+        t = {f'ours_{d}': min(v) for d, v in runs.items()}
+        t['reference'] = timed(lambda: ref.limit_max_id(src, os.path.join(root, 'ref'), m))
+        want = us.snapshot(os.path.join(root, 'ref'))
+        equal, davis = {}, True
+        for d in decoders:
+            ours = us.snapshot(os.path.join(root, 'ours_' + d))
+            equal[d] = sorted(ours) == sorted(want) and all(
+                ours[k][:2] == want[k][:2] and np.array_equal(ours[k][2], want[k][2]) for k in want)
+            davis = davis and all(v[1] == us.sha(bytes(davis_palette)) for v in ours.values())
         out = {'card': card(), 'cpu_threads': os.cpu_count(),
                'dataset': {'videos': args.videos, 'frames': n, 'size': [H, W], 'labels_per_frame': [20, 60],
                            'max_num_objects': m},
                'per_frame_ms': {k: round(v * 1e3 / n, 3) for k, v in t.items()},
-               'speedup': round(t['reference'] / t['ours'], 1), 'files_equal': bool(equal), 'files': len(want),
-               'palette_is_davis': all(v[1] == us.sha(bytes(davis_palette)) for v in ours.values()),
+               'speedup': {d: round(t['reference'] / t['ours_' + d], 1) for d in decoders},
+               'files_equal': {d: bool(v) for d, v in equal.items()}, 'files': len(want), 'palette_is_davis': davis,
                'ours_parts_per_frame': parts(src, m)}
         print(json.dumps(out))
     finally:

@@ -126,7 +126,10 @@ def main():
     ap.add_argument('--videos', type=int, default=4)
     ap.add_argument('--frames', type=int, default=25)
     ap.add_argument('--segments', type=int, default=60)
+    ap.add_argument('--png-decoder', choices=('pil', 'device', 'both'), default='pil',
+                    help="the input decoder of our passes; 'both' times the two, alternating, in one run")
     args = ap.parse_args()
+    decoders = ('pil', 'device') if args.png_decoder == 'both' else (args.png_decoder,)
     from deva import _native as nat
     nat.require_device()
     ref = load_reference()
@@ -148,22 +151,31 @@ def main():
         t['ref_merge'] = timed(lambda: ref_merged.extend(ref['stuff_merging'].process_single_video(a, submit,
                                                                                                    root + '/m_ref')
                                                          for a in anns))
-        np.random.seed(0)
-        t['ours_merge'] = timed(lambda: merge_stuff(submit, root + '/m_ours', isthing=isthing))
-        t['ours_vpq'] = timed(lambda: eval_vpq(submit, truth, gt_path))
-        t['ours_stq'] = timed(lambda: eval_stq(submit, truth, gt_path))
-        ours_files = {n: open(os.path.join(submit, n)).read() for n in os.listdir(submit) if n.endswith('.txt')}
-        t['ours_vps'] = timed(lambda: eval_vps(submit, truth, gt_path))
+        ours_files, merged = {}, {}
+        for _ in range(2 if len(decoders) > 1 else 1):  # alternating, so both paths see the same machine state
+            for d in decoders:
+                np.random.seed(0)
+                t[f'ours_merge_{d}'] = min(t.get(f'ours_merge_{d}', 1e9), timed(
+                    lambda: merge_stuff(submit, root + '/m_ours_' + d, isthing=isthing, png_decoder=d)))
+                merged[d] = json.load(open(root + '/m_ours_' + d + '/pred.json'))
+                t[f'ours_vpq_{d}'] = min(t.get(f'ours_vpq_{d}', 1e9), timed(
+                    lambda: eval_vpq(submit, truth, gt_path, png_decoder=d)))
+                t[f'ours_stq_{d}'] = min(t.get(f'ours_stq_{d}', 1e9), timed(
+                    lambda: eval_stq(submit, truth, gt_path, png_decoder=d)))
+                ours_files[d] = {n: open(os.path.join(submit, n)).read() for n in os.listdir(submit)
+                                 if n.endswith('.txt')}
+                t[f'ours_vps_{d}'] = min(t.get(f'ours_vps_{d}', 1e9), timed(
+                    lambda: eval_vps(submit, truth, gt_path, png_decoder=d)))
         t['ref_vpq'] = timed(lambda: ref['eval_vpq_vipseg'].eval_vpq(submit, truth, gt_path, num_processes=n_proc))
         t['ref_stq'] = timed(lambda: ref['eval_stq_vipseg'].eval_stq(submit, truth, gt_path))
         ref_files = {n: open(os.path.join(submit, n)).read() for n in os.listdir(submit) if n.endswith('.txt')}
-        out['merge_json_equal'] = json.load(open(root + '/m_ours/pred.json')) == {'annotations': ref_merged}
+        out['merge_json_equal'] = {d: m == {'annotations': ref_merged} for d, m in merged.items()}
         out['card'] = card()
         out['cpu_threads'] = os.cpu_count()
         out['dataset'] = {'videos': args.videos, 'frames': args.frames, 'size': [720, 1280],
                           'segments_per_frame': args.segments}
         out['per_video_s'] = {k: round(v / args.videos, 3) for k, v in t.items()}
-        out['files_equal'] = ours_files == ref_files
+        out['files_equal'] = {d: f == ref_files for d, f in ours_files.items()}
         out['ours_pass_parts_per_video_ms'] = {k: (round(v / args.videos, 2) if k.endswith('_ms') else v)
                                                for k, v in parts(submit, truth, gt_path).items()}
         print(json.dumps(out))

@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 23
+ABI_VERSION = 24
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -125,6 +125,8 @@ _SIGNATURES = {
     'deva_b200_rle_bound': (c_size_t, [c_int, c_int, c_int]),
     'deva_b200_rle_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'deva_b200_rle_encode': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'deva_b200_png_decode_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
+    'deva_b200_png_decode': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -568,6 +570,25 @@ def rle_encode(ids, seg_ids, workspace, out, offsets):
     assert workspace.numel() * workspace.element_size() >= rle_workspace_bytes(h, w, n)
     _check(lib().deva_b200_rle_encode(_ptr(ids), h, w, _ptr(seg_ids), n, _ptr(workspace), _ptr(out), _ptr(offsets),
                                       _stream()), 'rle_encode')
+
+
+PNG_DESC_FIELDS = 8
+
+
+def png_decode_workspace_bytes(h, w, colour_type, bits) -> int:
+    return int(lib().deva_b200_png_decode_workspace_bytes(h, w, colour_type, bits))
+
+
+def png_decode(streams, desc, out, workspace, status):
+    """streams uint8: the files' zlib streams; desc int64 [n, 8]; out uint8: the arrays at their offsets; workspace
+    uint8: the filtered streams at their offsets; status int32 [n]; all on the device (see include/deva_b200.h)."""
+    n = desc.shape[0]
+    assert desc.dtype == torch.int64 and desc.is_cuda and desc.is_contiguous() and desc.shape == (n, PNG_DESC_FIELDS)
+    assert status.dtype == torch.int32 and status.is_cuda and status.numel() == n
+    for t in (streams, out, workspace):
+        assert t.dtype == torch.uint8 and t.is_cuda and t.is_contiguous()
+    _check(lib().deva_b200_png_decode(_ptr(streams), _ptr(desc), n, _ptr(out), _ptr(workspace), _ptr(status),
+                                      _stream()), 'png_decode')
 
 
 def transpose_append(src, dst, ld_dst, n, c):

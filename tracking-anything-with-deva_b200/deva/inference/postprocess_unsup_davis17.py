@@ -15,7 +15,9 @@ Per video each file is decoded once on a pool of host threads and uploaded throu
 the device for both passes.  ``deva_b200_label_areas`` counts every frame's labels, and the per-frame lists come to the
 host once; the selection runs there, on lists of at most a few thousand entries.  The (label -> index) table goes back
 to the device, ``deva_b200_label_to_index`` rewrites every frame, and the index maps come back through pinned memory
-to be encoded on the thread pool.  With ``png_encoder='device'`` (or ``DEVA_B200_PNG_ENCODER=device``) they are encoded
+to be encoded on the thread pool.  With ``png_decoder='device'`` (or ``DEVA_B200_PNG_DECODER=device``) the files are
+read on the pool and decoded a video at a time on the device (png_pipeline.DeviceDecoder); a file the device does not
+take is read by read_frame as before.  With ``png_encoder='device'`` (or ``DEVA_B200_PNG_ENCODER=device``) they are encoded
 as PNGs on the device instead (deva/utils/png_encode.py), and only the compressed files come back.  Files are read in
 full before any of their video is written, so input_path == output_path (as evaluation/eval_with_detections.py calls
 it) is safe.
@@ -34,7 +36,8 @@ from PIL import Image
 
 from deva.utils.device_download import write
 from deva.utils.png_encode import encode_png_async, resolve_encoder
-from deva.utils.png_pipeline import Decoder, Uploader
+from deva.utils.png_decode import resolve_decoder
+from deva.utils.png_pipeline import Decoder, DeviceDecoder, Uploader
 
 CAPACITY = 1024  # label table entries per frame; a frame with more distinct labels is counted again with a larger table
 MODES = ('P', 'L', 'RGB', 'RGBA')
@@ -158,17 +161,22 @@ def _limit_video(decoder, upload, video_path, out_dir, max_num_objects, palette,
         raise unreadable  # the rewrite pass wrote the frames before it
 
 
-def limit_max_id(input_path, output_path, max_num_objects=20, *, palette=None, num_threads=None, png_encoder=None):
+def limit_max_id(input_path, output_path, max_num_objects=20, *, palette=None, num_threads=None, png_encoder=None,
+                 png_decoder=None):
     """palette: the PNGs' palette; None = DAVIS's (deva.utils.palette.davis_palette, which comes from the reference
     checkout).  num_threads: host threads that decode and encode PNGs.  png_encoder: 'pil' or 'device'; None reads
-    DEVA_B200_PNG_ENCODER (default 'pil')."""
+    DEVA_B200_PNG_ENCODER (default 'pil').  png_decoder: 'pil' or 'device'; None reads DEVA_B200_PNG_DECODER (default
+    'pil')."""
     png_encoder = resolve_encoder(png_encoder)
+    png_decoder = resolve_decoder(png_decoder)
     if palette is None:
         from deva.utils.palette import davis_palette as palette
     from deva import _native
     _native.require_device()
     dev = torch.device('cuda', torch.cuda.current_device())
-    decoder, upload = Decoder(read_frame, num_threads), Uploader(dev)
+    decoder = DeviceDecoder(read_frame, dev, num_threads=num_threads) if png_decoder == 'device' else \
+        Decoder(read_frame, num_threads)
+    upload = Uploader(dev)
     try:
         for video in sorted(os.listdir(input_path)):
             _limit_video(decoder, upload, path.join(input_path, video), path.join(output_path, video), max_num_objects,

@@ -8,6 +8,6 @@ from pkgutil import extend_path
 __path__ = extend_path(__path__, __name__)
 
 
-def eval_vps(submit_dir, truth_dir, pan_gt_json_file, num_processes=None):
+def eval_vps(submit_dir, truth_dir, pan_gt_json_file, num_processes=None, *, png_decoder=None):
     from deva.vps_metrics.video_pass import eval_vps as run
-    return run(submit_dir, truth_dir, pan_gt_json_file, num_processes)
+    return run(submit_dir, truth_dir, pan_gt_json_file, num_processes, png_decoder=png_decoder)

@@ -7,13 +7,14 @@ import time
 from deva.vps_metrics import video_pass
 
 
-def eval_vpq(submit_dir, truth_dir, pan_gt_json_file, num_processes=None):
-    """num_processes: host threads that decode PNGs (default: up to 16)."""
+def eval_vpq(submit_dir, truth_dir, pan_gt_json_file, num_processes=None, *, png_decoder=None):
+    """num_processes: host threads that decode PNGs (default: up to 16).  png_decoder: 'pil' or 'device'; None reads
+    DEVA_B200_PNG_DECODER (default 'pil')."""
     output_dir = submit_dir
     if not os.path.isdir(submit_dir):
         print("%s doesn't exist" % submit_dir)
     start_all = time.time()
     vpq_stats, _, categories_list = video_pass.evaluate(submit_dir, truth_dir, pan_gt_json_file, stq=False,
-                                                        num_threads=num_processes)
+                                                        num_threads=num_processes, png_decoder=png_decoder)
     video_pass.write_vpq(output_dir, vpq_stats, categories_list)
     print('==> All:', time.time() - start_all, 'sec')

@@ -6,7 +6,9 @@ new id, every stuff category maps to one id, and a collision draws from the glob
 That gives each frame a table -> output-id rewrite, which ``deva_b200_pano_remap`` applies per pixel while it writes the
 RGB of the new id and counts the pixels of every output id (the areas that decide which stuff entries are kept).  PNGs
 are decoded and encoded on a pool of host threads; with ``png_encoder='device'`` (or ``DEVA_B200_PNG_ENCODER=device``)
-the rewritten maps are encoded on the device (deva/utils/png_encode.py) and only the compressed files come back.
+the rewritten maps are encoded on the device (deva/utils/png_encode.py) and only the compressed files come back; with
+``png_decoder='device'`` (or ``DEVA_B200_PNG_DECODER=device``) the input maps are decoded on the device
+(deva/utils/png_decode.py) and only the compressed files go up.
 
 Videos are processed in order in this process.  The reference maps them over ``Pool(16)``, so its random draws depend on
 which worker handles which video; here they follow the order of ``pred.json``, as a serial run of the reference's
@@ -21,6 +23,7 @@ import torch
 from PIL import Image
 
 from deva.utils.device_download import write
+from deva.utils.png_decode import resolve_decoder
 from deva.utils.png_encode import encode_png_async, resolve_encoder
 from deva.vps_metrics import scoring, video_pass
 
@@ -29,18 +32,19 @@ def _save(rgb: np.ndarray, file: str):
     Image.fromarray(rgb).save(file)
 
 
-def merge_stuff(input_path, output_path, isthing=None, num_threads=None, *, png_encoder=None):
+def merge_stuff(input_path, output_path, isthing=None, num_threads=None, *, png_encoder=None, png_decoder=None):
     """isthing: {category id: bool}; None = the VIPSeg category table (deva.utils.pano_utils.vipseg_cat_to_isthing,
     which comes from the reference checkout).  png_encoder: 'pil' or 'device'; None reads DEVA_B200_PNG_ENCODER
-    (default 'pil')."""
+    (default 'pil').  png_decoder: 'pil' or 'device'; None reads DEVA_B200_PNG_DECODER (default 'pil')."""
     png_encoder = resolve_encoder(png_encoder)
+    png_decoder = resolve_decoder(png_decoder)
     if isthing is None:
         from deva.utils.pano_utils import vipseg_cat_to_isthing as isthing
     from deva import _native
     with open(path.join(input_path, 'pred.json')) as f:
         annotations = json.load(f)['annotations']
     dev = video_pass.require_device()
-    decoder, upload = video_pass.Decoder(num_threads), video_pass.Uploader(dev)
+    decoder, upload = video_pass.make_decoder(png_decoder, dev, num_threads), video_pass.Uploader(dev)
     writes = []
     output_annotations = []
     try:

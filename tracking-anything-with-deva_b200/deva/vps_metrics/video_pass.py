@@ -1,7 +1,8 @@
 """The one per-video device pass behind VPQ, STQ and stuff merging.
 
 PNGs are decoded with PIL on a pool of host threads (in order, ahead of use), copied into a ring of pinned staging
-buffers and uploaded; each frame pair is reduced by ``deva_b200_pano_joint_hist`` into its slice of one int32
+buffers and uploaded, or with ``png_decoder='device'`` (``DEVA_B200_PNG_DECODER=device``) decoded a video at a time on
+the device (png_pipeline.DeviceDecoder); each frame pair is reduced by ``deva_b200_pano_joint_hist`` into its slice of one int32
 ``[T, G + 1, P + 1]`` buffer, and that buffer comes to the host once per video.  Importing this module does not
 initialise CUDA.
 """
@@ -13,6 +14,7 @@ import torch
 from PIL import Image
 
 from deva.utils import png_pipeline
+from deva.utils.png_decode import resolve_decoder
 from deva.utils.png_pipeline import RING, Uploader  # noqa: F401  (part of this module's interface)
 from deva.vps_metrics import scoring
 
@@ -32,6 +34,14 @@ class Decoder(png_pipeline.Decoder):
         super().__init__(read_rgb, num_threads)
 
 
+def make_decoder(png_decoder, device, num_threads=None):
+    """The frame source of RGB id PNGs: Decoder for 'pil', the device's for 'device' (RGB and RGBA files; every other
+    file goes through read_rgb and raises its error)."""
+    if png_decoder == 'device':
+        return png_pipeline.DeviceDecoder(read_rgb, device, modes=('RGB', 'RGBA'), rgb=True, num_threads=num_threads)
+    return Decoder(num_threads)
+
+
 def require_device():
     from deva import _native
     _native.require_device()
@@ -45,10 +55,13 @@ def video_histograms(decoder, upload, gt_paths, pred_paths, gt_ids, pred_ids):
     g = torch.from_numpy(gt_ids).to(dev, non_blocking=True)
     p = torch.from_numpy(pred_ids).to(dev, non_blocking=True)
     hist = torch.empty(len(gt_paths), len(gt_ids) + 1, len(pred_ids) + 1, dtype=torch.int32, device=dev)
-    gts, preds = decoder.frames(gt_paths), decoder.frames(pred_paths)
-    for t, (gt, pred) in enumerate(zip(gts, preds)):
-        if gt.shape != pred.shape:
-            raise ValueError(f'{gt_paths[t]} and {pred_paths[t]} differ in size: {gt.shape} vs {pred.shape}')
+    # one frame source over gt 0, pred 0, gt 1, ...: the order in which a pair's errors are met, and one batch of the
+    # device decoder over both sides
+    frames = decoder.frames([path for pair in zip(gt_paths, pred_paths) for path in pair])
+    for t, (gt, pred) in enumerate(zip(frames, frames)):
+        if tuple(gt.shape) != tuple(pred.shape):
+            raise ValueError(f'{gt_paths[t]} and {pred_paths[t]} differ in size: {tuple(gt.shape)} vs '
+                             f'{tuple(pred.shape)}')
         _native.pano_joint_hist(upload(gt), upload(pred), g, p, hist[t])
     return hist.cpu().numpy()
 
@@ -81,17 +94,21 @@ def png_labels(paths):
     return labels
 
 
-def evaluate(submit_dir, truth_dir, pan_gt_json_file, *, vpq=True, stq=True, num_threads=None, histograms=None):
+def evaluate(submit_dir, truth_dir, pan_gt_json_file, *, vpq=True, stq=True, num_threads=None, histograms=None,
+             png_decoder=None):
     """One decode pass over the dataset.  -> ({nframes: PQStat} or None, STQuality or None, categories list).
-    histograms(decoder, gt_paths, pred_paths, gt_ids, pred_ids) -> int [T, G + 1, P + 1]; default: the device pass."""
+    histograms(decoder, gt_paths, pred_paths, gt_ids, pred_ids) -> int [T, G + 1, P + 1]; default: the device pass.
+    png_decoder: 'pil' or 'device'; None reads DEVA_B200_PNG_DECODER (default 'pil')."""
+    png_decoder = resolve_decoder(png_decoder)
     categories_list, videos = load_dataset(submit_dir, truth_dir, pan_gt_json_file)
     categories = {el['id']: el for el in categories_list}
+    dev = require_device() if histograms is None or png_decoder == 'device' else None
     if histograms is None:
-        upload = Uploader(require_device())
+        upload = Uploader(dev)
 
         def histograms(decoder, *args):
             return video_histograms(decoder, upload, *args)
-    decoder = Decoder(num_threads)
+    decoder = make_decoder(png_decoder, dev, num_threads)
     vpq_stats = {n: scoring.PQStat() for n in scoring.NFRAMES} if vpq else None
     stq_metric = scoring.STQuality(scoring.thing_list(categories_list)) if stq else None
     try:
@@ -133,10 +150,11 @@ def write_stq(output_dir, stq_metric):
     return result
 
 
-def eval_vps(submit_dir, truth_dir, pan_gt_json_file, num_processes=None):
+def eval_vps(submit_dir, truth_dir, pan_gt_json_file, num_processes=None, *, png_decoder=None):
     """VPQ at every window size and STQ from one decode pass: writes vpq-{n}.txt, vpq-simple.txt and stq.txt into
-    submit_dir, as eval_vpq and eval_stq do.  num_processes: host decode threads."""
+    submit_dir, as eval_vpq and eval_stq do.  num_processes: host decode threads.  png_decoder: 'pil' or 'device'; None
+    reads DEVA_B200_PNG_DECODER (default 'pil')."""
     vpq_stats, stq_metric, categories_list = evaluate(submit_dir, truth_dir, pan_gt_json_file,
-                                                      num_threads=num_processes)
+                                                      num_threads=num_processes, png_decoder=png_decoder)
     write_vpq(submit_dir, vpq_stats, categories_list)
     write_stq(submit_dir, stq_metric)
