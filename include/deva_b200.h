@@ -27,7 +27,8 @@
 extern "C" {
 #endif
 
-/* v24: deva_b200_png_decode_workspace_bytes and deva_b200_png_decode (the post-processing passes' PNGs decoded on the
+/* v25: deva_b200_jpeg_decode_workspace_bytes and deva_b200_jpeg_decode (baseline JPEG files decoded on the device).
+ * v24: deva_b200_png_decode_workspace_bytes and deva_b200_png_decode (the post-processing passes' PNGs decoded on the
  * device).
  * v23: deva_b200_rle_bound, deva_b200_rle_workspace_bytes and deva_b200_rle_encode (BURST's per-segment COCO RLE encoded
  * on the device).
@@ -46,7 +47,7 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 24
+#define DEVA_B200_ABI_VERSION 25
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -460,6 +461,30 @@ DEVA_B200_API int deva_b200_rle_encode(const int64_t* ids, int h, int w, const i
 DEVA_B200_API size_t deva_b200_png_decode_workspace_bytes(int h, int w, int colour_type, int bits);
 DEVA_B200_API int deva_b200_png_decode(const uint8_t* streams, const int64_t* desc, int n, uint8_t* out, void* workspace,
                                        int32_t* status, deva_stream_t stream);
+
+/* ---- JPEG decode (deva/utils/jpeg_decode.py; the format rules are DESIGN §7) ---------------------------------------
+ * A batch of n baseline files, all on the device: scans holds their entropy-coded data with the stuffing bytes and
+ * RSTn markers removed; desc int64 [n, 11] per file {scan offset, scan length, h, w, luma h sampling, luma v sampling,
+ * tables index, output offset, workspace offset, first subsequence, subsequences}; tables int32 [n, 5016] per file (the
+ * DC and AC Huffman lookups of each component and its quantisation table in natural order, csrc/jpeg_decode.cuh);
+ * intervals int64 [n_intervals, 6] per restart interval {file, bit start, bit end, first block, blocks, first
+ * subsequence}; subs int64 [n_subs, 3] per subsequence {interval, bit start, bit end}, the subsequences of an interval
+ * consecutive and covering it, bits counted from scans.  Y is sampled 1x1, 2x1 or 2x2 and Cb, Cr 1x1.  For each file
+ * whose every interval decodes to exactly its blocks, with at most 7 padding bits left, every code in its table,
+ * categories <= 11 (DC) and 10 (AC), no run past coefficient 63, and every block in the range where libjpeg-turbo's C
+ * and x86 SIMD islow IDCTs agree, out[output offset ..] receives Pillow's array ([h, w, 3] uint8: islow IDCT, fancy
+ * upsampling, jdcolor.c's YCbCr -> RGB) and status[i] = 0; any other file gets a nonzero int32 status and undefined
+ * output bytes.  Every read of the scans is bounded by its interval and every write by the file's shape.  workspace:
+ * deva_b200_jpeg_decode_workspace_bytes(0, 0, 0, 0, 0) bytes shared by the batch (its int32 word 3 receives the number
+ * of synchronisation rounds), then at each file's workspace offset deva_b200_jpeg_decode_workspace_bytes(h, w, luma h,
+ * luma v, subsequences) bytes (0 for an unsupported shape).  The entropy decode is one cooperative launch.  Enqueued on
+ * stream without synchronising the host; allocates nothing. */
+DEVA_B200_API size_t deva_b200_jpeg_decode_workspace_bytes(int h, int w, int luma_h, int luma_v,
+                                                           int64_t subsequences);
+DEVA_B200_API int deva_b200_jpeg_decode(const uint8_t* scans, const int64_t* desc, int n, const int32_t* tables,
+                                        const int64_t* intervals, int64_t n_intervals, const int64_t* subs,
+                                        int64_t n_subs, uint8_t* out, void* workspace, int32_t* status,
+                                        deva_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -1,6 +1,6 @@
 """Per-frame cost of the result saver, the reference's and this package's, and one end-to-end demo loop with each.
 
-    python tools/bench_saver.py [--frames 20] [--ref-frames 4] [--e2e-steps 60] [--ref-e2e-steps 15]
+    python tools/bench_saver.py [--frames 20] [--ref-frames 4] [--e2e-steps 60] [--ref-e2e-steps 15] [--path-to-image]
 
 Per frame at 1080p: prob float32 [K+1, 480, 854] on the device, save_mask(need_resize=True, shape=(1080, 1920)) in
   * demo mode (long ids: RGB id PNG, JSON areas, overlay JPEG from a uint8 image_np) and
@@ -12,6 +12,12 @@ wait on the frame's copies).  Files go to a temporary directory that is removed 
 End to end: 1080p uint8 host frames -> frame_from_rgb8(size=480) -> step (bench.py's c2 setup: 5 objects, 2k slots,
 at 480x853) -> save_mask(need_resize=True, shape=(1080, 1920), image_np=frame) in demo mode with long ids, then end();
 frames/s over the whole run, next to the same loop without a saver.
+
+With --path-to-image, only the overlay given as a file is measured, with this package's saver and both device encoders:
+the demo frames are 1080p JPEGs (Pillow quality 90, 4:2:0) passed as path_to_image, decoded by Pillow on the writer
+thread and blended on the host (jpeg_decoder='pil') or decoded and blended on the device (jpeg_decoder='device').  It
+reports save_ms / writer_ms per frame for K = 16 and the end-to-end loop with each decoder, next to the same loop with
+the frames as image_np.
 
 The reference's ResultSaver is the unmodified module staged under oracle/_ref (oracle/build_ref.py), loaded by path
 under its own module name; oracle/_ref goes on sys.path after this package, so its imports of deva.* resolve to this
@@ -198,16 +204,110 @@ def e2e(savers, steps, ref_steps, warmup=RING_SIZE + 1, impls=('none', 'ours', '
     return out
 
 
+def _demo_jpegs(root, n=5):
+    """n 1080p demo frames as JPEG files -> (paths, the arrays Pillow decodes them to)."""
+    import io
+    from PIL import Image
+    sys.path.insert(0, os.path.join(ROOT, 'tests', 'golden'))
+    import jpeg_cases
+    paths, arrays = [], []
+    for t in range(n):
+        b = io.BytesIO()
+        Image.fromarray(jpeg_cases.overlay(1080, 1920, seed=t)).save(b, 'JPEG', quality=90)
+        paths.append(os.path.join(root, f'frame{t}.jpg'))
+        with open(paths[-1], 'wb') as f:
+            f.write(b.getvalue())
+        arrays.append(np.asarray(Image.open(io.BytesIO(b.getvalue()))).copy())
+    return paths, arrays
+
+
+def path_to_image(n, steps, warmup=RING_SIZE + 1):
+    """save_ms / writer_ms per 1080p frame (K = 16) and the end-to-end demo loop, with the overlay's frame given as a
+    JPEG path (Pillow or device decoder) or as image_np; device PNG and JPEG encoders throughout."""
+    from deva.inference import result_utils
+    from deva.inference.frame_io import frame_from_rgb8
+    from deva.inference.result_utils import ResultSaver
+    result_utils.Queue = TimedQueue  # only the frame queue calls task_done(), so only it accumulates
+    src = tempfile.mkdtemp()
+    paths, arrays = _demo_jpegs(src)
+    variants = {'image_np': ('pil', lambda i: dict(image_np=arrays[i % 5])),
+                'path_pil': ('pil', lambda i: dict(path_to_image=paths[i % 5])),
+                'path_device': ('device', lambda i: dict(path_to_image=paths[i % 5]))}
+    out = {'per_frame_k16': {}, 'e2e': {}}
+    g = torch.Generator(device='cuda').manual_seed(0)
+    prob = torch.softmax(4 * torch.randn(17, 480 // 8, 854 // 8, device='cuda', generator=g), 0)
+    prob = torch.nn.functional.interpolate(prob[None], (480, 854), mode='bilinear')[0].contiguous()
+    wl = dict(bench.WORKLOADS['c2'], w=853)
+    frames = [torch.from_numpy(a).pin_memory() for a in arrays]
+    try:
+        for name, (decoder, kw) in variants.items():
+            root = tempfile.mkdtemp()
+            try:
+                saver = ResultSaver(root, 'v', dataset='demo', object_manager=make_om(16, True), png_encoder='device',
+                                    jpeg_encoder='device', jpeg_decoder=decoder)
+                for i in range(warmup):
+                    saver.save_mask(prob, f'warm{i}.jpg', need_resize=True, shape=(1080, 1920), **kw(i))
+                saver.queue.join()
+                saver.queue.busy, saver.queue.items = 0.0, 0
+                torch.cuda.synchronize()
+                calls = []
+                for i in range(n):
+                    a = time.perf_counter()
+                    saver.save_mask(prob, f'{i:05d}.jpg', need_resize=True, shape=(1080, 1920), **kw(i))
+                    calls.append(time.perf_counter() - a)
+                saver.end()
+                free = calls[:QUEUE_SIZE - 1]
+                out['per_frame_k16'][name] = {'save_ms': round(sum(free) * 1e3 / len(free), 3),
+                                              'writer_ms': round(saver.queue.busy * 1e3 / saver.queue.items, 2)}
+            finally:
+                shutil.rmtree(root, ignore_errors=True)
+            clip = bench.Clip(wl, torch.device('cuda', 0), seed=0)
+            clip.core.object_manager.use_long_id = True
+            root = tempfile.mkdtemp()
+            try:
+                saver = ResultSaver(root, None, dataset='demo', object_manager=clip.core.object_manager,
+                                    png_encoder='device', jpeg_encoder='device', jpeg_decoder=decoder)
+
+                def one(i):
+                    p = clip.core.step(frame_from_rgb8(frames[i % 5], size=480))
+                    saver.save_mask(p, f'{i:05d}.jpg', need_resize=True, shape=(1080, 1920), **kw(i))
+                    clip.clamp()
+
+                for i in range(warmup):
+                    one(i)
+                saver.queue.join()
+                saver.queue.busy, saver.queue.items = 0.0, 0
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                for i in range(steps):
+                    one(i)
+                saver.end()
+                torch.cuda.synchronize()
+                ms = (time.perf_counter() - t0) * 1e3 / steps
+                out['e2e'][name] = {'ms_per_frame': round(ms, 2), 'fps': round(1e3 / ms, 2), 'frames': steps,
+                                    'writer_ms': round(saver.queue.busy * 1e3 / saver.queue.items, 2)}
+            finally:
+                shutil.rmtree(root, ignore_errors=True)
+    finally:
+        shutil.rmtree(src, ignore_errors=True)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--frames', type=int, default=20)
     ap.add_argument('--ref-frames', type=int, default=4)
     ap.add_argument('--e2e-steps', type=int, default=60)
     ap.add_argument('--ref-e2e-steps', type=int, default=15)
+    ap.add_argument('--path-to-image', action='store_true')
     args = ap.parse_args()
     from deva import _native as nat
     nat.require_device()
     torch.set_grad_enabled(False)
+    if args.path_to_image:
+        print(json.dumps({'card': card(), 'cpu_threads': torch.get_num_threads(),
+                          'path_to_image_1080p_demo': path_to_image(args.frames, args.e2e_steps)}))
+        return
     savers = load_savers()
     out = {'card': card(), 'cpu_threads': torch.get_num_threads(),
            'per_frame_1080p': per_frame(savers, args.frames, args.ref_frames), 'pil_encode_1080p_ms': encode_ms(),

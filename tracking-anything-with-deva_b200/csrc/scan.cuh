@@ -63,7 +63,7 @@ struct Carver {
   size_t bytes = 0;
 
   template <typename T>
-  T* take(long long count) {
+  __host__ __device__ T* take(long long count) {
     T* at = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
     bytes += ((size_t)count * sizeof(T) + kAlign - 1) / kAlign * kAlign;
     return at;

@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 24
+ABI_VERSION = 25
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -127,6 +127,9 @@ _SIGNATURES = {
     'deva_b200_rle_encode': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'deva_b200_png_decode_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
     'deva_b200_png_decode': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'deva_b200_jpeg_decode_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int, c_int64]),
+    'deva_b200_jpeg_decode': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p,
+                                      c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -589,6 +592,26 @@ def png_decode(streams, desc, out, workspace, status):
         assert t.dtype == torch.uint8 and t.is_cuda and t.is_contiguous()
     _check(lib().deva_b200_png_decode(_ptr(streams), _ptr(desc), n, _ptr(out), _ptr(workspace), _ptr(status),
                                       _stream()), 'png_decode')
+
+
+def jpeg_decode_workspace_bytes(h, w, luma_h, luma_v, subsequences) -> int:
+    return int(lib().deva_b200_jpeg_decode_workspace_bytes(h, w, luma_h, luma_v, subsequences))
+
+
+def jpeg_decode(scans, desc, tables, intervals, subs, out, workspace, status):
+    """scans uint8: the files' unstuffed scans; desc int64 [n, 11]; tables int32 [n, 5016]; intervals int64
+    [., 6]; subs int64 [., 3]; out uint8: the arrays at their offsets; workspace uint8; status int32 [n]; all on the
+    device (see include/deva_b200.h)."""
+    n = desc.shape[0]
+    assert desc.dtype == torch.int64 and desc.is_cuda and desc.is_contiguous() and desc.shape == (n, 11)
+    assert tables.dtype == torch.int32 and tables.is_cuda and tables.shape == (n, 5016)
+    assert intervals.dtype == torch.int64 and subs.dtype == torch.int64 and intervals.is_cuda and subs.is_cuda
+    assert status.dtype == torch.int32 and status.is_cuda and status.numel() == n
+    for t in (scans, out, workspace):
+        assert t.dtype == torch.uint8 and t.is_cuda and t.is_contiguous()
+    _check(lib().deva_b200_jpeg_decode(_ptr(scans), _ptr(desc), n, _ptr(tables), _ptr(intervals), intervals.shape[0],
+                                       _ptr(subs), subs.shape[0], _ptr(out), _ptr(workspace), _ptr(status),
+                                       _stream()), 'jpeg_decode')
 
 
 def transpose_append(src, dst, ld_dst, n, c):

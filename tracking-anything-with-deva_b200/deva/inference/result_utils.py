@@ -22,6 +22,15 @@ With ``rle_encoder='device'`` (or ``DEVA_B200_RLE_ENCODER=device``) burst's per-
 device (deva/utils/rle_encode.py), string for string pycocotools': every segment's string comes from one pass over the
 id map right after ``prob_to_segments``, and only the strings come to the host, not the id map.  The writer builds the
 same JSON entries from them, with no per-segment pixel work and no pycocotools.
+
+With ``jpeg_decoder='device'`` (or ``DEVA_B200_JPEG_DECODER=device``) an overlay given as ``path_to_image`` (no
+``image_np``) is blended on the device too: ``save_mask`` reads the file, and when it is a device-eligible JPEG
+(deva/utils/jpeg_decode.py) of the output size it decodes it on the current stream and feeds it to
+``prob_to_segments(frame=...)``, as it does with ``image_np``.  Whether the device accepted the file is known only to the
+writer, through a status downloaded with the frame's other copies; on a nonzero status the writer makes exactly what
+the Pillow path makes - Pillow's decode and the host blend - from the frame's device id map and RGB id image, which the
+queued frame keeps referenced and downloads only then.  A file that cannot be read, does not parse or has another size
+takes the Pillow path as before.
 """
 import copy
 import os
@@ -36,6 +45,8 @@ import torch
 from PIL import Image
 
 from deva.inference.frame_io import prob_to_ids, prob_to_segments
+from deva.utils import jpeg_decode
+from deva.utils.device_decode import read_bytes
 from deva.utils.device_download import Pending, write
 from deva.utils.jpeg_encode import encode_jpeg_async, host_bytes as jpeg_host_bytes
 from deva.utils.jpeg_encode import resolve_encoder as resolve_jpeg_encoder
@@ -50,15 +61,17 @@ RING_SIZE = QUEUE_SIZE + 2  # the queued frames, the one the writer holds and th
 class ResultSaver:
     def __init__(self, output_root: str, video_name: str, *, dataset: str, object_manager, palette=None,
                  png_encoder: Optional[str] = None, jpeg_encoder: Optional[str] = None,
-                 rle_encoder: Optional[str] = None):
+                 rle_encoder: Optional[str] = None, jpeg_decoder: Optional[str] = None):
         """png_encoder: 'pil' (Pillow on the writer thread) or 'device'; None reads DEVA_B200_PNG_ENCODER (default
         'pil').  jpeg_encoder: the same for the overlay JPEG; None reads DEVA_B200_JPEG_ENCODER (default 'pil').
         rle_encoder: 'pycocotools' (on the writer thread) or 'device' for burst's RLE; None reads DEVA_B200_RLE_ENCODER
-        (default 'pycocotools')."""
+        (default 'pycocotools').  jpeg_decoder: 'pil' (Pillow on the writer thread) or 'device' for an overlay's
+        ``path_to_image``; None reads DEVA_B200_JPEG_DECODER (default 'pil')."""
         self.output_root = output_root
         self.png_encoder = resolve_encoder(png_encoder)
         self.jpeg_encoder = resolve_jpeg_encoder(jpeg_encoder)
         self.rle_encoder = resolve_rle_encoder(rle_encoder)
+        self.jpeg_decoder = jpeg_decode.resolve_decoder(jpeg_decoder)
         self.video_name = video_name
         self.dataset = dataset.lower()
         self.palette = palette
@@ -129,12 +142,23 @@ class ResultSaver:
         if overlay and image_np is None and path_to_image is None:
             raise ValueError('Cannot visualize without image_np or path_to_image')
 
+        header = None
+        if overlay and image_np is None and path_to_image is not None and self.jpeg_decoder == 'device':
+            data = read_bytes(path_to_image)
+            header = None if data is None else jpeg_decode.parse(data)
+            if header is not None and header.shape != (*size, 3):
+                header = None
+
         slot = self.free_slots.get()  # blocks only while every slot is queued or being written
-        frame = None
+        frame = decoded = None
         if overlay and on_device:
             staged = _pinned(slot, 'image', image_np.shape, torch.uint8)
             staged.numpy()[...] = image_np
             frame = staged.to(prob.device, non_blocking=True)
+        elif header is not None:
+            frame, status, keep = jpeg_decode.decode_async(header)
+            decoded = Decoded(status, keep)
+            on_device = True  # the blend, its encoding and its downloads take the image_np path
         seg = prob_to_segments(prob, self.object_manager, size, index=save_the_mask and not long_id,
                                rgb=save_the_mask and long_id, frame=frame,
                                stats=self.json_style is not None or self.visualize, remap=self.need_remapping)
@@ -169,6 +193,12 @@ class ResultSaver:
             if rle is None or (overlay and not on_device):  # encoded RLE strings replace the id map's download
                 host['ids'] = _pinned(slot, 'ids', ids.shape, ids.dtype)
                 host['ids'].copy_(ids, non_blocking=True)
+        if decoded is not None:
+            # what a declined file's host blend needs, kept on the device and downloaded only then
+            lut = torch.tensor(seg.lut, dtype=torch.int32).pin_memory().to(prob.device, non_blocking=True)
+            decoded.ids, decoded.rgb, decoded.frame = prob_to_ids(prob, size=size, lut=lut), seg.rgb, frame
+            host['jpeg_status'] = _pinned(slot, 'jpeg_status', (1, ), torch.int32)
+            host['jpeg_status'].copy_(decoded.status, non_blocking=True)
         done = torch.cuda.Event()
         done.record()
 
@@ -182,6 +212,7 @@ class ResultSaver:
             frame_name=frame_name,
             save_the_mask=save_the_mask,
             image_np=None if on_device else image_np,
+            decoded=decoded,
             prompts=prompts,
             path_to_image=path_to_image,
             all_obj_ids=[int(o.id) for o in self.object_manager.obj_to_tmp_id],
@@ -206,6 +237,17 @@ def _pinned(slot: Dict[str, torch.Tensor], name: str, shape, dtype) -> torch.Ten
 
 
 @dataclass
+class Decoded:
+    """A ``path_to_image`` JPEG decoded on the device: its status, and what stays referenced until the writer is done -
+    the decode's buffers, the frame, and the id map and RGB id image a declined file's host blend downloads."""
+    status: torch.Tensor
+    keep: object
+    ids: Optional[torch.Tensor] = None
+    rgb: Optional[torch.Tensor] = None
+    frame: Optional[torch.Tensor] = None
+
+
+@dataclass
 class ResultArgs:
     saver: ResultSaver
     slot: Dict[str, torch.Tensor]  # pinned ring slot, returned to saver.free_slots when written
@@ -223,6 +265,7 @@ class ResultArgs:
     png: Optional[Pending] = None  # the id image's PNG, encoded on the device
     jpeg: Optional[Pending] = None  # the overlay's JPEG, encoded on the device
     rle: Optional[Pending] = None  # burst's RLE of every entry of segments_info, encoded on the device
+    decoded: Optional[Decoded] = None  # path_to_image decoded on the device
 
 
 def save_result(queue: Queue):
@@ -295,18 +338,22 @@ def _write(args: ResultArgs):
 
     if not (saver.visualize and args.long_id):
         return
-    if args.jpeg is not None:
+    # a path_to_image the device declined: the device's overlay (and its JPEG) are discarded for Pillow's path
+    declined = args.decoded is not None and int(host['jpeg_status'][0]) != 0
+    if args.jpeg is not None and not declined:
         write(args.jpeg, _path(saver, saver.visualize_postfix, frame_name[:-4] + '.jpg'))
         return
-    if 'overlay' in host:
+    if 'overlay' in host and not declined:
         blend = host['overlay'].numpy()
     else:
         image_np = args.image_np
         if image_np is None:
             image_np = np.array(Image.open(args.path_to_image))
+        ids = args.decoded.ids.cpu().numpy() if declined else host['ids'].numpy()
+        rgb = host['rgb'].numpy() if 'rgb' in host else args.decoded.rgb.cpu().numpy()
         # the reference's blend: alpha = 1 where the id is 0, else 0.5
-        alpha = (host['ids'].numpy() == 0).astype(np.float32)[:, :, None] * 0.5 + 0.5
-        blend = (image_np * alpha + host['rgb'].numpy() * (1 - alpha)).astype(np.uint8)
+        alpha = (ids == 0).astype(np.float32)[:, :, None] * 0.5 + 0.5
+        blend = (image_np * alpha + rgb * (1 - alpha)).astype(np.uint8)
 
     if args.prompts is not None and len(segments_info) > 0:
         import supervision as sv

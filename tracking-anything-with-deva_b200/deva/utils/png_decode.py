@@ -23,7 +23,6 @@ Files go to the device in batches of at most ``BUDGET`` decoded bytes: one pinne
 descriptors and streams, one launch, and one host synchronisation to read the statuses.  Importing this module does
 not initialise CUDA.
 """
-import io
 import struct
 import zlib
 from typing import List, NamedTuple, Optional
@@ -31,7 +30,7 @@ from typing import List, NamedTuple, Optional
 import numpy as np
 import torch
 
-from deva.utils import device_download
+from deva.utils import device_decode, device_download
 
 DECODERS = ('pil', 'device')
 ENV = 'DEVA_B200_PNG_DECODER'
@@ -178,35 +177,13 @@ def decode_batch(files, device=None):
     return results
 
 
-def _pillow(source) -> np.ndarray:
-    from PIL import Image
-    return np.asarray(Image.open(io.BytesIO(source) if isinstance(source, (bytes, bytearray, memoryview)) else source))
-
-
-def read_bytes(source):
-    """The bytes of a path or bytes source; None when a path cannot be read (Pillow then raises its own error)."""
-    if isinstance(source, (bytes, bytearray, memoryview)):
-        return bytes(source)
-    try:
-        with open(source, 'rb') as f:
-            return f.read()
-    except OSError:
-        return None
+read_bytes = device_decode.read_bytes
 
 
 def batches(headers, budget=BUDGET):
     """Consecutive index ranges [a, b) of files whose decoded bytes (arrays and filtered streams) stay within budget;
     a file over the budget is a batch of its own.  headers: Header or None per file."""
-    out, a, used = [], 0, 0
-    for i, hd in enumerate(headers):
-        n = 0 if hd is None else 2 * hd.nbytes + hd.h
-        if i > a and used + n > budget:
-            out.append((a, i))
-            a, used = i, 0
-        used += n
-    if a < len(headers):
-        out.append((a, len(headers)))
-    return out
+    return device_decode.batches([0 if hd is None else 2 * hd.nbytes + hd.h for hd in headers], budget)
 
 
 def decode_results(sources, device=None, budget=BUDGET, datas=None) -> List[object]:
@@ -214,30 +191,14 @@ def decode_results(sources, device=None, budget=BUDGET, datas=None) -> List[obje
     Pillow raises for it.  datas: the sources' bytes when already read (None for an unreadable path)."""
     datas = [read_bytes(s) for s in sources] if datas is None else datas
     headers = [None if d is None else parse(d) for d in datas]
-    results = []
-    for a, b in batches(headers, budget):
-        for k, (st, t) in enumerate(decode_batch(list(zip(datas[a:b], headers[a:b])), device), a):
-            if st == 0:
-                results.append(t)
-                continue
-            try:
-                arr = _pillow(sources[k])
-            except Exception as e:  # noqa: BLE001  (Pillow's own error is the result)
-                results.append(e)
-                continue
-            up = device_download.upload(arr if arr.flags.writeable else arr.copy())  # Pillow's arrays are read-only
-            results.append(up if device is None else up.to(device))
-    return results
+    costs = [0 if hd is None else 2 * hd.nbytes + hd.h for hd in headers]
+    return device_decode.decode_results(sources, datas, headers, costs, decode_batch, device, budget)
 
 
 def decode_pngs(sources) -> List[torch.Tensor]:
     """The CUDA tensors of ``np.asarray(Image.open(s))`` for every path or bytes ``s``; raises the first file's error
     that Pillow would raise."""
-    out = decode_results(sources)
-    for r in out:
-        if isinstance(r, BaseException):
-            raise r
-    return out
+    return device_decode.raise_first(decode_results(sources))
 
 
 def decode_png(source) -> torch.Tensor:
