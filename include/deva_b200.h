@@ -27,7 +27,9 @@
 extern "C" {
 #endif
 
-/* v25: deva_b200_jpeg_decode_workspace_bytes and deva_b200_jpeg_decode (baseline JPEG files decoded on the device).
+/* v26: deva_b200_pil_resample_u8 and deva_b200_mask_nearest_ids (the dataset readers' soft masks and detection masks
+ * resized on the device).
+ * v25: deva_b200_jpeg_decode_workspace_bytes and deva_b200_jpeg_decode (baseline JPEG files decoded on the device).
  * v24: deva_b200_png_decode_workspace_bytes and deva_b200_png_decode (the post-processing passes' PNGs decoded on the
  * device).
  * v23: deva_b200_rle_bound, deva_b200_rle_workspace_bytes and deva_b200_rle_encode (BURST's per-segment COCO RLE encoded
@@ -47,7 +49,7 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 25
+#define DEVA_B200_ABI_VERSION 26
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -309,6 +311,23 @@ DEVA_B200_API int deva_b200_ingest_rgb8_resize(const uint8_t* src, int h, int w,
  * (video_reader.py:159-161), then eval_vos.py:162-164's flip. */
 DEVA_B200_API int deva_b200_mask_nearest(const uint8_t* src, int h, int w, int out_h, int out_w, const int32_t* x_idx,
                                          const int32_t* y_idx, int flip, int64_t* dst, deva_stream_t stream);
+/* Mask u8 [h, w, channels] (channels 1 or 3) -> int32 [out_h, out_w] through the same gather as deva_b200_mask_nearest:
+ * one channel gives the index, three give the RGB id r + 256 g + 65536 b.  With PIL's NEAREST index maps this is the
+ * detection reader's Resize(NEAREST) of a P / L / RGB mask and its np.array(..., dtype=np.int32) id map
+ * (detection_video_reader.py:99-106). */
+DEVA_B200_API int deva_b200_mask_nearest_ids(const uint8_t* src, int channels, int h, int w, int out_h, int out_w,
+                                             const int32_t* x_idx, const int32_t* y_idx, int flip, int32_t* dst,
+                                             deva_stream_t stream);
+/* Pillow's Image.resize((out_w, out_h), BILINEAR) of k 8-bit one-channel planes src u8 [k, h, w], written as float32
+ * v / 255 into dst [k, out_h, out_w] (the reader's soft mask, video_reader.py:188-191).  Per axis, bounds int32
+ * [n_out, 2] (first input index, taps) and coef int32 [n_out, taps] are libImaging's precompute_coeffs and
+ * normalize_coeffs_8bpc (22-bit fixed point); the horizontal pass runs first and rounds to u8 in scratch u8
+ * [k, h, out_w], then the vertical pass.  A pass whose axis keeps its size is skipped (its tables may be NULL); scratch
+ * is needed only when both run. */
+DEVA_B200_API int deva_b200_pil_resample_u8(const uint8_t* src, int k, int h, int w, int out_h, int out_w,
+                                            const int32_t* x_bounds, const int32_t* x_coef, int x_taps,
+                                            const int32_t* y_bounds, const int32_t* y_coef, int y_taps, uint8_t* scratch,
+                                            float* dst, deva_stream_t stream);
 /* Driver post-step (evaluation/eval_vos.py:169-181) in one pass: optional bilinear resize (align_corners=False) of
  * prob fp32 [c, h, w] to [out_h, out_w], optional horizontal flip, argmax over channels (first maximum wins),
  * temporary-id -> object-id remap through lut int32 [c] (lut[0] = 0).  Writes out_u8 [out_h, out_w] and/or

@@ -1061,14 +1061,75 @@ resize_cols_kernel(const float* __restrict__ tmp, int h, int out_h, int out_w, c
   dst[c * plane + (long long)oy * out_w + (flip ? out_w - 1 - ox : ox)] = a;
 }
 
-// Index mask u8 [h, w] -> int64 [out_h, out_w] by row / column gather (nearest), optionally flipped after the resize.
+// Index mask u8 [h, w, C] -> Out [out_h, out_w] by row / column gather (nearest), optionally flipped after the resize.
+// One channel is the index itself; three are an RGB id r + 256 g + 65536 b.
+template <int C, typename Out>
 __global__ void __launch_bounds__(256)
 mask_gather_kernel(const unsigned char* __restrict__ src, int w, int out_h, int out_w, const int* __restrict__ x_idx,
-                   const int* __restrict__ y_idx, int flip, long long* __restrict__ dst) {
+                   const int* __restrict__ y_idx, int flip, Out* __restrict__ dst) {
+  static_assert(C == 1 || C == 3, "one index or three RGB channels");
   const long long i = blockIdx.x * 256ll + threadIdx.x;
   if (i >= (long long)out_h * out_w) return;
   const int oy = (int)(i / out_w), ox = (int)(i - (long long)oy * out_w);
-  dst[i] = src[(long long)y_idx[oy] * w + x_idx[flip ? out_w - 1 - ox : ox]];
+  const unsigned char* p = src + ((long long)y_idx[oy] * w + x_idx[flip ? out_w - 1 - ox : ox]) * C;
+  if constexpr (C == 1) {
+    dst[i] = p[0];
+  } else {
+    dst[i] = (Out)p[0] + 256 * (Out)p[1] + 65536 * (Out)p[2];
+  }
+}
+
+// Pillow's 8-bit two-pass BILINEAR resample (libImaging Resample.c, ImagingResampleHorizontal_8bpc /
+// ImagingResampleVertical_8bpc): per output pixel a window [lo, lo + n) of the input axis, 22-bit fixed-point
+// coefficients, a half added before the sum and the result shifted back and clamped (clip8).
+constexpr int kPilPrecision = 22;
+
+__device__ __forceinline__ int pil_clip8(int ss) {
+  ss >>= kPilPrecision;
+  return ss < 0 ? 0 : (ss > 255 ? 255 : ss);
+}
+__device__ __forceinline__ void pil_store(unsigned char* p, int v) { *p = (unsigned char)v; }
+// torch.FloatTensor(np.array(mask)) / 255: one correctly rounded float32 division
+__device__ __forceinline__ void pil_store(float* p, int v) { *p = __fdiv_rn((float)v, 255.f); }
+
+// Horizontal pass: src u8 [k, h, w] -> dst [k, h, out_w].  bounds int32 [out_w, 2] (first tap, taps), coef int32
+// [out_w, taps].  Without bounds the axis keeps its size and the pass copies (the resize skips it).
+template <typename Out>
+__global__ void __launch_bounds__(256)
+pil_resample_rows_kernel(const unsigned char* __restrict__ src, int k, int h, int w, int out_w,
+                         const int* __restrict__ bounds, const int* __restrict__ coef, int taps, Out* __restrict__ dst) {
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= (long long)k * h * out_w) return;
+  const long long row = i / out_w;
+  const int ox = (int)(i - row * out_w);
+  const unsigned char* s = src + row * w;
+  if (!bounds) {
+    pil_store(dst + i, s[ox]);
+    return;
+  }
+  const int lo = bounds[2 * ox], n = bounds[2 * ox + 1];
+  const int* c = coef + (long long)ox * taps;
+  int ss = 1 << (kPilPrecision - 1);
+  for (int j = 0; j < n; ++j) ss += (int)s[lo + j] * c[j];
+  pil_store(dst + i, pil_clip8(ss));
+}
+
+// Vertical pass: src u8 [k, h, out_w] -> dst float [k, out_h, out_w] (v / 255), with the same tables along y.
+__global__ void __launch_bounds__(256)
+pil_resample_cols_kernel(const unsigned char* __restrict__ src, int k, int h, int out_h, int out_w,
+                         const int* __restrict__ bounds, const int* __restrict__ coef, int taps, float* __restrict__ dst) {
+  const long long plane = (long long)out_h * out_w;
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= k * plane) return;
+  const int p = (int)(i / plane);
+  const long long r = i - p * plane;
+  const int oy = (int)(r / out_w), ox = (int)(r - (long long)oy * out_w);
+  const int lo = bounds[2 * oy], n = bounds[2 * oy + 1];
+  const int* c = coef + (long long)oy * taps;
+  const unsigned char* s = src + (long long)p * h * out_w + ox;
+  int ss = 1 << (kPilPrecision - 1);
+  for (int j = 0; j < n; ++j) ss += (int)s[(long long)(lo + j) * out_w] * c[j];
+  pil_store(dst + i, pil_clip8(ss));
 }
 
 // ---------------------------------------------------------------- detector masks -> detection id map
@@ -1247,8 +1308,51 @@ DEVA_B200_API int deva_b200_mask_nearest(const uint8_t* src, int h, int w, int o
                                          const int32_t* y_idx, int flip, int64_t* dst, deva_stream_t stream) {
   B200_REQUIRE(h > 0 && w > 0 && out_h > 0 && out_w > 0 && x_idx && y_idx, "mask_nearest: bad arguments");
   const long long n = (long long)out_h * out_w;
-  ew::mask_gather_kernel<<<(unsigned)ceil_div(n, 256ll), 256, 0, S(stream)>>>(src, w, out_h, out_w, x_idx, y_idx, flip,
-                                                                             reinterpret_cast<long long*>(dst));
+  ew::mask_gather_kernel<1, long long><<<(unsigned)ceil_div(n, 256ll), 256, 0, S(stream)>>>(
+      src, w, out_h, out_w, x_idx, y_idx, flip, reinterpret_cast<long long*>(dst));
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+DEVA_B200_API int deva_b200_mask_nearest_ids(const uint8_t* src, int channels, int h, int w, int out_h, int out_w,
+                                             const int32_t* x_idx, const int32_t* y_idx, int flip, int32_t* dst,
+                                             deva_stream_t stream) {
+  B200_REQUIRE(src && dst && (channels == 1 || channels == 3) && h > 0 && w > 0 && out_h > 0 && out_w > 0 && x_idx &&
+               y_idx, "mask_nearest_ids: bad arguments");
+  const long long n = (long long)out_h * out_w;
+  const unsigned blocks = (unsigned)ceil_div(n, 256ll);
+  if (channels == 1)
+    ew::mask_gather_kernel<1, int32_t><<<blocks, 256, 0, S(stream)>>>(src, w, out_h, out_w, x_idx, y_idx, flip, dst);
+  else
+    ew::mask_gather_kernel<3, int32_t><<<blocks, 256, 0, S(stream)>>>(src, w, out_h, out_w, x_idx, y_idx, flip, dst);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+DEVA_B200_API int deva_b200_pil_resample_u8(const uint8_t* src, int k, int h, int w, int out_h, int out_w,
+                                            const int32_t* x_bounds, const int32_t* x_coef, int x_taps,
+                                            const int32_t* y_bounds, const int32_t* y_coef, int y_taps, uint8_t* scratch,
+                                            float* dst, deva_stream_t stream) {
+  const bool horiz = out_w != w, vert = out_h != h;
+  B200_REQUIRE(src && dst && k > 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, "pil_resample_u8: bad arguments");
+  B200_REQUIRE(!horiz || (x_bounds && x_coef && x_taps > 0), "pil_resample_u8: the horizontal pass needs its tables");
+  B200_REQUIRE(!vert || (y_bounds && y_coef && y_taps > 0), "pil_resample_u8: the vertical pass needs its tables");
+  B200_REQUIRE(!(horiz && vert) || scratch, "pil_resample_u8: two passes need the scratch plane");
+  const cudaStream_t s = S(stream);
+  const long long n1 = (long long)k * h * out_w, n2 = (long long)k * out_h * out_w;
+  if (!vert) {  // one pass (or a copy) straight to float
+    ew::pil_resample_rows_kernel<float><<<(unsigned)ceil_div(n1, 256ll), 256, 0, s>>>(
+        src, k, h, w, out_w, horiz ? x_bounds : nullptr, x_coef, x_taps, dst);
+    B200_LAUNCH_CHECK();
+    return 0;
+  }
+  const uint8_t* mid = src;
+  if (horiz) {
+    ew::pil_resample_rows_kernel<unsigned char><<<(unsigned)ceil_div(n1, 256ll), 256, 0, s>>>(
+        src, k, h, w, out_w, x_bounds, x_coef, x_taps, scratch);
+    B200_LAUNCH_CHECK();
+    mid = scratch;
+  }
+  ew::pil_resample_cols_kernel<<<(unsigned)ceil_div(n2, 256ll), 256, 0, s>>>(mid, k, h, out_h, out_w, y_bounds, y_coef,
+                                                                             y_taps, dst);
   B200_LAUNCH_CHECK();
   return 0;
 }

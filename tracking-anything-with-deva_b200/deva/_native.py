@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 25
+ABI_VERSION = 26
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -95,6 +95,10 @@ _SIGNATURES = {
                                              ctypes.POINTER(ctypes.c_float), c_void_p]),
     'deva_b200_mask_nearest': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
                                        c_void_p]),
+    'deva_b200_mask_nearest_ids': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                           c_void_p, c_void_p]),
+    'deva_b200_pil_resample_u8': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                          c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     'deva_b200_prob_to_ids': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                       c_void_p]),
     'deva_b200_prob_to_segments': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
@@ -380,6 +384,18 @@ def ingest_rgb8_resize(src, h, w, out_h, out_w, x_idx, x_w, y_idx, y_w, scratch,
 def mask_nearest(src, h, w, out_h, out_w, x_idx, y_idx, flip, dst):
     _check(lib().deva_b200_mask_nearest(_ptr(src), h, w, out_h, out_w, _ptr(x_idx), _ptr(y_idx), int(flip), _ptr(dst),
                                         _stream()), 'mask_nearest')
+
+
+def mask_nearest_ids(src, channels, h, w, out_h, out_w, x_idx, y_idx, flip, dst):
+    _check(lib().deva_b200_mask_nearest_ids(_ptr(src), channels, h, w, out_h, out_w, _ptr(x_idx), _ptr(y_idx), int(flip),
+                                            _ptr(dst), _stream()), 'mask_nearest_ids')
+
+
+def pil_resample_u8(src, k, h, w, out_h, out_w, x_bounds, x_coef, y_bounds, y_coef, scratch, dst):
+    _check(lib().deva_b200_pil_resample_u8(_ptr(src), k, h, w, out_h, out_w, _p(x_bounds), _p(x_coef),
+                                           0 if x_coef is None else x_coef.shape[1], _p(y_bounds), _p(y_coef),
+                                           0 if y_coef is None else y_coef.shape[1], _p(scratch), _ptr(_f32(dst)),
+                                           _stream()), 'pil_resample_u8')
 
 
 def prob_to_ids(prob, c, h, w, out_h, out_w, flip, lut, out_u8, out_i64):

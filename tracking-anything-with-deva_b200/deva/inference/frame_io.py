@@ -91,6 +91,29 @@ def pil_nearest_map(n_in: int, n_out: int) -> np.ndarray:
     return out
 
 
+def pil_bilinear_coeffs(n_in: int, n_out: int) -> Tuple[np.ndarray, np.ndarray]:
+    """int32 [n_out, 2] (first input index, taps) and int32 [n_out, taps] 22-bit fixed-point coefficients of Pillow's
+    8-bit BILINEAR resample along one axis (libImaging Resample.c: precompute_coeffs, then normalize_coeffs_8bpc): a
+    triangle whose support is scaled by the downscale factor, double arithmetic, weights normalised per output pixel
+    and rounded half away from zero.  Unused taps are 0."""
+    scale = float(np.float32(n_in)) / n_out
+    filterscale = max(scale, 1.0)
+    support = filterscale
+    taps = int(np.ceil(support)) * 2 + 1
+    center = (np.arange(n_out, dtype=np.float64) + 0.5) * scale
+    lo = np.maximum((center - support + 0.5).astype(np.int64), 0)
+    n = np.minimum((center + support + 0.5).astype(np.int64), n_in) - lo
+    x = np.abs(((lo[:, None] + np.arange(taps)).astype(np.float64) - center[:, None] + 0.5) * (1.0 / filterscale))
+    wt = np.where(x < 1.0, 1.0 - x, 0.0)
+    wt[np.arange(taps)[None, :] >= n[:, None]] = 0.0
+    total = np.zeros(n_out)
+    for j in range(taps):  # Pillow sums the weights in tap order
+        total = total + wt[:, j]
+    wt = np.where(total[:, None] != 0.0, wt / np.where(total == 0.0, 1.0, total)[:, None], wt)
+    fixed = np.trunc(wt * (1 << 22) + np.where(wt < 0, -0.5, 0.5)).astype(np.int32)
+    return np.stack([lo, n], 1).astype(np.int32), fixed
+
+
 _TABLES: Dict[tuple, Tuple[torch.Tensor, ...]] = {}
 
 
@@ -100,6 +123,8 @@ def _axis_table(kind: str, n_in: int, n_out: int, device) -> Tuple[torch.Tensor,
     if key not in _TABLES:
         if kind == 'nearest':
             arrays = (pil_nearest_map(n_in, n_out),)
+        elif kind == 'pil_bilinear':
+            arrays = pil_bilinear_coeffs(n_in, n_out)
         else:
             arrays = (antialias_taps if kind == 'antialias' else bilinear_taps)(n_in, n_out)
         _TABLES[key] = tuple(torch.from_numpy(a).to(device) for a in arrays)
@@ -151,6 +176,44 @@ def mask_from_index8(mask: torch.Tensor, size: Optional[int] = None, *, flip: bo
     (x_idx,), (y_idx,) = _axis_table('nearest', w, ow, mask.device), _axis_table('nearest', h, oh, mask.device)
     out = torch.empty(oh, ow, dtype=torch.long, device=mask.device)
     nat.mask_nearest(mask, h, w, oh, ow, x_idx, y_idx, flip, out)
+    return out
+
+
+def mask_ids_from_u8(mask: torch.Tensor, size: Optional[int] = None, *, device: Optional[torch.device] = None,
+                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """uint8 [H, W] index mask or [H, W, 3] RGB mask (host or device) -> int32 [H', W'] ids on the device: the
+    detection reader's ``Resize(size, NEAREST)`` (PIL's nearest, output size as torchvision's ``Resize(size)``), then
+    the index itself, or ``r + 256 g + 65536 b`` for RGB.  ``out`` (int32 [H', W'] on the device) receives the ids."""
+    assert mask.dtype == torch.uint8 and (mask.dim() == 2 or (mask.dim() == 3 and mask.shape[2] == 3)), mask.shape
+    assert size is None or size > 0, size
+    mask = _to_device(mask, device)
+    h, w = mask.shape[:2]
+    oh, ow = (h, w) if size is None else reader_size(h, w, size)
+    (x_idx,), (y_idx,) = _axis_table('nearest', w, ow, mask.device), _axis_table('nearest', h, oh, mask.device)
+    if out is None:
+        out = torch.empty(oh, ow, dtype=torch.int32, device=mask.device)
+    assert out.dtype == torch.int32 and out.is_contiguous() and tuple(out.shape) == (oh, ow), (out.dtype, out.shape)
+    nat.mask_nearest_ids(mask, 1 if mask.dim() == 2 else 3, h, w, oh, ow, x_idx, y_idx, False, out)
+    return out
+
+
+def soft_from_u8(planes: torch.Tensor, size: Optional[int] = None, *, device: Optional[torch.device] = None,
+                 out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """uint8 [K, H, W] soft-mask planes (host or device) -> float32 [K, H', W'] on the device: per plane the reader's
+    ``Resize(size, BILINEAR)`` of an L image (Pillow's 8-bit resample, bit for bit; output size as torchvision's
+    ``Resize(size)``), then ``torch.FloatTensor(np.array(mask)) / 255``.  One launch per pass for all K planes."""
+    assert planes.dtype == torch.uint8 and planes.dim() == 3 and planes.shape[0] > 0, (planes.dtype, planes.shape)
+    assert size is None or size > 0, size
+    planes = _to_device(planes, device)
+    k, h, w = planes.shape
+    oh, ow = (h, w) if size is None else reader_size(h, w, size)
+    if out is None:
+        out = torch.empty(k, oh, ow, dtype=torch.float32, device=planes.device)
+    assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (k, oh, ow), (out.dtype, out.shape)
+    xb, xc = _axis_table('pil_bilinear', w, ow, planes.device) if ow != w else (None, None)
+    yb, yc = _axis_table('pil_bilinear', h, oh, planes.device) if oh != h else (None, None)
+    scratch = torch.empty(k, h, ow, dtype=torch.uint8, device=planes.device) if ow != w and oh != h else None
+    nat.pil_resample_u8(planes, k, h, w, oh, ow, xb, xc, yb, yc, scratch, out)
     return out
 
 

@@ -20,7 +20,7 @@ matching Adler-32 and nothing after it, and every row's filter type is at most 4
 status sends the file to Pillow.
 
 Files go to the device in batches of at most ``BUDGET`` decoded bytes: one pinned staging copy of the batch's
-descriptors and streams, one launch, and one host synchronisation to read the statuses.  Importing this module does
+descriptors and streams, one launch (``enqueue``), and one host synchronisation to read the statuses.  Importing this module does
 not initialise CUDA.
 """
 import struct
@@ -137,20 +137,17 @@ def _aligned(n):
     return (n + _ALIGN - 1) // _ALIGN * _ALIGN
 
 
-def decode_batch(files, device=None):
-    """One device launch for ``files``, a list of (file bytes, Header or None).  -> [(status, tensor)]: for a file
-    with no Header (None, None); else the device's status and, when it is 0, the decoded CUDA uint8 tensor (a view of
-    one buffer shared by the batch).  Synchronises the host once, to read the statuses."""
+def enqueue(files, device=None):
+    """Enqueues one device launch for ``files``, a list of (file bytes, Header), on the current stream without
+    synchronising the host.  -> (status int32 CUDA tensor [n], [CUDA uint8 tensor per file], keep): a file's tensor
+    (a view of one buffer shared by the batch) holds Pillow's array once its status is 0; keep (the launch's device
+    buffers) must stay referenced until the work completes."""
     from deva import _native
     device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
-    todo = [(i, data, hd) for i, (data, hd) in enumerate(files) if hd is not None]
-    results = [(None, None)] * len(files)
-    if not todo:
-        return results
-    streams = [hd.stream(data) for _, data, hd in todo]
-    desc = np.zeros((len(todo), _native.PNG_DESC_FIELDS), np.int64)
+    streams = [hd.stream(data) for data, hd in files]
+    desc = np.zeros((len(files), _native.PNG_DESC_FIELDS), np.int64)
     s_at = out_at = work_at = 0
-    for k, ((_, _, hd), st) in enumerate(zip(todo, streams)):
+    for k, ((_, hd), st) in enumerate(zip(files, streams)):
         desc[k] = (s_at, len(st), hd.h, hd.w, hd.colour_type, hd.bits, out_at, work_at)
         s_at += len(st)
         out_at += _aligned(hd.nbytes)
@@ -167,13 +164,24 @@ def decode_batch(files, device=None):
     dev[:head + s_at].copy_(host, non_blocking=True)
     out = torch.empty(max(out_at, 1), dtype=torch.uint8, device=device)
     work = torch.empty(max(work_at, 1), dtype=torch.uint8, device=device)
-    status = torch.empty(len(todo), dtype=torch.int32, device=device)
+    status = torch.empty(len(files), dtype=torch.int32, device=device)
     _native.png_decode(dev[head:head + s_at] if s_at else dev[head:head + 1], dev[:head].view(torch.int64).view(
-        len(todo), _native.PNG_DESC_FIELDS), out, work, status)
-    for k, st in enumerate(status.tolist()):  # the batch's one synchronisation
-        i, _, hd = todo[k]
-        o = int(desc[k, 6])
-        results[i] = (st, out[o:o + hd.nbytes].view(hd.shape) if st == 0 else None)
+        len(files), _native.PNG_DESC_FIELDS), out, work, status)
+    arrays = [out[int(desc[k, 6]):int(desc[k, 6]) + hd.nbytes].view(hd.shape) for k, (_, hd) in enumerate(files)]
+    return status, arrays, (dev, out, work)
+
+
+def decode_batch(files, device=None):
+    """One device launch for ``files``, a list of (file bytes, Header or None).  -> [(status, tensor)]: for a file
+    with no Header (None, None); else the device's status and, when it is 0, the decoded CUDA uint8 tensor (a view of
+    one buffer shared by the batch).  Synchronises the host once, to read the statuses."""
+    todo = [(i, data, hd) for i, (data, hd) in enumerate(files) if hd is not None]
+    results = [(None, None)] * len(files)
+    if not todo:
+        return results
+    status, arrays, _ = enqueue([(data, hd) for _, data, hd in todo], device)
+    for (i, _, _), st, t in zip(todo, status.tolist(), arrays):  # the batch's one synchronisation
+        results[i] = (st, t if st == 0 else None)
     return results
 
 
