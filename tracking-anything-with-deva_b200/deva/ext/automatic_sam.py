@@ -9,7 +9,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from deva.ext.detector_masks import output_size, scored_id_map
+from deva.ext.detector_masks import host_image, output_size, scored_id_map
 from deva.inference.object_info import ObjectInfo
 
 
@@ -50,10 +50,12 @@ def _positive_points(config: Dict, forward_mask: torch.Tensor, device) -> np.nda
 
 def auto_segment(config: Dict, auto_sam, image: np.ndarray, forward_mask: Optional[torch.Tensor], min_side: int,
                  suppress_small_mask: bool) -> (torch.Tensor, List[ObjectInfo]):
-    """image: H*W*3 uint8 (0~255); forward_mask: H*W, or None.
+    """image: H*W*3 uint8 (0~255), a numpy array or a CUDA tensor; forward_mask: H*W, or None.
 
     Returns the int64 id map at the working resolution (shorter side ``min_side``; the image size when min_side <= 0)
-    on the generator's device, and one ObjectInfo(id, score=predicted IoU) per segment."""
+    on the generator's device, and one ObjectInfo(id, score=predicted IoU) per segment.  SAM is given the host array:
+    a CUDA image is downloaded once into pinned memory, a host synchronisation on top of the one the id map needs."""
+    image = host_image(image)
     device = auto_sam.predictor.device
     h, w = image.shape[:2]
     new_h, new_w = output_size(h, w, min_side)

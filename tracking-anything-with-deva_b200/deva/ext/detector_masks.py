@@ -26,6 +26,17 @@ def _to_device(array: np.ndarray, device) -> torch.Tensor:
     return torch.from_numpy(np.ascontiguousarray(array)).pin_memory().to(device, non_blocking=True)
 
 
+def host_image(image):
+    """A detector's input image as the host array the reference passes it.  A CUDA uint8 tensor (a frame decoded on the
+    device) is downloaded into pinned memory: one host synchronisation.  Anything else is returned as it is."""
+    if not (isinstance(image, torch.Tensor) and image.is_cuda and image.dtype == torch.uint8):
+        return image
+    host = torch.empty(image.shape, dtype=torch.uint8, pin_memory=True)
+    host.copy_(image, non_blocking=True)
+    torch.cuda.current_stream(image.device).synchronize()
+    return host.numpy()
+
+
 def _map(slot: torch.Tensor, lut: np.ndarray) -> torch.Tensor:
     return torch.index_select(_to_device(lut, slot.device), 0, slot.view(-1)).view(slot.shape)
 

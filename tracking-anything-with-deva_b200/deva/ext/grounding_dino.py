@@ -9,7 +9,7 @@ from typing import Dict, List
 import numpy as np
 import torch
 
-from deva.ext.detector_masks import cover_id_map, output_size, stack_masks
+from deva.ext.detector_masks import cover_id_map, host_image, output_size, stack_masks
 from deva.inference.object_info import ObjectInfo
 
 
@@ -54,13 +54,16 @@ def get_grounding_dino_model(config: Dict, device: str):
 
 def segment_with_text(config: Dict, gd_model, sam, image: np.ndarray, prompts: List[str],
                       min_side: int) -> (torch.Tensor, List[ObjectInfo]):
-    """image: H*W*3 uint8 RGB (0~255); prompts: class names.
+    """image: H*W*3 uint8 RGB (0~255), a numpy array or a CUDA tensor; prompts: class names.
 
     Returns the int64 id map at the working resolution (shorter side ``min_side``; the image size when min_side <= 0)
-    on the detector's device, and one ObjectInfo(id, category_id=class id, score=confidence) per painted mask."""
+    on the detector's device, and one ObjectInfo(id, category_id=class id, score=confidence) per painted mask.  SAM and
+    Grounding-DINO are given the host array: a CUDA image is downloaded once into pinned memory, a host
+    synchronisation on top of the one the id map needs."""
     import cv2
     import torchvision
 
+    image = host_image(image)
     threshold = config['DINO_THRESHOLD']
     sam.set_image(image, image_format='RGB')
     detections = gd_model.predict_with_classes(image=cv2.cvtColor(image, cv2.COLOR_RGB2BGR), classes=prompts,

@@ -5,6 +5,11 @@ Item ``i`` is ``default_collate([reader[i]])`` (what ``DataLoader(reader, batch_
 ``data['rgb']`` and ``data['mask']`` are CUDA tensors on the current device, produced there: rgb bit for bit at the
 frame's own size and within 1e-6 when resized; masks, soft masks, ``valid_labels`` and every info field exactly equal.
 
+With the demos' ``SimpleVideoReader`` it replaces ``DataLoader(reader, batch_size=None, collate_fn=no_collate,
+num_workers=8)``: item ``i`` is ``(frame, im_path)`` where ``frame`` is the CUDA uint8 [H, W, 3] tensor equal to
+``torch.from_numpy(reader[i][0])``, neither collated nor normalised (the demos' processors hand the raw frame to the
+detectors and the overlay, and normalise it themselves through ``demo_utils.get_input_frame_for_deva``).
+
 Pipeline, for windows of ``prefetch // 2`` frames (at most ``prefetch`` frames are read ahead):
   * host threads run each frame's ``reader.plan(i)``, read its files and parse them (``jpeg_decode.parse``,
     ``png_decode.parse``; a ``size_dir`` shape is read from the file's header, without a decode);
@@ -34,6 +39,7 @@ from torch.utils.data import default_collate
 
 from deva.inference import frame_io
 from deva.inference.data.detection_video_reader import DetectionVideoReader
+from deva.inference.data.simple_video_reader import SimpleVideoReader
 from deva.inference.data.video_reader import (MASK_DETECTION, MASK_ID, MASK_SOFT, MASK_SOFT_MULTI, Plan,
                                               VideoReader)
 from deva.utils import device_decode, jpeg_decode, png_decode
@@ -90,6 +96,7 @@ class _Window:
     """One window's device work: per frame its outputs, and the pinned copy of the statuses read at hand-out."""
 
     def __init__(self, start, parsed, size, stream):
+        """size: the reader's working short side (< 0: the frame's own size; None: the raw uint8 frame)."""
         self.start, self.parsed = start, parsed
         self.out = [None] * len(parsed)
         self.keep = []
@@ -111,10 +118,10 @@ class _Window:
             for j, (k, _) in enumerate(files):
                 self.status_of[k].append(len(on) + j)
             hists = []
-            size_arg = None if size < 0 else size
+            size_arg = None if size is None or size < 0 else size
             for j, k in enumerate(on):
                 p = parsed[k]
-                rgb = frame_io.frame_from_rgb8(frames[j], size=size_arg, resize='reader')
+                rgb = frames[j] if size is None else frame_io.frame_from_rgb8(frames[j], size=size_arg, resize='reader')
                 mine = [masks[m] for m, (kk, _) in enumerate(files) if kk == k]
                 mask, hist = None, None
                 if mine and p.plan.mask_kind == MASK_ID:
@@ -149,17 +156,19 @@ class _Window:
 
 class DeviceLoader:
     """Iterates ``reader`` (this package's ``VideoReader`` or ``DetectionVideoReader``) like
-    ``DataLoader(reader, batch_size=1)``, with the frames and masks read on the device (see the module's docstring).
+    ``DataLoader(reader, batch_size=1)``, or a ``SimpleVideoReader`` like ``DataLoader(reader, batch_size=None,
+    collate_fn=no_collate)``, with the frames and masks read on the device (see the module's docstring).
     prefetch: frames read ahead of the one handed out; num_threads: host threads reading and parsing files (default:
     the host's cores, at most 8).  ``host_indices`` lists the items of the last pass the host read."""
 
     def __init__(self, reader, *, prefetch: int = 16, num_threads: Optional[int] = None):
-        if not isinstance(reader, (VideoReader, DetectionVideoReader)):
-            raise TypeError(f'DeviceLoader reads a deva.inference.data VideoReader or DetectionVideoReader, not '
-                            f'{type(reader).__name__}')
+        if not isinstance(reader, (VideoReader, DetectionVideoReader, SimpleVideoReader)):
+            raise TypeError(f'DeviceLoader reads a deva.inference.data VideoReader, DetectionVideoReader or '
+                            f'SimpleVideoReader, not {type(reader).__name__}')
         if prefetch < 1:
             raise ValueError(f'DeviceLoader: prefetch must be at least 1, got {prefetch}')
         self.reader = reader
+        self.raw = isinstance(reader, SimpleVideoReader)
         self.window = max(1, prefetch // 2)
         self.num_threads = num_threads or min(8, os.cpu_count() or 1)
         self.host_indices: List[int] = []
@@ -168,8 +177,11 @@ class DeviceLoader:
         return len(self.reader)
 
     def _host_item(self, i):
-        data = default_collate([self.reader[i]])
         dev = torch.device('cuda', torch.cuda.current_device())
+        if self.raw:
+            frame, im_path = self.reader[i]
+            return torch.from_numpy(frame).to(dev), im_path
+        data = default_collate([self.reader[i]])
         for key in ('rgb', 'mask'):
             if key in data:
                 data[key] = data[key].to(dev)
@@ -178,6 +190,11 @@ class DeviceLoader:
     def _device_item(self, win, k):
         p = win.parsed[k]
         rgb, mask, hist = win.out[k]
+        if self.raw:
+            consumer = torch.cuda.current_stream()
+            consumer.wait_event(win.ready)
+            rgb.record_stream(consumer)
+            return rgb, p.plan.image
         if p.plan.mask_kind == MASK_DETECTION:
             item = self.reader.assemble(p.plan, None, p.shape, mask, p.masks[0][1].mode == 'RGB' if p.masks else None)
         else:
@@ -209,7 +226,7 @@ class DeviceLoader:
                 return [pool.submit(_parse, self.reader, i) for i in range(s, min(n, s + self.window))]
 
             def enqueue(s, futures):
-                return _Window(s, [f.result() for f in futures], self.reader.size, stream)
+                return _Window(s, [f.result() for f in futures], None if self.raw else self.reader.size, stream)
 
             futures = {s: submit(s) for s in starts[:2]}
             pending = enqueue(starts[0], futures.pop(starts[0])) if starts else None

@@ -31,6 +31,11 @@ writer, through a status downloaded with the frame's other copies; on a nonzero 
 the Pillow path makes - Pillow's decode and the host blend - from the frame's device id map and RGB id image, which the
 queued frame keeps referenced and downloads only then.  A file that cannot be read, does not parse or has another size
 takes the Pillow path as before.
+
+``image_np`` may also be a CUDA uint8 [h, w, 3] tensor of the output size (a frame the demos read on the device): it is
+blended as it is, with no staging copy, and the queued frame keeps it referenced until its copies are done; everything
+after the blend is the numpy ``image_np`` path.  A CUDA ``image_np`` of another shape or dtype is copied to pinned memory
+with the frame's other downloads and the writer treats it as that numpy array.
 """
 import copy
 import os
@@ -139,6 +144,9 @@ class ResultSaver:
         long_id = self.object_manager.use_long_id
         overlay = save_the_mask and self.visualize and long_id
         on_device = (isinstance(image_np, np.ndarray) and image_np.dtype == np.uint8 and image_np.shape == (*size, 3))
+        cuda_image = isinstance(image_np, torch.Tensor) and image_np.is_cuda
+        if cuda_image:
+            on_device = image_np.dtype == torch.uint8 and tuple(image_np.shape) == (*size, 3)
         if overlay and image_np is None and path_to_image is None:
             raise ValueError('Cannot visualize without image_np or path_to_image')
 
@@ -151,7 +159,9 @@ class ResultSaver:
 
         slot = self.free_slots.get()  # blocks only while every slot is queued or being written
         frame = decoded = None
-        if overlay and on_device:
+        if overlay and on_device and cuda_image:
+            frame = image_np
+        elif overlay and on_device:
             staged = _pinned(slot, 'image', image_np.shape, torch.uint8)
             staged.numpy()[...] = image_np
             frame = staged.to(prob.device, non_blocking=True)
@@ -181,6 +191,9 @@ class ResultSaver:
             if t is not None:
                 host[name] = _pinned(slot, name, t.shape, t.dtype)
                 host[name].copy_(t, non_blocking=True)
+        if overlay and cuda_image and not on_device:  # the writer blends it as the numpy array the reference got
+            host['image_np'] = _pinned(slot, 'image_np', image_np.shape, image_np.dtype)
+            host['image_np'].copy_(image_np, non_blocking=True)
         segments_info = copy.deepcopy(self.object_manager.get_current_segments_info())
         rle = None
         if self.json_style == 'burst' or (overlay and not on_device):
@@ -211,7 +224,8 @@ class ResultSaver:
             long_id=long_id,
             frame_name=frame_name,
             save_the_mask=save_the_mask,
-            image_np=None if on_device else image_np,
+            image_np=None if on_device or cuda_image else image_np,
+            frame=frame if cuda_image else None,
             decoded=decoded,
             prompts=prompts,
             path_to_image=path_to_image,
@@ -266,6 +280,7 @@ class ResultArgs:
     jpeg: Optional[Pending] = None  # the overlay's JPEG, encoded on the device
     rle: Optional[Pending] = None  # burst's RLE of every entry of segments_info, encoded on the device
     decoded: Optional[Decoded] = None  # path_to_image decoded on the device
+    frame: Optional[torch.Tensor] = None  # a CUDA image_np blended as it is, referenced until the copies are done
 
 
 def save_result(queue: Queue):
@@ -347,6 +362,8 @@ def _write(args: ResultArgs):
         blend = host['overlay'].numpy()
     else:
         image_np = args.image_np
+        if image_np is None and 'image_np' in host:
+            image_np = host['image_np'].numpy()
         if image_np is None:
             image_np = np.array(Image.open(args.path_to_image))
         ids = args.decoded.ids.cpu().numpy() if declined else host['ids'].numpy()
