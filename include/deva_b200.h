@@ -27,7 +27,9 @@
 extern "C" {
 #endif
 
-/* v26: deva_b200_pil_resample_u8 and deva_b200_mask_nearest_ids (the dataset readers' soft masks and detection masks
+/* v27: deva_b200_conv2d takes flat spatial tiles, th = 0 and tw = 128 (stride 1, no out_pool4): 128 consecutive output
+ * pixels of one image in row-major order.
+ * v26: deva_b200_pil_resample_u8 and deva_b200_mask_nearest_ids (the dataset readers' soft masks and detection masks
  * resized on the device).
  * v25: deva_b200_jpeg_decode_workspace_bytes and deva_b200_jpeg_decode (baseline JPEG files decoded on the device).
  * v24: deva_b200_png_decode_workspace_bytes and deva_b200_png_decode (the post-processing passes' PNGs decoded on the
@@ -49,7 +51,7 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 26
+#define DEVA_B200_ABI_VERSION 27
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -202,7 +204,9 @@ typedef struct deva_b200_conv_desc {
   const void* w_packed; /* fp16 [cout_pad, kh*kw*cin_pad] */
   int32_t kh, kw, stride; /* 1x1 or 3x3, stride 1 or 2, padding kh/2 (nn.Conv2d semantics) */
   int32_t cout, cout_pad, nt; /* real / padded output channels, channel tile (multiple of 32, <= 256, divides cout_pad) */
-  int32_t th, tw;       /* spatial tile of the implicit GEMM, th*tw == 128 */
+  int32_t th, tw;       /* spatial tile of the implicit GEMM: a th x tw rectangle with th*tw == 128, or th = 0, tw = 128
+                         * for flat tiles (stride 1, no out_pool4): output pixels 128t .. 128t+127 of one image in
+                         * row-major order, so that no MMA row is spent on padding where no rectangle fits ho x wo */
   const float* bias;
   const void* res;      /* optional fp16 NHWC residual added before the activation (shape of the output) */
   const void* res_lo;   /* optional low-order part of the residual */

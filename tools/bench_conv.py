@@ -30,6 +30,11 @@ CASES = {
     # the sensory update as the product runs it: gate epilogue, 192-column tiles; and the plain epilogue on 192-column tiles
     'gru_gates': (16, 68, 120, 512, 1536, 3, 'gates'),
     'gru_n192': (16, 68, 120, 512, 1536, 3, 'two192'),
+    # batch-1 layers at 1/16 (the pixel encoder's layer3, the projections, the fusers' shared halves): 64 flat pixel
+    # tiles, so the channel tile decides how many SMs they occupy
+    'layer3_c2_precise_b1': (1, 68, 120, 256, 256, 3, 'precise'),
+    'proj1_b1': (1, 68, 120, 1024, 512, 1, 'raw'),
+    'fuser_c1x_b1': (1, 68, 120, 512, 512, 3, 'raw'),
 }
 
 
@@ -109,7 +114,13 @@ def run_matmul(name, iters=8, reps=10):
 if __name__ == '__main__':
     ap = argparse.ArgumentParser()
     ap.add_argument('--cases', default=','.join([*CASES, *MATMULS]))
+    ap.add_argument('--rect', action='store_true', help='rectangular pixel tiles only (no flat tiles at 1/16)')
+    ap.add_argument('--packed-nt', action='store_true', help='every launch takes the packed channel tile')
     a = ap.parse_args()
     nat.require_device()
+    if a.rect:
+        ops.FLAT_TILES = False
+    if a.packed_nt:
+        ops.choose_nt = lambda nt, *_: nt
     for c in a.cases.split(','):
         print(json.dumps(run_matmul(c) if c in MATMULS else run(c)))

@@ -4,14 +4,20 @@
 //
 //   D[pixel, cout] = sum_{tap, cin} X[b, y*s + dy(tap), x*s + dx(tap), cin] * W[cout, tap, cin]
 //
-//   M = 128 output pixels = a TH x TW rectangle of one image, N = NT output channels (<= 256),
-//   K = 64 input channels of one filter tap per k-iteration.
+//   M = 128 output pixels = a TH x TW rectangle of one image, or (flat tiles, stride 1) 128 consecutive pixels of one
+//   image in row-major order; N = NT output channels (<= 256), K = 64 input channels of one filter tap per k-iteration.
 //
 // A operand: the activation tensor is described to TMA as a rank-5 tiled tensor (C, W, H, B, 1); the box
 //   (64, TW, TH, 1, 1) lands in shared memory as 128 rows of 128 bytes in exactly the 128B-swizzled K-major
 //   layout wgmma wants.  A filter tap is just a shifted box origin; convolution padding is TMA's
 //   out-of-bounds zero fill (also for negative coordinates).  Stride-2 convolutions use one tensor map per
 //   input phase (y%2, x%2) over the same memory, so every tap is again a unit-stride box.
+//   Flat tiles: no rectangle of 128 pixels fits an output like 68 x 120, and the best one, (1, 128), spends 6.25 % of
+//   the MMA rows on padding.  A flat tile t of image b is pixels 128t .. 128t+127 of that image, loaded through an
+//   im2col-mode tensor map (rank 4: C, W, H, B): the load starts at the tile's first output pixel shifted by -pad, walks
+//   128 pixels through the bounding box of filter-window origins, and a filter tap is the im2col offset (dx, dy) + pad.
+//   Padding is again the zero fill.  Rows past the image's last pixel read the next image (or the zero fill) and
+//   compute values that are never stored; the staged epilogue's maps see the image as [B, 1, Ho*Wo, C].
 // B operand: weights packed [Cout_pad, taps * Cin_pad] fp16 (K-major), 2-D TMA.
 // Epilogue (straight from the accumulator registers): + bias (folded BatchNorm), + optional residual (own or
 //   batch-broadcast), + optional rank-1 term w1[cout] * x1[b, pixel] (the "+1" mask / logit input channel of
@@ -72,6 +78,10 @@ static_assert(SMEM_BYTES <= 232448, "conv: shared-memory budget");
 struct Params {
   int batch, ho, wo, cout;
   int tiles_x, tiles_y, tw, th;
+  // flat tiles (flat_wo = the output width > 0): everything but the activation loads sees each output image as one row,
+  // ho = 1, wo = Ho * Wo, tiled by th x tw = 1 x 128; the loads recover the pixel's (y, x) from flat_wo.  pad: the
+  // filter's padding (a tap's im2col offset is its input offset + pad).
+  int flat_wo, pad;
   int n_tiles, nt;
   int taps, cblocks;
   int m_tiles;   // batch * tiles_y * tiles_x
@@ -120,12 +130,13 @@ struct Params {
 };
 
 struct Maps {
-  CUtensorMap act[8];
+  CUtensorMap act[8];     // box {64, tw, th}; flat tiles: im2col, 128 pixels x 64 channels
   CUtensorMap wgt;        // box {64, nt}
-  CUtensorMap act8;       // e4m3 low-order activations, box {128 B, tw, th}
+  CUtensorMap act8;       // e4m3 low-order activations, box {128 B, tw, th}; flat tiles: im2col, 128 pixels x 128 B
   CUtensorMap wgt8;       // e4m3 weights, box {128 B, nt}
   CUtensorMap res, res_lo;  // staged epilogue: residual (hi, lo) [B or 1, Ho, Wo, Cout], box {64, tw, th}
   CUtensorMap out[3];       // staged epilogue: the output stored from region k, box {64, tw, th}
+                            // (flat tiles: [B or 1, 1, Ho*Wo, Cout], box {64, 128, 1})
 };
 
 __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, const int (&c)[5]) {
@@ -133,6 +144,17 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m
       "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes "
       "[%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(smem_u32(smem_dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c[0]), "r"(c[1]), "r"(c[2]), "r"(c[3]), "r"(c[4])
+      : "memory");
+}
+
+// Im2col load of 128 pixels (flat tiles): c = (channel, x, y, image) of the first pixel's filter-window origin,
+// (dx, dy) the tap's offset inside the window.
+__device__ __forceinline__ void tma_load_im2col_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, const int (&c)[4],
+                                                   uint16_t dx, uint16_t dy) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes "
+      "[%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c[0]), "r"(c[1]), "r"(c[2]), "r"(c[3]), "h"(dx), "h"(dy)
       : "memory");
 }
 
@@ -532,14 +554,23 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
         int b, y0, x0, n0, ks;
         tile_decode(u, p, b, y0, x0, n0, ks);
         const int k_lo = ks * p.k_per_split, k_hi = min(k_iters, k_lo + p.k_per_split);
+        // flat tiles: the first pixel's filter-window origin
+        const int fy = p.flat_wo ? x0 / p.flat_wo : 0, fx = x0 - fy * p.flat_wo - p.pad;
         // one k-iteration: activation box of tap t / channel block cb (+ the matching weight columns) into `stage`
         auto issue = [&](const int t, const int cb, const bool f8) {
-          int c[5] = {f8 ? cb * 128 : cb * BK, x0 + p.tap_dx[t], y0 + p.tap_dy[t], b, 0};  // (channel, x, y, image, 1)
+          const int ch = f8 ? cb * 128 : cb * BK;
           const CUtensorMap* am = f8 ? &maps.act8 : &maps.act[p.tap_map[t]];
           const int wcol = f8 ? (p.tap_w[t] * p.cblocks8 + cb) * 128 : (p.tap_w[t] * p.cblocks + cb) * BK;
           mbar_wait(&empty[stage], phase ^ 1);
           mbar_expect_tx(&full[stage], stage_tx);
-          tma_load_5d(sA + stage * A_BYTES, am, &full[stage], c);
+          if (p.flat_wo) {
+            const int c[4] = {ch, fx, fy - p.pad, b};  // (channel, x, y, image)
+            tma_load_im2col_4d(sA + stage * A_BYTES, am, &full[stage], c, (uint16_t)(p.tap_dx[t] + p.pad),
+                               (uint16_t)(p.tap_dy[t] + p.pad));
+          } else {
+            const int c[5] = {ch, x0 + p.tap_dx[t], y0 + p.tap_dy[t], b, 0};  // (channel, x, y, image, 1)
+            tma_load_5d(sA + stage * A_BYTES, am, &full[stage], c);
+          }
           tma_load_2d(sB + stage * B_BYTES_MAX, f8 ? &maps.wgt8 : &maps.wgt, &full[stage], wcol, n0);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         };
@@ -631,7 +662,8 @@ conv_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p)
 
 using namespace b200;
 
-// Staged epilogue plan (p.staged, output regions, tensor maps): every tile spans exactly N existing channels, fp16 / e4m3
+// Staged epilogue plan (p.staged, output regions, tensor maps; ho, wo, p.th, p.tw as the kernel sees them, i.e. 1, Ho * Wo,
+// 1, 128 for flat tiles): every tile spans exactly N existing channels, fp16 / e4m3
 // outputs that fit the three regions of a stage, 16-byte aligned operands (TMA).  DEVA_B200_CONV_EPI=regs keeps the
 // per-thread epilogue (A/B comparisons); DEVA_B200_CONV_EPI=staged refuses a launch that cannot take the staged one.
 static int plan_staged(const deva_b200_conv_desc& d, int ho, int wo, int n_mma, conv::Params& p, conv::Maps& maps) {
@@ -667,20 +699,20 @@ static int plan_staged(const deva_b200_conv_desc& d, int ho, int wo, int n_mma, 
       if (!used[k]) continue;
       *regs_of[k] = (signed char)k16;
       if (outs[k]) {
-        rc |= make_tmap_act5(&maps.out[k16], outs[k], d.cout, wo, ho, d.batch, cstr, wstr, bstr, d.tw, d.th, &err);
+        rc |= make_tmap_act5(&maps.out[k16], outs[k], d.cout, wo, ho, d.batch, cstr, wstr, bstr, p.tw, p.th, &err);
         p.store_mask |= 1 << k16;
       }
       ++k16;
     }
     if (d.out_relu_lo8) {
       p.reg_lo8 = (signed char)r_lo8;
-      rc |= make_tmap_act5_u8(&maps.out[r_lo8], d.out_relu_lo8, d.cout, wo, ho, d.batch, cstr, wstr, bstr, 64, d.tw, d.th,
+      rc |= make_tmap_act5_u8(&maps.out[r_lo8], d.out_relu_lo8, d.cout, wo, ho, d.batch, cstr, wstr, bstr, 64, p.tw, p.th,
                               &err);
       p.store_mask |= 1 << r_lo8;
     }
     const int rb = d.res_broadcast ? 1 : d.batch;
-    if (d.res) rc |= make_tmap_act5(&maps.res, d.res, d.cout, wo, ho, rb, cstr, wstr, bstr, d.tw, d.th, &err);
-    if (d.res_lo) rc |= make_tmap_act5(&maps.res_lo, d.res_lo, d.cout, wo, ho, rb, cstr, wstr, bstr, d.tw, d.th, &err);
+    if (d.res) rc |= make_tmap_act5(&maps.res, d.res, d.cout, wo, ho, rb, cstr, wstr, bstr, p.tw, p.th, &err);
+    if (d.res_lo) rc |= make_tmap_act5(&maps.res_lo, d.res_lo, d.cout, wo, ho, rb, cstr, wstr, bstr, p.tw, p.th, &err);
     if (rc) {
       set_error("conv: %s", err ? err : "epilogue tensor maps");
       return 3;
@@ -701,7 +733,11 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
   B200_REQUIRE(d.stride == 1 || d.stride == 2, "conv: stride %d unsupported", d.stride);
   B200_REQUIRE(d.kh == d.kw && (d.kh == 1 || d.kh == 3), "conv: %dx%d filter unsupported here", d.kh, d.kw);
   B200_REQUIRE(d.nt % 32 == 0 && d.nt >= 32 && d.nt <= 256 && d.cout_pad % d.nt == 0, "conv: bad channel tile %d", d.nt);
-  B200_REQUIRE(d.tw * d.th == 128 && d.tw <= 256 && d.th <= 256, "conv: spatial tile %dx%d must cover 128 pixels", d.th, d.tw);
+  const bool flat = d.th == 0;  // flat tiles: 128 consecutive pixels of one image (th = 0, tw = 128)
+  B200_REQUIRE(flat ? d.tw == 128 : (d.th > 0 && d.tw * d.th == 128 && d.tw <= 256 && d.th <= 256),
+               "conv: spatial tile %dx%d must cover 128 pixels (or be 0 x 128: flat tiles)", d.th, d.tw);
+  B200_REQUIRE(!flat || (d.stride == 1 && !d.out_pool4),
+               "conv: flat tiles need stride 1 (got %d) and no out_pool4 (its windows need rectangular tiles)", d.stride);
   B200_REQUIRE(d.cout_pad <= conv::kMaxBias && (!d.rank1_w || d.cout_pad <= conv::kMaxRank1),
                "conv: Cout_pad %d exceeds the shared-memory bias table (%d; %d with a rank-1 input)", d.cout_pad, conv::kMaxBias,
                conv::kMaxRank1);
@@ -738,7 +774,10 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
     for (int ph = 0; ph < phases; ++ph) {
       const int py = ph / 2, px = ph % 2;
       int rc;
-      if (d.stride == 1) {
+      if (flat) {
+        rc = make_tmap_im2col4(&maps.act[sidx * 4], TmapType::F16, xs, d.cin_pad, d.w, d.h, d.batch, 64, pad, &err);
+        built[sidx * 4] = true;
+      } else if (d.stride == 1) {
         rc = make_tmap_act5(&maps.act[sidx * 4], xs, d.cin_pad, d.w, d.h, d.batch, (long long)d.cin_pad,
                             (long long)d.w * d.cin_pad, (long long)d.h * d.w * d.cin_pad, d.tw, d.th, &err);
         built[sidx * 4] = true;
@@ -780,8 +819,13 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
     return 3;
   }
   p.batch = d.batch; p.ho = ho; p.wo = wo; p.cout = d.cout;
-  p.tw = d.tw; p.th = d.th;
-  p.tiles_x = ceil_div(wo, d.tw); p.tiles_y = ceil_div(ho, d.th);
+  if (flat) {  // see Params::flat_wo
+    p.ho = 1; p.wo = ho * wo; p.th = 1; p.tw = 128;
+    p.flat_wo = wo; p.pad = pad;
+  } else {
+    p.tw = d.tw; p.th = d.th;
+  }
+  p.tiles_x = ceil_div(p.wo, p.tw); p.tiles_y = ceil_div(p.ho, p.th);
   p.nt = d.nt; p.n_tiles = d.cout_pad / d.nt;
   p.cblocks = d.cin_pad / 64;
   p.m_tiles = p.batch * p.tiles_y * p.tiles_x;
@@ -838,8 +882,9 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
   maps.wgt8 = maps.wgt;
   if (d.split_mode == 3) {
     const uint64_t k8 = (uint64_t)ktaps * d.cin_pad;  // bytes per weight row (cin_pad is a multiple of 128)
-    if (make_tmap_act5_u8(&maps.act8, d.x_lo8, d.cin_pad, d.w, d.h, d.batch, (long long)d.cin_pad, (long long)d.w * d.cin_pad,
-                          (long long)d.h * d.w * d.cin_pad, 128, d.tw, d.th, &err) ||
+    if ((flat ? make_tmap_im2col4(&maps.act8, TmapType::U8, d.x_lo8, d.cin_pad, d.w, d.h, d.batch, 128, pad, &err)
+              : make_tmap_act5_u8(&maps.act8, d.x_lo8, d.cin_pad, d.w, d.h, d.batch, (long long)d.cin_pad,
+                                  (long long)d.w * d.cin_pad, (long long)d.h * d.w * d.cin_pad, 128, d.tw, d.th, &err)) ||
         make_tmap_2d(&maps.wgt8, TmapType::U8, d.w8_packed, k8, d.cout_pad, k8, 128, d.nt, &err)) {
       set_error("conv: %s", err ? err : "fp8 tensor maps");
       return 3;
@@ -856,7 +901,7 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
   p.k_per_split = (k_iters_total + p.ksplit - 1) / p.ksplit;
   p.ksplit = (k_iters_total + p.k_per_split - 1) / p.k_per_split;  // no empty trailing split
   p.f32_split_stride = (long long)d.batch * ho * wo * d.cout;
-  if (const int rc = plan_staged(d, ho, wo, n_mma, p, maps)) return rc;
+  if (const int rc = plan_staged(d, p.ho, p.wo, n_mma, p, maps)) return rc;
   const long long units = (long long)p.m_tiles * p.n_tiles * p.ksplit;
   B200_REQUIRE(units <= INT32_MAX, "conv: %lld work units", units);
   p.units = (int)units;

@@ -7,24 +7,38 @@ namespace b200 {
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*,
+                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                   CUtensorMapFloatOOBfill);
 
-static EncodeTiledFn resolve_encode(const char** err) {
-  static EncodeTiledFn fn = nullptr;
+// The driver entry point `Name`, resolved once through the runtime (no libcuda link).
+template <typename Fn>
+static Fn resolve_driver(const char* name, const char* missing, const char** err) {
+  static Fn fn = nullptr;
   static std::once_flag once;
   static const char* failure = nullptr;
-  std::call_once(once, [] {
+  std::call_once(once, [&] {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult qres;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres);
+    cudaError_t e = cudaGetDriverEntryPoint(name, &p, cudaEnableDefault, &qres);
     if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || p == nullptr) {
-      failure = "cuTensorMapEncodeTiled not available (no CUDA driver?)";
+      failure = missing;
       (void)cudaGetLastError();
     } else {
-      fn = reinterpret_cast<EncodeTiledFn>(p);
+      fn = reinterpret_cast<Fn>(p);
     }
   });
   if (!fn && err) *err = failure;
   return fn;
+}
+static EncodeTiledFn resolve_encode(const char** err) {
+  return resolve_driver<EncodeTiledFn>("cuTensorMapEncodeTiled", "cuTensorMapEncodeTiled not available (no CUDA driver?)",
+                                       err);
+}
+static EncodeIm2colFn resolve_encode_im2col(const char** err) {
+  return resolve_driver<EncodeIm2colFn>("cuTensorMapEncodeIm2col",
+                                        "cuTensorMapEncodeIm2col not available (no CUDA driver?)", err);
 }
 
 static CUtensorMapDataType to_cu(TmapType t, uint32_t* esize) {
@@ -120,6 +134,33 @@ int make_tmap_act5(CUtensorMap* out, const void* base, uint64_t c, uint64_t w, u
   const long long strides[4] = {stride_w, stride_h, stride_b, stride_b * (long long)b};
   const uint32_t box[5] = {64, box_w, box_h, 1, 1};
   return make_tmap_f16_5d(out, base, dims, strides, box, err);
+}
+
+int make_tmap_im2col4(CUtensorMap* out, TmapType type, const void* base, uint64_t c, uint64_t w, uint64_t h, uint64_t b,
+                      uint32_t box_c, int pad, const char** err) {
+  EncodeIm2colFn fn = resolve_encode_im2col(err);
+  if (!fn) return 1;
+  uint32_t esize;
+  const CUtensorMapDataType dt = to_cu(type, &esize);
+  const uint64_t row = c * esize;
+  if ((reinterpret_cast<uintptr_t>(base) & 15) || (row & 15) || box_c * esize != 128 || c < box_c || w == 0 || h == 0 ||
+      b == 0 || pad < 0 || pad > 127) {
+    if (err) *err = "make_tmap_im2col4: bad alignment / box";
+    return 2;
+  }
+  cuuint64_t gdim[4] = {c, w, h, b};
+  cuuint64_t gstride[3] = {row, row * w, row * w * h};
+  // base pixels (the filter window's top-left input pixel) span [-pad, dim - 1 - pad] in W and H
+  const int lower[2] = {-pad, -pad}, upper[2] = {-pad, -pad};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = fn(out, dt, 4, const_cast<void*>(base), gdim, gstride, lower, upper, box_c, 128, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    if (err) *err = "cuTensorMapEncodeIm2col failed";
+    return 3;
+  }
+  return 0;
 }
 
 }  // namespace b200

@@ -31,4 +31,12 @@ int make_tmap_act5_u8(CUtensorMap* out, const void* base, uint64_t c, uint64_t w
 int make_tmap_f16_5d(CUtensorMap* out, const void* base, const uint64_t (&dims)[5], const long long (&strides)[4],
                      const uint32_t (&box)[5], const char** err);
 
+// Im2col map of an NHWC tensor for stride-1 convolutions with `pad` pixels of zero padding: rank-4 dims (C, W, H, B),
+// 128 pixels of box_c channels (box_c * element size = 128 B, 128-byte swizzle) per load.  A load at coordinates
+// (c0, x - pad, y - pad, b) with im2col offsets (dx, dy) in [0, 2 pad] fetches, for the 128 consecutive output pixels
+// that start at (y, x) of image b in row-major order, input pixel (y' - pad + dy, x' - pad + dx) of each; rows past
+// the image continue into the next one, and everything outside the tensor is zero-filled.
+int make_tmap_im2col4(CUtensorMap* out, TmapType type, const void* base, uint64_t c, uint64_t w, uint64_t h, uint64_t b,
+                      uint32_t box_c, int pad, const char** err);
+
 }  // namespace b200

@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 26
+ABI_VERSION = 27
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192

@@ -16,11 +16,16 @@ CHAIN = 27      # chain length when a longer loop is split (= one 3x3 filter ove
 PROFILE = None  # set to a list by bench.py to collect (start event, end event, algorithmic FLOPs, MMA passes) per conv
 
 _TILES = ((1, 128), (2, 64), (4, 32), (8, 16), (16, 8), (32, 4))
+FLAT = (0, 128)  # flat tiles: 128 consecutive output pixels of one image (stride 1, no pool4)
+FLAT_TILES = True  # False: rectangles only (tools/bench_conv.py --rect compares the two)
+NT_WIDTHS = (256, 192, 128, 64)  # channel tiles with a wgmma width of their own (the staged epilogue takes exactly these)
 
 
-def choose_tile(ho: int, wo: int, pool4: bool = False) -> Tuple[int, int]:
+def choose_tile(ho: int, wo: int, pool4: bool = False, stride: int = 1) -> Tuple[int, int]:
     """(th, tw) with th*tw = 128 that wastes the fewest MMA rows on an ho x wo output (``pool4``: among the tiles
-    whose sides are multiples of 4, which the epilogue's 4x4 pooling needs; the tile does not change any result)."""
+    whose sides are multiples of 4, which the epilogue's 4x4 pooling needs).  A stride-1 launch without ``pool4`` takes
+    flat tiles (``FLAT``) when they waste strictly fewer rows than the best rectangle, e.g. at 68 x 120 (1/16 of 1080p),
+    where (1, 128) computes 68 tiles for 63.75 tiles of pixels.  The tile does not change any result."""
     best, best_cost = None, None
     for th, tw in _TILES:
         if pool4 and (th % 4 or tw % 4):
@@ -28,7 +33,47 @@ def choose_tile(ho: int, wo: int, pool4: bool = False) -> Tuple[int, int]:
         cost = -(-ho // th) * th * (-(-wo // tw) * tw)
         if best_cost is None or cost < best_cost or (cost == best_cost and tw > best[1]):
             best, best_cost = (th, tw), cost
+    if FLAT_TILES and stride == 1 and not pool4 and -(-ho * wo // 128) * 128 < best_cost:
+        return FLAT
     return best
+
+
+def pixel_tiles(ho: int, wo: int, tile: Tuple[int, int]) -> int:
+    """Pixel tiles of one ho x wo image under ``tile`` (th, tw), flat or rectangular."""
+    th, tw = tile
+    return -(-ho * wo // 128) if th == 0 else -(-ho // th) * -(-wo // tw)
+
+
+def choose_nt(nt: int, cout_pad: int, m_tiles: int, ksplit: int, sms: int) -> int:
+    """Channel tile of one launch.  The kernel's persistent CTAs take work units (pixel tile, channel tile, k-split) in
+    waves of ``sms``; a unit costs about its width, so a launch costs ~ ceil(units / sms) * width.  Of ``nt`` (the
+    packed default) and the narrower widths in NT_WIDTHS that divide ``cout_pad`` this returns the cheapest, ties to the
+    wider.  A narrower tile must save more than 1/8: it re-reads the activation tile and runs one more epilogue per
+    pixel tile, which the model leaves out, so launches of four or more waves keep ``nt``.  A ``nt`` outside NT_WIDTHS
+    (a ragged tile) stays.  A batch-1 1/16-resolution layer with 256 channels is 64 pixel tiles: one
+    256-wide wave on 64 SMs, or one 128-wide wave on 128.  No width changes any result: every output element takes the
+    same k-iterations in the same order."""
+    if nt not in NT_WIDTHS:
+        return nt
+    ksplit = max(ksplit, 1)
+
+    def cost(w):
+        return -(-m_tiles * (cout_pad // w) * ksplit // sms) * w
+    best, base = nt, cost(nt)
+    for w in NT_WIDTHS:  # widest first: a tie keeps the wider
+        if w < nt and cout_pad % w == 0 and 8 * cost(w) < 7 * base and cost(w) < cost(best):
+            best = w
+    return best
+
+
+_SMS = {}
+
+
+def _sm_count(dev) -> int:
+    idx = dev.index if dev.index is not None else torch.cuda.current_device()
+    if idx not in _SMS:
+        _SMS[idx] = torch.cuda.get_device_properties(idx).multi_processor_count
+    return _SMS[idx]
 
 
 def _round_up(x, m):
@@ -89,9 +134,11 @@ class PackedConv:
             self.nt = _round_up(cout, 32)
         if self.nt == 0:
             self.nt = 256
+        self.nt_fixed = gates  # the gate epilogue takes 192-wide tiles only
         if nt_override is not None:  # channel-tile experiments (tools/bench_conv.py)
             assert not gates and nt_override % 32 == 0 and 32 <= nt_override <= 256
             self.nt = nt_override
+            self.nt_fixed = True
         self.cout_pad = _round_up(cout, self.nt)
         nsrc = 2 if two_inputs else 1
         w = torch.zeros(self.cout_pad, nsrc, kh * kw, self.cin_pad, dtype=torch.float32, device=dev)
@@ -168,7 +215,7 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
             assert other.dtype == torch.float16 and other.is_contiguous() and other.shape == x.shape
     b, h, w, _ = x.shape
     ho, wo = pc.out_hw(h, w)
-    th, tw = choose_tile(ho, wo, want_pool4)
+    th, tw = choose_tile(ho, wo, want_pool4, pc.stride)
     dev = x.device
 
     def new(dtype=torch.float16):
@@ -230,7 +277,10 @@ def conv_ex(x: torch.Tensor, pc: PackedConv, *, x2: Optional[torch.Tensor] = Non
     if PROFILE is not None:  # bench.py's conv-roofline pass: CUDA events around the launch + algorithmic FLOPs
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
-    nat.conv2d(x, b, h, w, pc.cin_pad, pc.w_packed, pc.k, pc.stride, pc.cout, pc.cout_pad, pc.nt, th, tw, pc.bias,
+    nt = pc.nt
+    if not (pc.nt_fixed or head_w is not None):  # the head needs the whole Cout in one tile
+        nt = choose_nt(pc.nt, pc.cout_pad, b * pixel_tiles(ho, wo, (th, tw)), ksplit, _sm_count(dev))
+    nat.conv2d(x, b, h, w, pc.cin_pad, pc.w_packed, pc.k, pc.stride, pc.cout, pc.cout_pad, nt, th, tw, pc.bias,
                x2=x2, x_lo=x_lo, res=res, res_lo=res_lo, res_broadcast=res_b, rank1_w=pc.rank1_w,
                rank1_x=rank1_x if pc.rank1_w is not None else None, out_raw=o.raw, out_relu=o.relu, out_f32=o.f32,
                out_raw_lo=o.raw_lo, out_relu_lo=o.relu_lo, head_w=head_w, head_out=o.head, head_n=head_n,
