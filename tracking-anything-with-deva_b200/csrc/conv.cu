@@ -807,6 +807,11 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
       ph = py * 2 + px;
       dy = (oy - py) / 2;
       dx = (ox - px) / 2;
+      // An input one row (column) high (wide) has no odd-row (odd-column) phase: every tap of that phase reads
+      // padding, but its map slot holds phase 0's map.  Its box is moved wholly above (left of) the image instead, so
+      // that TMA fills it with zeros: the output is then one row (column) high, y0 = 0 (x0 = 0).
+      if (py >= d.h) dy = -d.th;
+      if (px >= d.w) dx = -d.tw;
     }
     p.tap_map[t] = (signed char)(pass_src[pass] * 4 + ph);
     p.tap_w[t] = (signed char)(t < p.taps16 ? pass_w[pass] * ktaps + kt : kt);
@@ -840,9 +845,11 @@ DEVA_B200_API int deva_b200_conv2d(const deva_b200_conv_desc* desc, deva_stream_
   p.out_raw_lo = reinterpret_cast<__half*>(d.out_raw_lo);
   p.out_relu_lo = reinterpret_cast<__half*>(d.out_relu_lo);
   if (d.gate_out) {
+    // the gates are evaluated on the unscaled accumulator (epilogue_gates)
     B200_REQUIRE(d.gate_h && d.nt == 192 && d.cout == d.cout_pad && d.cout % 192 == 0 && !d.head_w && !d.res && !d.rank1_w &&
-                     !d.out_raw && !d.out_relu && !d.out_f32,
-                 "conv: the gate epilogue needs nt == 192, cout = 3 * C with C %% 64 == 0 (got %d) and no other outputs", d.cout);
+                     !d.out_raw && !d.out_relu && !d.out_f32 && p.acc_scale == 1.f,
+                 "conv: the gate epilogue needs nt == 192, cout = 3 * C with C %% 64 == 0 (got %d), acc_scale 1 and no other "
+                 "outputs", d.cout);
     p.gate_h = reinterpret_cast<const __half*>(d.gate_h);
     p.gate_out = reinterpret_cast<__half*>(d.gate_out);
     p.gate_c = d.cout / 3;
