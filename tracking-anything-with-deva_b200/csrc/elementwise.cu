@@ -90,11 +90,14 @@ stem_im2col_kernel(const float* __restrict__ src, __half* __restrict__ dst, __ha
   }
 }
 
-// Pixel-per-thread variant for the shapes the network uses (C = 1: mask planes, Kp = 64; C = 3: image, Kp = 192, with
-// or without the fp16 remainders).  The generic kernel spends ~120 instructions of index arithmetic per 16-byte store
-// and ran at 16-28 % of the HBM peak; here a thread owns one output pixel, reads its 49*C taps from a patch staged in
-// shared memory (even / odd input columns de-interleaved so consecutive pixels read consecutive words) with compile-time
-// tap offsets, and writes its whole im2col row with 16-byte stores.  Same values as the generic kernel.
+// Block variant for the shapes the network uses (C = 1: mask planes, Kp = 64; C = 3: image, Kp = 192, with or without
+// the fp16 remainders).  The generic kernel spends ~120 instructions of index arithmetic per 16-byte store and ran at
+// 16-28 % of the HBM peak.  Here a block stages the patch under IM1_XT output pixels x ROWS output rows in shared memory
+// (even / odd input columns de-interleaved), with a table of each column's patch offset.  The block's output in one row
+// is nx * Kp contiguous halves, and thread t writes its 16-byte pieces t, t + IM1_XT, ...: a warp stores 512
+// contiguous bytes per instruction.  (With one pixel per thread, a warp's 16-byte stores were 32 pieces Kp * 2 bytes
+// apart, and the kernel wrote the pixel encoder's 400 MB of columns at about a fifth of the HBM bandwidth.)  Same values
+// as the generic kernel.
 constexpr int IM1_XT = 128;
 template <int C, int ROWS, bool LO>
 __global__ void __launch_bounds__(IM1_XT)
@@ -102,7 +105,9 @@ stem_im2col_px_kernel(const float* __restrict__ src, __half* __restrict__ dst, _
   constexpr int PR = 2 * ROWS + 5;      // input rows under ROWS output rows
   constexpr int PH = IM1_XT + 3;        // input column x_in0 + 2*i (+1) for i in [0, PH)
   constexpr int KP = (49 * C + 63) / 64 * 64;
-  __shared__ float pe[C][PR][PH], po[C][PR][PH];
+  constexpr int K8 = KP / 8;            // 16-byte pieces of one pixel's row
+  __shared__ float patch[2][C][PR][PH];  // [input column parity][plane][row][column / 2]
+  __shared__ __align__(16) int tab[KP];  // column k = (ky*7 + kx)*C + c -> its offset in patch for output (row 0, pixel 0)
   const int Ho = H / 2, Wo = W / 2;
   const int groups = (Ho + ROWS - 1) / ROWS;
   const int b = blockIdx.y / groups, yo0 = (blockIdx.y - b * groups) * ROWS;
@@ -112,50 +117,41 @@ stem_im2col_px_kernel(const float* __restrict__ src, __half* __restrict__ dst, _
   for (int i = threadIdx.x; i < C * PR * 2 * PH; i += IM1_XT) {
     const int px = i % (2 * PH), r = (i / (2 * PH)) % PR, c = i / (2 * PH * PR);
     const int y = y_in0 + r, x = x_in0 + px;
-    const float v = (y >= 0 && y < H && x >= 0 && x < W) ? img[((long long)c * H + y) * W + x] : 0.f;
-    if (px & 1) po[c][r][px >> 1] = v;
-    else pe[c][r][px >> 1] = v;
+    patch[px & 1][c][r][px >> 1] = (y >= 0 && y < H && x >= 0 && x < W) ? img[((long long)c * H + y) * W + x] : 0.f;
+  }
+  for (int k = threadIdx.x; k < KP; k += IM1_XT) {
+    const int tap = k / C, c = k - tap * C, ky = tap / 7, kx = tap - ky * 7;
+    tab[k] = k < 49 * C ? &patch[kx & 1][c][ky][kx >> 1] - &patch[0][0][0][0] : -1;
   }
   __syncthreads();
-  const int xl = threadIdx.x, xo = xo0 + xl;
-  if (xo >= Wo) return;
+  const float* pf = &patch[0][0][0][0];
+  const int nx = min(IM1_XT, Wo - xo0);
 #pragma unroll 1
   for (int rr = 0; rr < ROWS; ++rr) {
     const int yo = yo0 + rr;
     if (yo >= Ho) break;
-    const long long out = (((long long)b * Ho + yo) * Wo + xo) * KP;
+    const long long out = (((long long)b * Ho + yo) * Wo + xo0) * KP;
+#pragma unroll 2
+    for (int j = threadIdx.x; j < nx * K8; j += IM1_XT) {  // piece j: pixel xo0 + j / K8, columns 8 (j % K8) + 0..7
+      const int xl = j / K8, k0 = (j - xl * K8) * 8;
+      const int base = 2 * rr * PH + xl;
+      const int4 t0 = *reinterpret_cast<const int4*>(tab + k0), t1 = *reinterpret_cast<const int4*>(tab + k0 + 4);
+      const int t[8] = {t0.x, t0.y, t0.z, t0.w, t1.x, t1.y, t1.z, t1.w};
+      uint4 oh, ol;
+      __half2* h2 = reinterpret_cast<__half2*>(&oh);
+      __half2* l2 = reinterpret_cast<__half2*>(&ol);
 #pragma unroll
-    for (int k0 = 0; k0 < KP; k0 += 16) {  // 16 columns = two 16-byte stores (and two for the remainders)
-      uint4 oh[2], ol[2];
-      __half2* h2 = reinterpret_cast<__half2*>(oh);
-      __half2* l2 = reinterpret_cast<__half2*>(ol);
-#pragma unroll
-      for (int k2 = 0; k2 < 8; ++k2) {
-        float v[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int k = k0 + 2 * k2 + e;  // column k = (ky*7 + kx)*C + c
-          if (k < 49 * C) {
-            const int tap = k / C, c = k - tap * C, ky = tap / 7, kx = tap - ky * 7;
-            v[e] = (kx & 1) ? po[c][2 * rr + ky][xl + (kx >> 1)] : pe[c][2 * rr + ky][xl + (kx >> 1)];
-          } else {
-            v[e] = 0.f;
-          }
-        }
-        h2[k2] = __floats2half2_rn(v[0], v[1]);
+      for (int k2 = 0; k2 < 4; ++k2) {
+        const float v0 = t[2 * k2] >= 0 ? pf[t[2 * k2] + base] : 0.f;
+        const float v1 = t[2 * k2 + 1] >= 0 ? pf[t[2 * k2 + 1] + base] : 0.f;
+        h2[k2] = __floats2half2_rn(v0, v1);
         if (LO) {
           const float2 back = __half22float2(h2[k2]);
-          l2[k2] = __floats2half2_rn(v[0] - back.x, v[1] - back.y);
+          l2[k2] = __floats2half2_rn(v0 - back.x, v1 - back.y);
         }
       }
-      uint4* dh = reinterpret_cast<uint4*>(dst + out + k0);
-      dh[0] = oh[0];
-      dh[1] = oh[1];
-      if (LO) {
-        uint4* dl = reinterpret_cast<uint4*>(dst_lo + out + k0);
-        dl[0] = ol[0];
-        dl[1] = ol[1];
-      }
+      reinterpret_cast<uint4*>(dst + out)[j] = oh;
+      if (LO) reinterpret_cast<uint4*>(dst_lo + out)[j] = ol;
     }
   }
 }
@@ -231,10 +227,12 @@ up2_add_split_kernel(const __half* __restrict__ g, const __half* __restrict__ g_
   // weights 0.25 / 0.75, so the source quad (hi + lo) is loaded once per four outputs and there is no serial walk:
   // every thread is one independent load -> compute -> store chain (the row-walking version kept the DRAM traffic at the
   // algorithmic 1x but ran at half the HBM rate: eight dependent rows per thread; the per-pixel version before it re-read
-  // the source 5x).  blockIdx.y = (image, k), k in [0, h]; the clamped border blocks produce the reference's values
-  // exactly (a + (a - a) * wx == a).
+  // the source 5x).  blockIdx.y = (k, image), k in [0, h]; the clamped border blocks produce the reference's values
+  // exactly (a + (a - a) * wx == a).  The image index runs fastest: the B blocks of one k read the same two skip rows
+  // back to back, so the broadcast skip (hi + lo, 134 MB at 1/4 of 1080p with 256 channels) comes from DRAM about once
+  // instead of once per image, and stays in L2 for the others.
   const int H = 2 * h, W = 2 * w, C8 = C / 8;
-  const int b = blockIdx.y / (h + 1), k = blockIdx.y - b * (h + 1);
+  const int k = blockIdx.y / B, b = blockIdx.y - k * B;
   const int ya = max(k - 1, 0), yb = min(k, h - 1);
   const int row_vecs = (w + 1) * C8;
   for (int i = blockIdx.x * 256 + threadIdx.x; i < row_vecs; i += gridDim.x * 256) {
