@@ -19,11 +19,9 @@ def _scenario(golden_dir):
     return sc
 
 
-def _net(cfg, sd, backend):
+def _net(cfg, sd):
     from deva.model.network import DEVA
-    net = DEVA(cfg)
-    net.conv_backend = backend
-    net = net.cuda().eval()
+    net = DEVA(cfg).cuda().eval()
     net.load_weights({k: v.cuda() for k, v in sd.items()})
     return net
 
@@ -33,17 +31,15 @@ def _golden(golden_dir):
     return g, json.load(open(os.path.join(golden_dir, 'consensus.json')))
 
 
-@pytest.mark.parametrize('backend,tol', [('native', 1e-3), ('torch', 1e-3)])
-def test_spatial_alignment_matches_reference(golden_dir, synthetic_sd, backend, tol):
+def test_spatial_alignment_matches_reference(golden_dir, synthetic_sd):
     from deva.inference.consensus_associated import find_consensus_with_established_association, spatial_alignment
     from deva.inference.image_feature_store import ImageFeatureStore
     from deva.utils.tensor_utils import pad_divide_by
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
+    tol = 1e-3
     sc = _scenario(golden_dir)
     g, meta = _golden(golden_dir)
     cfg = meta['config']
-    net = _net(cfg, synthetic_sd, backend)
+    net = _net(cfg, synthetic_sd)
     data = [(im.cuda(), ids.cuda()) for im, ids in sc.frames()]
     store = ImageFeatureStore(net, no_warning=True)
     img0, _ = pad_divide_by(data[0][0], 16)
@@ -52,7 +48,7 @@ def test_spatial_alignment_matches_reference(golden_dir, synthetic_sd, backend, 
     prob = spatial_alignment(10, img0, m0, 11, img1, net, store, cfg)[0]
     assert tuple(prob.shape) == tuple(g['align_prob'].shape)
     err = float((prob.float().cpu() - g['align_prob']).abs().max())
-    print(f'[{backend}] spatial_alignment max |prob - reference| = {err:.3e}')
+    print(f'spatial_alignment max |prob - reference| = {err:.3e}')
     assert err < tol, err
 
     pick = [(0, (3, 5)), (1, (1, 4)), (3, (7, 8))]
@@ -98,7 +94,7 @@ def test_vote_in_temporary_buffer(golden_dir, synthetic_sd):
     from deva.inference.inference_core import DEVAInferenceCore
     sc = _scenario(golden_dir)
     g, meta = _golden(golden_dir)
-    net = _net(meta['config'], synthetic_sd, 'native')
+    net = _net(meta['config'], synthetic_sd)
     core = DEVAInferenceCore(net, meta['config'])
     data = [(im.cuda(), ids.cuda()) for im, ids in sc.frames()]
     for f in _frame_infos(sc, data):

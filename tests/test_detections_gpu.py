@@ -11,21 +11,17 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize('backend,tol', [('native', 1e-3), ('torch', 1e-3)])
-def test_detection_session_matches_reference(golden_dir, synthetic_sd, backend, tol):
+def test_detection_session_matches_reference(golden_dir, synthetic_sd):
     from deva.inference.inference_core import DEVAInferenceCore
     from deva.inference.object_info import ObjectInfo
     from deva.model.network import DEVA
-    torch.backends.cudnn.allow_tf32 = False
-    torch.backends.cuda.matmul.allow_tf32 = False
+    tol = 1e-3
     spec = importlib.util.spec_from_file_location('consensus_scenario', os.path.join(golden_dir, 'consensus_scenario.py'))
     sc = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(sc)
     g = {k: torch.from_numpy(v) for k, v in np.load(os.path.join(golden_dir, 'detections.npz')).items()}
     meta = json.load(open(os.path.join(golden_dir, 'detections.json')))
-    net = DEVA(meta['config'])
-    net.conv_backend = backend
-    net = net.cuda().eval()
+    net = DEVA(meta['config']).cuda().eval()
     net.load_weights({k: v.cuda() for k, v in synthetic_sd.items()})
     np.random.seed(42)
     core = DEVAInferenceCore(net, meta['config'])

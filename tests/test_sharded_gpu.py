@@ -42,9 +42,7 @@ def _run(core, g, device):
 
 def _net(meta, sd, device):
     from deva.model.network import DEVA
-    net = DEVA(meta['config'])
-    net.conv_backend = 'native'
-    net = net.to(device).eval()
+    net = DEVA(meta['config']).to(device).eval()
     net.load_weights({k: v.to(device) for k, v in sd.items()})
     return net
 

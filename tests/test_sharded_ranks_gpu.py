@@ -266,9 +266,7 @@ def _det_inputs():
 def _net(cfg, dev):
     from deva.model.network import DEVA
     from deva.model.param_spec import synthetic_state_dict
-    net = DEVA(cfg)
-    net.conv_backend = 'native'
-    net = net.to(dev).eval()
+    net = DEVA(cfg).to(dev).eval()
     net.load_weights({k: v.to(dev) for k, v in synthetic_state_dict(seed=1).items()})
     return net
 

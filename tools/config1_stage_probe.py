@@ -1,5 +1,5 @@
 """GPU diagnostic: where does the product differ from the CPU oracle on the real-image clip (config 1)?  Steps the
-product core (both conv backends) and oracle.core.CoreOracle side by side and compares, frame by frame: key / shrinkage /
+product core and oracle.core.CoreOracle side by side and compares, frame by frame: key / shrinkage /
 selection, the memory read-out, the aggregated logits and the probabilities (each pipeline on its own state)."""
 import json
 import os
@@ -18,8 +18,6 @@ from oracle import network as onet  # noqa: E402
 from oracle.core import CoreOracle  # noqa: E402
 
 torch.set_grad_enabled(False)
-torch.backends.cudnn.allow_tf32 = False
-torch.backends.cuda.matmul.allow_tf32 = False
 
 
 def rel(a, b):
@@ -52,46 +50,40 @@ def main():
     onet.segment, onet.transform_key = seg_spy, key_spy
     np.random.seed(42)
     oracle = CoreOracle(sd, meta['config'])
-    cores = {}
-    for backend in ('torch', 'native'):
-        net = DEVA(meta['config'])
-        net.conv_backend = backend
-        net = net.cuda().eval()
-        net.load_weights({k: v.cuda() for k, v in sd.items()})
-        core = DEVAInferenceCore(net, meta['config'])
-        mm_, seg_, key_ = core.memory.match_memory, net.segment, net.transform_key
+    net = DEVA(meta['config']).cuda().eval()
+    net.load_weights({k: v.cuda() for k, v in sd.items()})
+    core = DEVAInferenceCore(net, meta['config'])
+    mm_, seg_, key_ = core.memory.match_memory, net.segment, net.transform_key
 
-        def mm_spy(k, s, _f=mm_, _b=backend):
-            out = _f(k, s)
-            cap[_b + '_readout'] = torch.stack([out[o].float() for o in sorted(out)]).unsqueeze(0)
-            return out
+    def mm_spy(k, s):
+        out = mm_(k, s)
+        cap['readout'] = torch.stack([out[o].float() for o in sorted(out)]).unsqueeze(0)
+        return out
 
-        def sg_spy(*a, _f=seg_, _b=backend, **kw):
-            out = _f(*a, **kw)
-            cap[_b + '_logits'], cap[_b + '_sensory'] = out[1].float(), out[0].float()
-            return out
+    def sg_spy(*a, **kw):
+        out = seg_(*a, **kw)
+        cap['logits'], cap['sensory'] = out[1].float(), out[0].float()
+        return out
 
-        def ky_spy(feat, _f=key_, _b=backend, **kw):
-            out = _f(feat, **kw)
-            cap[_b + '_key'] = [x.float() for x in out]
-            return out
+    def ky_spy(feat, **kw):
+        out = key_(feat, **kw)
+        cap['key'] = [x.float() for x in out]
+        return out
 
-        core.memory.match_memory, net.segment, net.transform_key = mm_spy, sg_spy, ky_spy
-        cores[backend] = core
+    core.memory.match_memory, net.segment, net.transform_key = mm_spy, sg_spy, ky_spy
     for t in range(4):
         po = oracle.step(frames[t], mask0 if t == 0 else None, meta['labels'] if t == 0 else None, end=(t == 3))
         print(f'frame {t}: oracle vs fixture lattice {float((po[:, 1::4, 2::4] - torch.from_numpy(g[f"prob_lattice_{t}"])).abs().max()):.2e}')
-        for backend, core in cores.items():
-            p = core.step(frames[t].cuda(), mask0.cuda() if t == 0 else None, meta['labels'] if t == 0 else None, end=(t == 3))
-            print(f'  [{backend}] prob {rel(p, po)}')
-            for i, name in enumerate(('key', 'shrinkage', 'selection')):
-                print(f'  [{backend}]   {name:10s} {rel(cap[backend + "_key"][i], cap["o_key"][i])}')
-            if t > 0:
-                print(f'  [{backend}]   readout    {rel(cap[backend + "_readout"], cap["o_readout"])}')
-                print(f'  [{backend}]   logits     {rel(cap[backend + "_logits"], cap["o_logits"])}')
-                print(f'  [{backend}]   sensory    {rel(cap[backend + "_sensory"], cap["o_sensory"])}')
-                d = (p.float().cpu() - po).abs()
-                print(f'  [{backend}]   pixels with |d| > 3e-4: {int((d > 3e-4).sum())} of {d.numel()};  > 6e-4: {int((d > 6e-4).sum())}')
+        p = core.step(frames[t].cuda(), mask0.cuda() if t == 0 else None, meta['labels'] if t == 0 else None, end=(t == 3))
+        print(f'  prob {rel(p, po)}')
+        for i, name in enumerate(('key', 'shrinkage', 'selection')):
+            print(f'    {name:10s} {rel(cap["key"][i], cap["o_key"][i])}')
+        if t > 0:
+            print(f'    readout    {rel(cap["readout"], cap["o_readout"])}')
+            print(f'    logits     {rel(cap["logits"], cap["o_logits"])}')
+            print(f'    sensory    {rel(cap["sensory"], cap["o_sensory"])}')
+            d = (p.float().cpu() - po).abs()
+            print(f'    pixels with |d| > 3e-4: {int((d > 3e-4).sum())} of {d.numel()};  > 6e-4: {int((d > 6e-4).sum())}')
 
 
 if __name__ == '__main__':

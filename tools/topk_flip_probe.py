@@ -1,7 +1,8 @@
 """GPU probe: how often, and by how much, does the fused similarity/top-k kernel pick a different top-30 than exact
 arithmetic on REAL-image keys (example clip of tests/golden/config1_vos.npz)?  Memory = keys of frame 0, queries = keys
-of frame 1, both from the cuDNN fp32 engine; ground truth = fp64 similarity on the CPU.  For every query whose set
-differs it reports delta = sim64(best excluded) - sim64(worst included): the similarity error that caused the swap."""
+of frame 1, both from the fp32 oracle network (oracle/network.py) on the CPU; ground truth = fp64 similarity on the CPU.
+For every query whose set differs it reports delta = sim64(best excluded) - sim64(worst included): the similarity error
+that caused the swap."""
 import os
 import sys
 
@@ -12,27 +13,26 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, 'tracking-anything-with-deva_b200'))
 from deva import _native as nat  # noqa: E402
-from deva.model.engine import Engine  # noqa: E402
 from deva.model.param_spec import synthetic_state_dict  # noqa: E402
 from deva.utils.tensor_utils import pad_divide_by  # noqa: E402
 from oracle import memory_math as mm  # noqa: E402
+from oracle import network as onet  # noqa: E402
 
 torch.set_grad_enabled(False)
-torch.backends.cudnn.allow_tf32 = False
-torch.backends.cuda.matmul.allow_tf32 = False
+torch.backends.cuda.matmul.allow_tf32 = False  # the reference's fp32 similarity below runs as an ATen GEMM on the GPU
 
 
 def main():
     g = np.load(os.path.join(ROOT, 'tests/golden/config1_vos.npz'))
     mean = torch.tensor([0.485, 0.456, 0.406]).view(3, 1, 1)
     std = torch.tensor([0.229, 0.224, 0.225]).view(3, 1, 1)
-    eng = Engine({k: v.cuda() for k, v in synthetic_state_dict(seed=1).items()})
+    sd = synthetic_state_dict(seed=1)
     keys = []
     for t in (0, 1):
-        img = ((torch.from_numpy(g['frames_u8'][t]).permute(2, 0, 1).float() / 255 - mean) / std).cuda()
+        img = (torch.from_numpy(g['frames_u8'][t]).permute(2, 0, 1).float() / 255 - mean) / std
         img, _ = pad_divide_by(img, 16)
-        _, feat = eng.encode_image(img.unsqueeze(0))
-        keys.append([x[0].flatten(1).contiguous() for x in eng.transform_key(feat)])
+        _, feat = onet.encode_image(sd, img.unsqueeze(0))
+        keys.append([x[0].flatten(1).contiguous().cuda() for x in onet.transform_key(sd, feat)])
     (mk, ms, _), (qk, _, qe) = keys
     ms = ms.reshape(-1).contiguous()
     n, q, ck = mk.shape[1], qk.shape[1], mk.shape[0]

@@ -41,8 +41,6 @@ def spatial_alignment(src_ti: int, src_image: torch.Tensor, src_mask: torch.Tens
     # the source frame as a one-frame memory bank (no long-term logic: nothing is consolidated or counted)
     bank = MemoryManager(dict(config, enable_long_term=False, enable_long_term_count_usage=False))
     bank.work_frames_without_long_term = 1
-    if getattr(network, 'prefers_nhwc', False):
-        bank.readout_layout = 'nhwc'
     objects = list(range(1, num_objects + 1))
     bank.add_memory(src_key, src_shrinkage, value, objects, selection=src_selection)
     readout = bank.match_memory(tar_key, tar_selection)

@@ -32,8 +32,6 @@ class DEVAInferenceCore:
         self.curr_ti = -1
         self.last_mem_ti = 0
         self.memory = MemoryManager(config=config)
-        if getattr(network, 'prefers_nhwc', False):
-            self.memory.readout_layout = 'nhwc'
         self.object_manager = ObjectManager()
         self.image_feature_store = image_feature_store or ImageFeatureStore(self.network)
         self.last_mask = None

@@ -50,8 +50,9 @@ class MemoryManager:
         self.engaged = False
         # optional profiling hook: a list that receives one (start, end) CUDA-event pair per match_memory call
         self.read_events = None
-        # 'nhwc': match_memory returns fp16 token-major-backed views (what the native NHWC decoder consumes)
-        self.readout_layout = 'nchw'
+        # 'nhwc' (the product layout): match_memory returns fp16 views of token-major storage, which the NHWC decoder
+        # consumes as they are; 'nchw': fp32 [CV,h,w] in the reference's layout
+        self.readout_layout = 'nhwc'
         self.fused_min_work = 16_000_000  # n_window * q above which the fused sparse-affinity readout is used
         self.work_frames_without_long_term = 16  # bank capacity (frames) when long-term memory is disabled
 

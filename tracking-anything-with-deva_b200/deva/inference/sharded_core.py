@@ -304,13 +304,10 @@ class ShardedDEVAInferenceCore(DEVAInferenceCore):
     calls on every rank); each rank returns the full [K+1, H, W] probabilities."""
     def __init__(self, network, config: Dict, *, group: Optional[dist.ProcessGroup] = None, image_feature_store=None):
         super().__init__(network, config, image_feature_store=image_feature_store)
-        if not getattr(network, 'prefers_nhwc', False):
-            raise RuntimeError('the bank-sharded core drives the native engine (conv_backend="native")')
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.memory = ShardedMemoryManager(config, group)
-        self.memory.readout_layout = 'nhwc'
 
     def _own(self, k: int) -> slice:
         lo, hi = object_bounds(k, self.world, self.rank)

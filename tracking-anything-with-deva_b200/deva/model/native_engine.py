@@ -1,8 +1,8 @@
 """The DEVA propagation network on the hand-written sm_90a kernels (NHWC fp16, wgmma implicit GEMM).
 
-Same forward graphs as ``deva.model.engine.Engine`` (which restates the reference's network.py /
-big_modules.py / modules.py / group_modules.py / cbam.py / resnet.py with BatchNorm folded and the
-shared halves hoisted), but every layer is a ``deva_b200_conv2d`` launch with its bias / residual /
+Same forward graphs as ``oracle/network.py`` (which restates the reference's network.py /
+big_modules.py / modules.py / group_modules.py / cbam.py / resnet.py), with BatchNorm folded and the
+shared halves hoisted by ``LayerTable``; every layer is a ``deva_b200_conv2d`` launch with its bias / residual /
 ReLU / rank-1 input fused in the epilogue, and the glue (max-pool, bilinear x2 + skip, area pooling,
 CBAM, GRU gates, soft aggregation + x4 upsampling + softmax) runs in the helper kernels of
 csrc/elementwise.cu.  No cuDNN / cuBLAS on this path.
@@ -18,7 +18,7 @@ import torch
 
 from deva import _native as nat
 from deva.model import native_ops as ops
-from deva.model.engine import LayerTable
+from deva.model.layer_table import LayerTable
 
 KEY_KSPLIT = 8  # accumulation chains of the key projection (see transform_key)
 
@@ -41,7 +41,6 @@ def _api(t_nhwc: torch.Tensor) -> torch.Tensor:
 
 
 class NativeEngine:
-    prefers_nhwc = True
     precision = 'parity'  # the name of the precision plan below, reported in bench.py's result line
 
     def __init__(self, sd: Dict[str, torch.Tensor]):

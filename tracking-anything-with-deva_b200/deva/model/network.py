@@ -2,7 +2,7 @@
 
 Holds the checkpoint tensors under the reference's own names (so ``state_dict()`` /
 ``load_state_dict()`` / ``load_weights()`` exchange checkpoints with the reference unchanged) and
-runs inference through ``deva.model.engine.Engine``.  Inference only: ``read_memory`` (the training-time twin of the
+runs inference through ``deva.model.native_engine.NativeEngine``.  Inference only: ``read_memory`` (the training-time twin of the
 memory read) is provided forward-only on the same kernels; the ``need_aux`` heads and the ``forward(mode, ...)`` dispatch
 used by DDP training are not part of the propagation hot path.
 """
@@ -12,9 +12,6 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-import os
-
-from deva.model.engine import Engine
 from deva.model.native_engine import NativeEngine
 from deva.model.param_spec import checkpoint_spec, synthetic_state_dict
 
@@ -43,13 +40,7 @@ class DEVA(nn.Module):
                 node.register_parameter(leaf, nn.Parameter(init[name].clone(), requires_grad=False))
         self._engine = None
         self._engine_key = None
-        # 'native' = hand-written sm_90a conv stack (default); 'torch' = cuDNN/ATen fp32 (debug / comparison only)
-        self.conv_backend = os.environ.get('DEVA_B200_CONV', 'native')
         self.return_full_logits = True  # segment() also returns the up-sampled logits like the reference
-
-    @property
-    def prefers_nhwc(self) -> bool:
-        return self.conv_backend == 'native'
 
     # ------------------------------------------------------------------ weights
     def load_weights(self, src_dict: Dict[str, torch.Tensor]) -> None:
@@ -61,7 +52,7 @@ class DEVA(nn.Module):
         return super()._apply(fn, *args, **kwargs)
 
     @property
-    def engine(self) -> Engine:
+    def engine(self) -> NativeEngine:
         probe = self.key_proj.key_proj.weight
         key = (probe.device, probe.data_ptr(), probe._version)
         if self._engine is None or self._engine_key != key:
@@ -69,14 +60,16 @@ class DEVA(nn.Module):
                 raise RuntimeError('deva_b200: the network runs on a CUDA device only (call .cuda()); '
                                    'there is no CPU fallback')
             with torch.no_grad():
-                cls = NativeEngine if self.conv_backend == 'native' else Engine
-                self._engine = cls({k: v.detach() for k, v in self.state_dict().items()})
+                self._engine = NativeEngine({k: v.detach() for k, v in self.state_dict().items()})
             self._engine_key = key
         return self._engine
 
     # ------------------------------------------------------------------ reference API
     def aggregate(self, prob: torch.Tensor, dim: int) -> torch.Tensor:
-        return Engine.aggregate(prob, dim)
+        """Soft aggregation (network.py:33-40), always fp32."""
+        prob = prob.float()
+        full = torch.cat([torch.prod(1 - prob, dim=dim, keepdim=True), prob], dim).clamp(1e-7, 1 - 1e-7)
+        return torch.log(full / (1 - full))
 
     @torch.no_grad()
     def encode_image(self, image: torch.Tensor) -> Tuple[Iterable[torch.Tensor], torch.Tensor]:
@@ -142,7 +135,7 @@ class DEVA(nn.Module):
             raise NotImplementedError('need_aux is a training-time head; this engine is inference only')
         sensory, logits = self.engine.decode(multi_scale_features, memory_readout, sensory, last_mask,
                                              update_sensory=update_sensory, chunk_size=chunk_size)
-        if self.conv_backend == 'native' and selector is None and not independent_objects:
+        if selector is None and not independent_objects:
             full_logits, prob = self.engine.probabilities(logits, want_logits=self.return_full_logits)
             return sensory, full_logits, prob
         logits = logits.float()
