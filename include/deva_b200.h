@@ -27,7 +27,9 @@
 extern "C" {
 #endif
 
-/* v27: deva_b200_conv2d takes flat spatial tiles, th = 0 and tw = 128 (stride 1, no out_pool4): 128 consecutive output
+/* v28: deva_b200_sim_topk_wide(_workspace_bytes), deva_b200_merge_lists_wide, deva_b200_readout_sparse_wide(_workspace_bytes)
+ * and deva_b200_readout_sparse_scatter_wide (memory reads at any top_k, top-k lists at a caller-given pitch ld_list).
+ * v27: deva_b200_conv2d takes flat spatial tiles, th = 0 and tw = 128 (stride 1, no out_pool4): 128 consecutive output
  * pixels of one image in row-major order.
  * v26: deva_b200_pil_resample_u8 and deva_b200_mask_nearest_ids (the dataset readers' soft masks and detection masks
  * resized on the device).
@@ -51,8 +53,8 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 27
-#define DEVA_B200_LIST_PITCH 32 /* row pitch of top-k outputs == max supported top_k */
+#define DEVA_B200_ABI_VERSION 28
+#define DEVA_B200_LIST_PITCH 32 /* row pitch of deva_b200_sim_topk's outputs == its max top_k (wider: the _wide calls) */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
 #define DEVA_B200_MASK_SMEM_COUNTERS 8192 /* per-mask counters of one mask call kept in shared memory, else global */
@@ -132,6 +134,34 @@ DEVA_B200_API int deva_b200_merge_lists(const float* part_val, const int32_t* pa
 /* get_similarity + do_softmax without top-k (max-subtracted branch, memory_utils.py:66-71) as used by
  * MemoryManager.consolidation (memory_manager.py:262-273).  sim_ws: [q, ld_sim] fp32 scratch;
  * affinity: [q, ld_affinity] fp16;  shr_out[q] = sum_n affinity[q,n]*shrinkage[n] (optional). */
+/* ---- wide read: the same read at any top_k (1 <= top_k <= n_window - n_lead), lists at pitch ld_list --------------
+ * deva_b200_sim_topk_wide: the similarity of deva_b200_sim_dense_softmax (same kernel, same fp32 values) written to
+ * workspace (deva_b200_sim_topk_wide_workspace_bytes(q, n_window) bytes: q rows of n_window rounded up to 32 floats),
+ * then per query an exact radix select of the top_k slots of [n_lead, n_window) under (similarity descending, slot
+ * ascending) - the tie rule of deva_b200_sim_topk, so for top_k <= 32 both select the same set - and the softmax
+ * (max-subtracted, fp32) over them.
+ *   out_idx/out_w (and out_sim, optional): [q, ld_list] int32 / fp32, ld_list a multiple of 32 and >= top_k; entries
+ *     0 .. top_k-1 hold the selected slots in ASCENDING SLOT order (not by similarity), entries beyond are slot 0,
+ *     weight 0, similarity -inf;
+ *   affinity, use_cnt, life_cnt, n_long, count_long, count_work: as deva_b200_sim_topk.  There is no warm start.
+ * A row of up to 24576 candidates is kept in shared memory during the select; a longer one is re-read from global
+ * memory by every radix pass.  Errors: top_k < 1, top_k > n_window - n_lead, a bad ld_list.
+ *
+ * deva_b200_merge_lists_wide: deva_b200_merge_lists at any top_k: part_val/part_idx [n_lists][ld_list][q_pitch]
+ * (n_lists <= 16, n_lists * ld_list <= 16384, idx < 0 = empty entry; the slot ids of one query must be distinct);
+ * outputs [q, ld_list] as above, the selected candidates in input order (list by list, entry by entry), the same
+ * order on every rank that passes the same lists.  If a query has fewer than top_k non-empty candidates, all of them
+ * are taken and the remaining entries are empty. */
+DEVA_B200_API size_t deva_b200_sim_topk_wide_workspace_bytes(int q, int n_window);
+DEVA_B200_API int deva_b200_sim_topk_wide(const void* k_hi, const void* k_lo, const float* neg_s, int n_window,
+                                          int n_lead, const void* q_hi, const void* q_lo, const float* bsq, int q, int ck,
+                                          int top_k, void* workspace, int32_t* out_idx, float* out_w, int ld_list,
+                                          void* affinity, int64_t ld_affinity, float* use_cnt, float* life_cnt,
+                                          int n_long, int count_long, int count_work, float* out_sim,
+                                          deva_stream_t stream);
+DEVA_B200_API int deva_b200_merge_lists_wide(const float* part_val, const int32_t* part_idx, int n_lists, int ld_list,
+                                             int top_k, int q, int q_pitch, int32_t* out_idx, float* out_w,
+                                             float* out_sim, deva_stream_t stream);
 DEVA_B200_API int deva_b200_sim_dense_softmax(const void* k_hi, const void* k_lo, const float* neg_s, const float* shrinkage,
                                 int n_window, int n_lead, const void* q_hi, const void* q_lo, const float* bsq,
                                 int q, int ck, float* sim_ws, int64_t ld_sim, void* affinity, int64_t ld_affinity,
@@ -158,6 +188,21 @@ DEVA_B200_API int deva_b200_readout_sparse(const void* values, int64_t values_ld
                                            int rows_per_group, const int32_t* idx, const float* w, int top_k,
                                            int n_window, int q, void* workspace, float* out, int64_t ld_out,
                                            void* out_tok, deva_stream_t stream);
+/* The sparse read-outs with lists at pitch ld_list (a multiple of 32, top_k <= ld_list): the lists of
+ * deva_b200_sim_topk_wide / deva_b200_merge_lists_wide.  workspace: deva_b200_readout_sparse_wide_workspace_bytes(q,
+ * n_window, ld_list) bytes.  With ld_list = 32 they equal deva_b200_readout_sparse(_scatter). */
+DEVA_B200_API size_t deva_b200_readout_sparse_wide_workspace_bytes(int q, int n_window, int ld_list);
+DEVA_B200_API int deva_b200_readout_sparse_wide(const void* values, int64_t values_ld, int64_t values_rows,
+                                                const int32_t* val_row, const int32_t* out_row, int n_groups,
+                                                int rows_per_group, const int32_t* idx, const float* w, int ld_list,
+                                                int top_k, int n_window, int q, void* workspace, float* out,
+                                                int64_t ld_out, void* out_tok, deva_stream_t stream);
+DEVA_B200_API int deva_b200_readout_sparse_scatter_wide(const void* values, int64_t values_ld, int64_t values_rows,
+                                                        const int32_t* val_row, const int32_t* out_row,
+                                                        const int32_t* owner, int n_groups, int rows_per_group,
+                                                        const int32_t* idx, const float* w, int ld_list, int top_k,
+                                                        int n_window, int q, void* workspace, float* const* rank_dst,
+                                                        int n_ranks, int64_t ld_out, deva_stream_t stream);
 /* Bank-sharded read (one video, slots split over the ranks of an NVLink box; SURVEY 8e): readout GEMM fused with the
  * reduce-scatter by object.  Each rank multiplies ITS slots; the tile of group g is added (red.add.f32, system scope)
  * straight from the GEMM epilogue into rank_dst[owner[g]] + out_row[g] * ld_out, the fp32 [objects_owned * cv, q]

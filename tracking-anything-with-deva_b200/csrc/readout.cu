@@ -180,12 +180,13 @@ readout_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_constant_
 
 
 // ======================================================================================================
-// Fused sparse-affinity readout.  The affinity has top_k (<= 32) non-zeros per query, so instead of reading a
+// Fused sparse-affinity readout.  The affinity has top_k non-zeros per query, so instead of reading a
 // dense [Q, N] fp16 operand from HBM/L2 the B tile (256 queries x 64 slots, 128B-swizzled K-major) is BUILT IN
 // SHARED MEMORY from the top-k lists: stage buffers are zeroed once, a generator warp scatters the ~50 non-zero
 // weights of the current k-block, and clears exactly those again when the stage is recycled.  Only the value
 // operand streams through TMA (16 KB instead of 48 KB per k-iteration), and no dense affinity is ever written.
-// The lists are pre-bucketed per (256-query tile, 64-slot k-block) by bucket_kernel.
+// The lists (rows of ld_list entries: 32 for deva_b200_sim_topk's, wider for the wide read) are pre-bucketed per
+// (256-query tile, 64-slot k-block) by bucket_kernel.
 // ======================================================================================================
 constexpr int SP_THREADS = CONSUMER_THREADS + 128;  // warps: 0-7 consumers, 8-11 value TMA + affinity generators (one per stage)
 constexpr int SP_REC = 1024;      // per-stage record of scattered offsets (falls back to a full clear beyond)
@@ -193,20 +194,20 @@ constexpr int SP_SMEM = STAGES * STAGE_BYTES + 1024 + 256 + STAGES * SP_REC * 2;
 
 // entry = (query_local << 24) | (slot_local << 16) | fp16 weight bits
 __global__ void __launch_bounds__(256)
-bucket_kernel(const int* __restrict__ idx, const float* __restrict__ w, int q, int top_k, int k_blocks,
+bucket_kernel(const int* __restrict__ idx, const float* __restrict__ w, int ld_list, int q, int top_k, int k_blocks,
               int* __restrict__ offsets, uint32_t* __restrict__ entries) {
   extern __shared__ int hist[];  // [k_blocks + 1]
   const int tile = blockIdx.x;
   const int q0 = tile * BN;
   const int nq = min(BN, q - q0);
   int* off = offsets + (long long)tile * (k_blocks + 1);
-  uint32_t* ent = entries + (long long)tile * BN * kListCap;
+  uint32_t* ent = entries + (long long)tile * BN * ld_list;
   for (int i = threadIdx.x; i <= k_blocks; i += 256) hist[i] = 0;
   __syncthreads();
   const int total = nq * top_k;
   for (int i = threadIdx.x; i < total; i += 256) {
     const int ql = i / top_k, j = i - ql * top_k;
-    const long long e = (long long)(q0 + ql) * kListCap + j;
+    const long long e = (long long)(q0 + ql) * ld_list + j;
     if (w[e] != 0.f) atomicAdd(&hist[idx[e] / BK + 1], 1);  // zero-weight entries (padding, other shards' slots) are dropped
   }
   __syncthreads();
@@ -217,11 +218,12 @@ bucket_kernel(const int* __restrict__ idx, const float* __restrict__ w, int q, i
   __syncthreads();
   for (int i = threadIdx.x; i < total; i += 256) {
     const int ql = i / top_k, j = i - ql * top_k;
-    if (w[(long long)(q0 + ql) * kListCap + j] == 0.f) continue;
-    const int n = idx[(long long)(q0 + ql) * kListCap + j];
+    const long long e = (long long)(q0 + ql) * ld_list + j;
+    if (w[e] == 0.f) continue;
+    const int n = idx[e];
     const int kb = n / BK;
     const int pos = atomicAdd(&hist[kb], 1);
-    const uint32_t hw = __half_as_ushort(__float2half_rn(w[(long long)(q0 + ql) * kListCap + j]));
+    const uint32_t hw = __half_as_ushort(__float2half_rn(w[e]));
     ent[pos] = ((uint32_t)ql << 24) | ((uint32_t)(n - kb * BK) << 16) | hw;
   }
 }
@@ -234,7 +236,8 @@ struct SpParams {
   __half* out_tok;
   int rows_per_group;
   const int* offsets;        // [n_tiles][k_blocks + 1]
-  const uint32_t* entries;   // [n_tiles][BN * kListCap]
+  const uint32_t* entries;   // [n_tiles][BN * ld_list]
+  int ld_list;
   int val_row[kMaxGroups];
   int out_row[kMaxGroups];
   // scatter-reduce mode (bank-sharded read): group g's tile is ADDED (red.add over NVLink / locally) into the buffer
@@ -298,7 +301,7 @@ readout_sparse_kernel(const __grid_constant__ CUtensorMap map_v, const __grid_co
       int m, n;
       tile_coords(tile, p.m_tiles, p.n_tiles, m, n);
       const int* off = p.offsets + (long long)n * (p.k_blocks + 1);
-      const uint32_t* ent = p.entries + (long long)n * BN * kListCap;
+      const uint32_t* ent = p.entries + (long long)n * BN * p.ld_list;
       const int e0 = off[kb], cnt = off[kb + 1] - e0;
       uint32_t e_a = 0, e_b = 0;   // first 64 entries prefetched before the stage is free
       if (lane < cnt) e_a = ent[e0 + lane];
@@ -418,10 +421,14 @@ DEVA_B200_API int deva_b200_readout(const void* values, int64_t values_ld, int64
   return 0;
 }
 
-DEVA_B200_API size_t deva_b200_readout_sparse_workspace_bytes(int q, int n_window) {
+DEVA_B200_API size_t deva_b200_readout_sparse_wide_workspace_bytes(int q, int n_window, int ld_list) {
   const size_t n_tiles = (q + readout::BN - 1) / readout::BN;
   const size_t k_blocks = (n_window + readout::BK - 1) / readout::BK;
-  return n_tiles * ((k_blocks + 1) * 4 + (size_t)readout::BN * kListCap * 4) + 256;
+  return n_tiles * ((k_blocks + 1) * 4 + (size_t)readout::BN * ld_list * 4) + 256;
+}
+
+DEVA_B200_API size_t deva_b200_readout_sparse_workspace_bytes(int q, int n_window) {
+  return deva_b200_readout_sparse_wide_workspace_bytes(q, n_window, kListCap);
 }
 
 }  // extern "C"
@@ -430,7 +437,8 @@ DEVA_B200_API size_t deva_b200_readout_sparse_workspace_bytes(int q, int n_windo
 // rank_dst[owner[g]] + out_row[g] * ld_out instead of stored to `out`).
 static int readout_sparse(const void* values, int64_t values_ld, int64_t values_rows, const int32_t* val_row,
                           const int32_t* out_row, const int32_t* owner, int n_groups, int rows_per_group,
-                          const int32_t* idx, const float* w, int top_k, int n_window, int q, void* workspace, float* out,
+                          const int32_t* idx, const float* w, int ld_list, int top_k, int n_window, int q,
+                          void* workspace, float* out,
                           float* const* rank_dst, int n_ranks, int64_t ld_out, void* out_tok, deva_stream_t stream) {
   using namespace readout;
   const cudaStream_t s = S(stream);
@@ -438,7 +446,7 @@ static int readout_sparse(const void* values, int64_t values_ld, int64_t values_
                "readout: scatter-reduce needs owners and 1..%d destination ranks", kMaxPeers);
   B200_REQUIRE(n_groups >= 1 && n_groups <= kMaxGroups, "readout: n_groups %d out of range [1,%d]", n_groups, kMaxGroups);
   B200_REQUIRE(rows_per_group % BM == 0, "readout: rows_per_group %d must be a multiple of %d", rows_per_group, BM);
-  B200_REQUIRE(n_window >= 1 && q >= 1 && top_k >= 1 && top_k <= kListCap, "readout: bad shape");
+  B200_REQUIRE(n_window >= 1 && q >= 1 && top_k >= 1 && top_k <= ld_list && ld_list % 32 == 0, "readout: bad shape");
   B200_REQUIRE(values_ld % 8 == 0, "readout: leading dimension must be a multiple of 8 halves");
   const char* err = nullptr;
   CUtensorMap map_v;
@@ -454,7 +462,7 @@ static int readout_sparse(const void* values, int64_t values_ld, int64_t values_
   p.q = q; p.ldo = ld_out; p.out = out; p.out_tok = H(out_tok); p.rows_per_group = rows_per_group;
   int* offsets = reinterpret_cast<int*>(workspace);
   uint32_t* entries = reinterpret_cast<uint32_t*>(offsets + (size_t)p.n_tiles * (p.k_blocks + 1));
-  p.offsets = offsets; p.entries = entries;
+  p.offsets = offsets; p.entries = entries; p.ld_list = ld_list;
   for (int i = 0; i < n_groups; ++i) { p.val_row[i] = val_row[i]; p.out_row[i] = out_row[i]; }
   p.reduce = rank_dst != nullptr;
   if (rank_dst) {
@@ -472,7 +480,8 @@ static int readout_sparse(const void* values, int64_t values_ld, int64_t values_
     B200_CUDA(cudaFuncSetAttribute(bucket_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     configured = true;
   }
-  bucket_kernel<<<p.n_tiles, 256, (p.k_blocks + 1) * sizeof(int), s>>>(idx, w, q, top_k, p.k_blocks, offsets, entries);
+  bucket_kernel<<<p.n_tiles, 256, (p.k_blocks + 1) * sizeof(int), s>>>(idx, w, ld_list, q, top_k, p.k_blocks, offsets,
+                                                                        entries);
   B200_LAUNCH_CHECK();
   const int total = p.m_tiles * p.n_tiles;
   const int grid = total < sm_count() ? total : sm_count();
@@ -488,8 +497,8 @@ DEVA_B200_API int deva_b200_readout_sparse(const void* values, int64_t values_ld
                                            int rows_per_group, const int32_t* idx, const float* w, int top_k,
                                            int n_window, int q, void* workspace, float* out, int64_t ld_out,
                                            void* out_tok, deva_stream_t stream) {
-  return readout_sparse(values, values_ld, values_rows, val_row, out_row, nullptr, n_groups, rows_per_group, idx, w, top_k,
-                        n_window, q, workspace, out, nullptr, 0, ld_out, out_tok, stream);
+  return readout_sparse(values, values_ld, values_rows, val_row, out_row, nullptr, n_groups, rows_per_group, idx, w,
+                        kListCap, top_k, n_window, q, workspace, out, nullptr, 0, ld_out, out_tok, stream);
 }
 
 DEVA_B200_API int deva_b200_readout_sparse_scatter(const void* values, int64_t values_ld, int64_t values_rows,
@@ -498,8 +507,27 @@ DEVA_B200_API int deva_b200_readout_sparse_scatter(const void* values, int64_t v
                                                    const int32_t* idx, const float* w, int top_k, int n_window, int q,
                                                    void* workspace, float* const* rank_dst, int n_ranks,
                                                    int64_t ld_out, deva_stream_t stream) {
-  return readout_sparse(values, values_ld, values_rows, val_row, out_row, owner, n_groups, rows_per_group, idx, w, top_k,
-                        n_window, q, workspace, nullptr, rank_dst, n_ranks, ld_out, nullptr, stream);
+  return readout_sparse(values, values_ld, values_rows, val_row, out_row, owner, n_groups, rows_per_group, idx, w,
+                        kListCap, top_k, n_window, q, workspace, nullptr, rank_dst, n_ranks, ld_out, nullptr, stream);
+}
+
+DEVA_B200_API int deva_b200_readout_sparse_wide(const void* values, int64_t values_ld, int64_t values_rows,
+                                                const int32_t* val_row, const int32_t* out_row, int n_groups,
+                                                int rows_per_group, const int32_t* idx, const float* w, int ld_list,
+                                                int top_k, int n_window, int q, void* workspace, float* out,
+                                                int64_t ld_out, void* out_tok, deva_stream_t stream) {
+  return readout_sparse(values, values_ld, values_rows, val_row, out_row, nullptr, n_groups, rows_per_group, idx, w,
+                        ld_list, top_k, n_window, q, workspace, out, nullptr, 0, ld_out, out_tok, stream);
+}
+
+DEVA_B200_API int deva_b200_readout_sparse_scatter_wide(const void* values, int64_t values_ld, int64_t values_rows,
+                                                        const int32_t* val_row, const int32_t* out_row,
+                                                        const int32_t* owner, int n_groups, int rows_per_group,
+                                                        const int32_t* idx, const float* w, int ld_list, int top_k,
+                                                        int n_window, int q, void* workspace, float* const* rank_dst,
+                                                        int n_ranks, int64_t ld_out, deva_stream_t stream) {
+  return readout_sparse(values, values_ld, values_rows, val_row, out_row, owner, n_groups, rows_per_group, idx, w,
+                        ld_list, top_k, n_window, q, workspace, nullptr, rank_dst, n_ranks, ld_out, nullptr, stream);
 }
 
 }  // extern "C"

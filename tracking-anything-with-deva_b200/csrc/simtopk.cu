@@ -412,6 +412,241 @@ __global__ void tick_kernel(float* __restrict__ life, int n) {
   if (i < n) life[i] += 1.f;
 }
 
+// ======================================================================================================
+// Wide selection (any top_k, in particular beyond the kListCap-entry running lists of simtopk_kernel).  One CTA per
+// query selects exactly the top_k of its candidates under (similarity descending, slot ascending) by a radix select on
+// the order-preserving uint32 image of the fp32 similarity: 8-bit digits from the top, each pass a shared-memory
+// histogram of the candidates that still match the prefix, stopping as soon as the threshold digit's bin holds exactly
+// the entries still needed.  If more candidates than needed share the threshold value, a second radix select over their
+// slots (ascending) keeps the lowest ones.  A compaction pass then writes the selected entries in candidate order, and
+// the softmax (max-subtracted, fp32), usage and affinity scatter follow over the top_k written entries.
+// Candidates are either a dense similarity row (written by simtopk_kernel<true>; kept in shared memory when it fits,
+// else re-read from global memory / L2 by every pass) or n candidate lists with explicit slot ids (the cross-rank merge).
+// ======================================================================================================
+constexpr int WIDE_THREADS = 512;
+constexpr int WIDE_WARPS = WIDE_THREADS / 32;
+constexpr int kWideRowCache = 24576;  // dense rows up to this many slots are kept in shared memory (96 KiB)
+constexpr int kWideMergeCap = 16384;  // candidates per query of one list merge, kept in shared memory (128 KiB)
+enum WideMode { WIDE_ROW_GLOBAL = 0, WIDE_ROW_SMEM = 1, WIDE_LISTS = 2 };
+
+struct WideParams {
+  const float* sim;        // rows: [q][ld_sim], slots [n_lead, n_window) are the candidates
+  long long ld_sim;
+  int n_lead, n_window;
+  const float* part_val;   // lists: [n_cand][q_pitch] values and slot ids (id < 0 = empty)
+  const int* part_idx;
+  int n_cand, q_pitch;
+  int q, top_k, ld_list;
+  int* out_idx;            // [q][ld_list]
+  float* out_w;
+  float* out_sim;
+  __half* P;               // optional [q][ldP]
+  long long ldP;
+  float* use_cnt;          // optional [n_window]
+  int n_long, add_long, add_work;
+};
+
+// -0 is mapped to +0 first: the order compares values, so the two zeros tie and their slots decide, as in merge_kernel.
+__device__ __forceinline__ uint32_t order_key(float v) {
+  const uint32_t b = __float_as_uint(v == 0.f ? 0.f : v);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float key_value(uint32_t k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// Every lane of the warp calls this; lanes with `on` add one to hist[bin], one atomic per distinct bin of the warp.
+__device__ __forceinline__ void hist_add(int* hist, uint32_t bin, bool on) {
+  const unsigned act = __ballot_sync(0xffffffffu, on);
+  if (on) {
+    const unsigned peers = __match_any_sync(act, bin);
+    if ((int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&hist[bin], __popc(peers));
+  }
+}
+
+// Radix select of the k largest keys among the candidates i < n for which get(i, key) is true.  On return the selected
+// set is { masked key > prefix } plus `k` (updated) of { masked key == prefix }; the result is true when that equal
+// set holds exactly k candidates (all taken), false when it holds more (the keys are then fully resolved: mask = ~0).
+template <class Get>
+__device__ bool radix_select(Get get, int n, int& k, uint32_t& prefix, uint32_t& mask, int* hist, int* ctl) {
+  const int lane = threadIdx.x & 31;
+  prefix = 0;
+  mask = 0;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = threadIdx.x; i < 256; i += WIDE_THREADS) hist[i] = 0;
+    __syncthreads();
+    for (int i0 = 0; i0 < n; i0 += WIDE_THREADS) {
+      const int i = i0 + threadIdx.x;
+      uint32_t key = 0;
+      const bool on = i < n && get(i, key) && (key & mask) == prefix;
+      hist_add(hist, (key >> shift) & 255u, on);
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {  // bin holding the k-th largest: lane l scans bins 255-8l .. 248-8l
+      int c[8], s = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { c[j] = hist[255 - (lane * 8 + j)]; s += c[j]; }
+      int incl = s;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+      }
+      int run = incl - s;
+      if (run < k && k <= incl) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          if (run + c[j] >= k) { ctl[0] = 255 - (lane * 8 + j); ctl[1] = run; ctl[2] = c[j]; break; }
+          run += c[j];
+        }
+      }
+    }
+    __syncthreads();
+    const uint32_t bin = (uint32_t)ctl[0];
+    const int above = ctl[1], cnt = ctl[2];
+    __syncthreads();  // ctl is rewritten by the next pass
+    prefix |= bin << shift;
+    mask |= 0xffu << shift;
+    k -= above;
+    if (cnt == k) return true;
+  }
+  return false;
+}
+
+__device__ __forceinline__ float block_sum(float v, float* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float t = 0.f;
+  for (int w = 0; w < WIDE_WARPS; ++w) t += red[w];
+  __syncthreads();
+  return t;
+}
+
+__device__ __forceinline__ float block_max(float v, float* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float t = -CUDART_INF_F;
+  for (int w = 0; w < WIDE_WARPS; ++w) t = fmaxf(t, red[w]);
+  __syncthreads();
+  return t;
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(WIDE_THREADS)
+wide_select_kernel(const __grid_constant__ WideParams p) {
+  extern __shared__ uint32_t wide_smem[];  // cached keys [n], then (lists) slot ids [n]
+  __shared__ int hist[256];
+  __shared__ int ctl[3];
+  __shared__ int wcnt[WIDE_WARPS];
+  __shared__ float red[WIDE_WARPS];
+  const int qi = blockIdx.x;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n = (MODE == WIDE_LISTS) ? p.n_cand : p.n_window - p.n_lead;
+  const float* row = (MODE == WIDE_LISTS) ? nullptr : p.sim + (long long)qi * p.ld_sim + p.n_lead;
+  uint32_t* skey = wide_smem;
+  int* sid = reinterpret_cast<int*>(wide_smem + n);
+
+  int n_active = n;
+  if (MODE != WIDE_ROW_GLOBAL) {
+    int cnt = 0;
+    for (int i = threadIdx.x; i < n; i += WIDE_THREADS) {
+      if (MODE == WIDE_LISTS) {
+        const long long off = (long long)i * p.q_pitch + qi;
+        const int id = p.part_idx[off];
+        skey[i] = order_key(p.part_val[off]);
+        sid[i] = id;
+        cnt += id >= 0;
+      } else {
+        skey[i] = order_key(row[i]);
+      }
+    }
+    if (MODE == WIDE_LISTS) n_active = (int)block_sum((float)cnt, red);  // exact: counts < 2^24
+    __syncthreads();
+  }
+  // candidate i -> (key, slot id); false for an empty list entry
+  auto fetch = [&](int i, uint32_t& key, int& id) -> bool {
+    if (MODE == WIDE_ROW_GLOBAL) { key = order_key(row[i]); id = p.n_lead + i; return true; }
+    key = skey[i];
+    if (MODE == WIDE_ROW_SMEM) { id = p.n_lead + i; return true; }
+    id = sid[i];
+    return id >= 0;
+  };
+  const int k_sel = min(p.top_k, n_active);
+  int k = k_sel;
+  uint32_t prefix = 0, mask = 0, id_prefix = 0, id_mask = 0;
+  bool exact = true;  // every candidate whose masked key equals the prefix is selected
+  if (k > 0) {
+    exact = radix_select([&](int i, uint32_t& key) { int id; return fetch(i, key, id); }, n, k, prefix, mask, hist, ctl);
+    if (!exact) {  // more candidates share the threshold value than are needed: the lowest slots win
+      const uint32_t thr = prefix;
+      radix_select(
+          [&](int i, uint32_t& key) {
+            uint32_t v; int id;
+            const bool on = fetch(i, v, id) && v == thr;
+            key = ~(uint32_t)id;
+            return on;
+          },
+          n, k, id_prefix, id_mask, hist, ctl);
+    }
+  }
+
+  // compaction in candidate order: entry e of the output = the e-th selected candidate
+  int* oi = p.out_idx + (long long)qi * p.ld_list;
+  float* ow = p.out_w + (long long)qi * p.ld_list;
+  float vmax = -CUDART_INF_F;
+  int base = 0;
+  for (int i0 = 0; i0 < n && base < k_sel; i0 += WIDE_THREADS) {
+    const int i = i0 + threadIdx.x;
+    uint32_t key = 0;
+    int id = 0;
+    bool sel = false;
+    if (i < n && fetch(i, key, id)) {
+      const uint32_t mk = key & mask;
+      sel = mk > prefix || (mk == prefix && (exact || (~(uint32_t)id & id_mask) >= id_prefix));
+    }
+    const unsigned b = __ballot_sync(0xffffffffu, sel);
+    if (lane == 0) wcnt[warp] = __popc(b);
+    __syncthreads();
+    int off = base, tot = 0;
+    for (int w = 0; w < WIDE_WARPS; ++w) {
+      off += (w < warp) ? wcnt[w] : 0;
+      tot += wcnt[w];
+    }
+    off += __popc(b & ((1u << lane) - 1u));
+    if (sel && off < k_sel) {
+      const float v = key_value(key);
+      oi[off] = id;
+      ow[off] = v;  // raw similarity for now; the weight replaces it below
+      vmax = fmaxf(vmax, v);
+    }
+    base += tot;
+    __syncthreads();
+  }
+  vmax = block_max(vmax, red);  // also orders the entries written above before the reads below
+  float s = 0.f;
+  for (int e = threadIdx.x; e < k_sel; e += WIDE_THREADS) s += expf(ow[e] - vmax);
+  s = block_sum(s, red);
+  for (int e = threadIdx.x; e < p.ld_list; e += WIDE_THREADS) {
+    if (e < k_sel) {
+      const int id = oi[e];
+      const float v = ow[e];
+      const float w = expf(v - vmax) / s;
+      ow[e] = w;
+      if (p.out_sim) p.out_sim[(long long)qi * p.ld_list + e] = v;
+      if (p.P) p.P[(long long)qi * p.ldP + id] = __float2half_rn(w);
+      if (p.use_cnt && ((id < p.n_long) ? p.add_long : p.add_work)) atomicAdd(p.use_cnt + id, w);
+    } else {
+      oi[e] = 0;
+      ow[e] = 0.f;
+      if (p.out_sim) p.out_sim[(long long)qi * p.ld_list + e] = -CUDART_INF_F;
+    }
+  }
+}
+
 }  // namespace simtopk
 
 namespace simtopk {
@@ -495,6 +730,72 @@ static int choose_split(int q_tiles, int tiles, int max_split) {
   return best;
 }
 
+
+// sim[q][ld_sim] (fp32, columns < n_window; slots < n_lead hold -inf) by the DENSE instantiation of simtopk_kernel: the
+// similarity of deva_b200_sim_dense_softmax and of the wide top-k read.
+static int dense_similarity(const __half* kh, const __half* kl, const float* neg_s, int n_window, int n_lead,
+                            const __half* qh, const __half* ql, const float* bsq, int q, int ck, float* sim,
+                            long long ld_sim, cudaStream_t s) {
+  using namespace simtopk;
+  CUtensorMap maps[4];
+  if (int rc = make_maps(maps, qh, ql, q, kh, kl, n_window, ck)) return rc;
+  Params p{};
+  p.q = q; p.n_window = n_window; p.n_lead = n_lead; p.kblocks = 2 * ck / 64; p.top_k = 1;
+  p.tiles_total = ceil_div(n_window, BNK);
+  const int q_tiles = ceil_div(q, BQ);
+  int nsplit = ceil_div(sm_count(), q_tiles);
+  if (nsplit > p.tiles_total) nsplit = p.tiles_total;
+  p.tiles_per_split = ceil_div(p.tiles_total, nsplit);
+  nsplit = ceil_div(p.tiles_total, p.tiles_per_split);
+  p.qpad = q_tiles * BQ;
+  p.neg_s = neg_s; p.bsq = bsq;
+  p.dense_out = sim; p.ld_dense = ld_sim;
+  static bool configured_dev[kMaxDevices] = {false};  // function attributes are per device
+  bool& configured = configured_dev[device_slot()];
+  if (!configured) {
+    B200_CUDA(cudaFuncSetAttribute(simtopk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    configured = true;
+  }
+  simtopk_kernel<true><<<dim3(q_tiles, nsplit), THREADS, SMEM_BYTES, s>>>(maps[0], maps[1], maps[2], maps[3], p);
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+
+// One wide_select_kernel launch per query: rows cached in shared memory when they fit, candidate lists always.
+static int wide_select(simtopk::WideParams& p, int n, cudaStream_t s) {
+  using namespace simtopk;
+  static bool configured_dev[kMaxDevices] = {false};  // function attributes are per device
+  bool& configured = configured_dev[device_slot()];
+  if (!configured) {
+    B200_CUDA(cudaFuncSetAttribute(wide_select_kernel<WIDE_ROW_SMEM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   kWideRowCache * 4));
+    B200_CUDA(cudaFuncSetAttribute(wide_select_kernel<WIDE_LISTS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   kWideMergeCap * 8));
+    configured = true;
+  }
+  if (p.sim == nullptr) {
+    wide_select_kernel<WIDE_LISTS><<<p.q, WIDE_THREADS, (size_t)n * 8, s>>>(p);
+  } else if (n <= kWideRowCache) {
+    wide_select_kernel<WIDE_ROW_SMEM><<<p.q, WIDE_THREADS, (size_t)n * 4, s>>>(p);
+  } else {
+    wide_select_kernel<WIDE_ROW_GLOBAL><<<p.q, WIDE_THREADS, 0, s>>>(p);
+  }
+  B200_LAUNCH_CHECK();
+  return 0;
+}
+
+static int tick_life(float* life_cnt, int n_lead, int n_long, int n_window, int count_long, int count_work,
+                      cudaStream_t s) {
+  // life += 1 for every slot whose usage is being counted (kv_memory_store.py:118-125)
+  const int lo = count_long ? n_lead : n_long;
+  const int hi = count_work ? n_window : n_long;
+  if (hi > lo) {
+    simtopk::tick_kernel<<<ceil_div(hi - lo, 256), 256, 0, s>>>(life_cnt + lo, hi - lo);
+    B200_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -557,13 +858,7 @@ DEVA_B200_API int deva_b200_sim_topk(const void* k_hi, const void* k_lo, const f
       count_work, out_sim);
   B200_LAUNCH_CHECK();
   if (life_cnt) {
-    // life += 1 for every slot whose usage is being counted (kv_memory_store.py:118-125)
-    const int lo = count_long ? n_lead : n_long;
-    const int hi = count_work ? n_window : n_long;
-    if (hi > lo) {
-      tick_kernel<<<ceil_div(hi - lo, 256), 256, 0, s>>>(life_cnt + lo, hi - lo);
-      B200_LAUNCH_CHECK();
-    }
+    if (int rc = tick_life(life_cnt, n_lead, n_long, n_window, count_long, count_work, s)) return rc;
   }
   return 0;
 }
@@ -594,30 +889,72 @@ DEVA_B200_API int deva_b200_sim_dense_softmax(const void* k_hi, const void* k_lo
   const cudaStream_t s = S(stream);
   B200_REQUIRE(ck == 32 || ck == 64, "simdense: key_dim %d unsupported (32 or 64)", ck);
   B200_REQUIRE(q >= 1 && n_window > n_lead && n_lead >= 0 && n_lead < 8, "simdense: bad shape");
-  CUtensorMap maps[4];
-  if (int rc = make_maps(maps, qh, ql, q, kh, kl, n_window, ck)) return rc;
-  Params p{};
-  p.q = q; p.n_window = n_window; p.n_lead = n_lead; p.kblocks = 2 * ck / 64; p.top_k = 1;
-  p.tiles_total = ceil_div(n_window, BNK);
-  const int q_tiles = ceil_div(q, BQ);
-  int nsplit = ceil_div(sm_count(), q_tiles);
-  if (nsplit > p.tiles_total) nsplit = p.tiles_total;
-  p.tiles_per_split = ceil_div(p.tiles_total, nsplit);
-  nsplit = ceil_div(p.tiles_total, p.tiles_per_split);
-  p.qpad = q_tiles * BQ;
-  p.neg_s = neg_s; p.bsq = bsq;
-  p.dense_out = sim_ws; p.ld_dense = ld_sim;
-  static bool configured_dev[kMaxDevices] = {false};  // function attributes are per device
-  bool& configured = configured_dev[device_slot()];
-  if (!configured) {
-    B200_CUDA(cudaFuncSetAttribute(simtopk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    configured = true;
-  }
-  simtopk_kernel<true><<<dim3(q_tiles, nsplit), THREADS, SMEM_BYTES, s>>>(maps[0], maps[1], maps[2], maps[3], p);
-  B200_LAUNCH_CHECK();
+  if (int rc = dense_similarity(kh, kl, neg_s, n_window, n_lead, qh, ql, bsq, q, ck, sim_ws, ld_sim, s)) return rc;
   row_softmax_kernel<<<q, 256, 0, s>>>(sim_ws, ld_sim, n_window, shrinkage, P, ld_affinity, shr_out);
   B200_LAUNCH_CHECK();
   return 0;
+}
+
+
+// ---- wide top-k read (any top_k; the path for top_k > kListCap) ----
+static long long wide_ld_sim(int n_window) { return ((long long)n_window + 31) / 32 * 32; }
+
+DEVA_B200_API size_t deva_b200_sim_topk_wide_workspace_bytes(int q, int n_window) {
+  if (q < 1 || n_window < 1) return 0;
+  return (size_t)q * (size_t)wide_ld_sim(n_window) * sizeof(float);
+}
+
+DEVA_B200_API int deva_b200_sim_topk_wide(const void* k_hi, const void* k_lo, const float* neg_s, int n_window,
+                                          int n_lead, const void* q_hi, const void* q_lo, const float* bsq, int q, int ck,
+                                          int top_k, void* workspace, int32_t* out_idx, float* out_w, int ld_list,
+                                          void* affinity, int64_t ld_affinity, float* use_cnt, float* life_cnt,
+                                          int n_long, int count_long, int count_work, float* out_sim,
+                                          deva_stream_t stream) {
+  using namespace simtopk;
+  const cudaStream_t s = S(stream);
+  B200_REQUIRE(ck == 32 || ck == 64, "simtopk_wide: key_dim %d unsupported (32 or 64)", ck);
+  B200_REQUIRE(top_k >= 1, "simtopk_wide: top_k %d must be at least 1", top_k);
+  B200_REQUIRE(n_window - n_lead >= top_k,
+               "simtopk_wide: top_k %d exceeds the %d memory slots (the reference raises too)", top_k, n_window - n_lead);
+  B200_REQUIRE(q >= 1 && n_lead >= 0 && n_lead < 8, "simtopk_wide: bad q / n_lead");
+  B200_REQUIRE(ld_list >= top_k && ld_list % 32 == 0, "simtopk_wide: ld_list %d must be a multiple of 32 and >= top_k %d",
+               ld_list, top_k);
+  B200_REQUIRE(workspace != nullptr && out_idx != nullptr && out_w != nullptr, "simtopk_wide: missing buffer");
+  float* sim = reinterpret_cast<float*>(workspace);
+  const long long ld_sim = wide_ld_sim(n_window);
+  if (int rc = dense_similarity(H(k_hi), H(k_lo), neg_s, n_window, n_lead, H(q_hi), H(q_lo), bsq, q, ck, sim, ld_sim, s))
+    return rc;
+  __half* P = H(affinity);
+  if (P) B200_CUDA(cudaMemsetAsync(P, 0, (size_t)q * ld_affinity * sizeof(__half), s));
+  WideParams p{};
+  p.sim = sim; p.ld_sim = ld_sim; p.n_lead = n_lead; p.n_window = n_window;
+  p.q = q; p.top_k = top_k; p.ld_list = ld_list;
+  p.out_idx = out_idx; p.out_w = out_w; p.out_sim = out_sim;
+  p.P = P; p.ldP = ld_affinity;
+  p.use_cnt = use_cnt; p.n_long = n_long; p.add_long = count_long; p.add_work = count_work;
+  if (int rc = wide_select(p, n_window - n_lead, s)) return rc;
+  if (life_cnt) {
+    if (int rc = tick_life(life_cnt, n_lead, n_long, n_window, count_long, count_work, s)) return rc;
+  }
+  return 0;
+}
+
+DEVA_B200_API int deva_b200_merge_lists_wide(const float* part_val, const int32_t* part_idx, int n_lists, int ld_list,
+                                             int top_k, int q, int q_pitch, int32_t* out_idx, float* out_w,
+                                             float* out_sim, deva_stream_t stream) {
+  using namespace simtopk;
+  B200_REQUIRE(n_lists >= 1 && n_lists <= kMaxMergeLists, "merge_wide: n_lists %d out of range [1,%d]", n_lists,
+               kMaxMergeLists);
+  B200_REQUIRE(top_k >= 1 && ld_list >= top_k && ld_list % 32 == 0,
+               "merge_wide: top_k %d must be in [1, ld_list] and ld_list %d a multiple of 32", top_k, ld_list);
+  B200_REQUIRE((long long)n_lists * ld_list <= kWideMergeCap, "merge_wide: %d lists of %d entries exceed %d candidates",
+               n_lists, ld_list, kWideMergeCap);
+  B200_REQUIRE(q >= 1 && q_pitch >= q, "merge_wide: bad shape");
+  WideParams p{};
+  p.part_val = part_val; p.part_idx = part_idx; p.n_cand = n_lists * ld_list; p.q_pitch = q_pitch;
+  p.q = q; p.top_k = top_k; p.ld_list = ld_list;
+  p.out_idx = out_idx; p.out_w = out_w; p.out_sim = out_sim;
+  return wide_select(p, p.n_cand, S(stream));
 }
 
 }  // extern "C"

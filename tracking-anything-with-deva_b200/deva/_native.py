@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 27
+ABI_VERSION = 28
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -51,6 +51,12 @@ _SIGNATURES = {
                                    c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'deva_b200_merge_lists': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                       c_void_p]),
+    'deva_b200_sim_topk_wide_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'deva_b200_sim_topk_wide': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                        c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_void_p,
+                                        c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    'deva_b200_merge_lists_wide': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                           c_void_p, c_void_p]),
     'deva_b200_sim_dense_softmax': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                             c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_int64, c_void_p,
                                             c_void_p]),
@@ -63,6 +69,14 @@ _SIGNATURES = {
     'deva_b200_readout_sparse_scatter': (c_int, [c_void_p, c_int64, c_int64, POINTER(c_int32), POINTER(c_int32),
                                                  POINTER(c_int32), c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                                  c_void_p, POINTER(c_void_p), c_int, c_int64, c_void_p]),
+    'deva_b200_readout_sparse_wide_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
+    'deva_b200_readout_sparse_wide': (c_int, [c_void_p, c_int64, c_int64, POINTER(c_int32), POINTER(c_int32), c_int,
+                                              c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                              c_int64, c_void_p, c_void_p]),
+    'deva_b200_readout_sparse_scatter_wide': (c_int, [c_void_p, c_int64, c_int64, POINTER(c_int32), POINTER(c_int32),
+                                                      POINTER(c_int32), c_int, c_int, c_void_p, c_void_p, c_int, c_int,
+                                                      c_int, c_int, c_void_p, POINTER(c_void_p), c_int, c_int64,
+                                                      c_void_p]),
     'deva_b200_peer_alloc': (c_int, [c_int, c_int64, POINTER(c_void_p), c_char_p]),
     'deva_b200_peer_open': (c_int, [c_int, c_char_p, POINTER(c_void_p)]),
     'deva_b200_peer_close': (c_int, [c_int, c_void_p]),
@@ -221,6 +235,31 @@ def merge_lists(part_val, part_idx, n_lists, top_k, q, q_pitch, out_idx, out_w, 
                                        _ptr(out_w), _ptr(out_sim), _stream()), 'merge_lists')
 
 
+def list_pitch(top_k: int) -> int:
+    """Row pitch of the top-k lists of a read at ``top_k``: LIST_PITCH up to it, else top_k rounded up to 32."""
+    return max(LIST_PITCH, (top_k + 31) // 32 * 32)
+
+
+def sim_topk_wide_workspace_bytes(q, n_window):
+    return int(lib().deva_b200_sim_topk_wide_workspace_bytes(q, n_window))
+
+
+def sim_topk_wide(k_hi, k_lo, neg_s, n_window, n_lead, q_hi, q_lo, bsq, q, ck, top_k, workspace, out_idx, out_w,
+                  ld_list, affinity, ld_affinity, use_cnt, life_cnt, n_long, count_long, count_work, out_sim=None):
+    """The read at any top_k: out_idx/out_w (out_sim) [q, ld_list], selected slots in ascending slot order."""
+    _check(lib().deva_b200_sim_topk_wide(_ptr(k_hi), _ptr(k_lo), _ptr(neg_s), n_window, n_lead, _ptr(q_hi),
+                                         _ptr(q_lo), _ptr(bsq), q, ck, top_k, _ptr(workspace), _ptr(out_idx),
+                                         _ptr(out_w), ld_list, _ptr(affinity), ld_affinity, _ptr(use_cnt),
+                                         _ptr(life_cnt), n_long, int(count_long), int(count_work), _ptr(out_sim),
+                                         _stream()), 'sim_topk_wide')
+
+
+def merge_lists_wide(part_val, part_idx, n_lists, ld_list, top_k, q, q_pitch, out_idx, out_w, out_sim=None):
+    """part_val/part_idx [n_lists, ld_list, q_pitch] -> [q, ld_list] lists, the selected entries in input order."""
+    _check(lib().deva_b200_merge_lists_wide(_ptr(part_val), _ptr(part_idx), n_lists, ld_list, top_k, q, q_pitch,
+                                            _ptr(out_idx), _ptr(out_w), _ptr(out_sim), _stream()), 'merge_lists_wide')
+
+
 def sim_dense_softmax(k_hi, k_lo, neg_s, shrinkage, n_window, n_lead, q_hi, q_lo, bsq, q, ck, sim_ws, ld_sim,
                       affinity, ld_affinity, shr_out):
     _check(lib().deva_b200_sim_dense_softmax(_ptr(k_hi), _ptr(k_lo), _ptr(neg_s), _ptr(shrinkage), n_window, n_lead,
@@ -252,6 +291,31 @@ def readout_sparse(values, values_ld, values_rows, val_row, out_row, rows_per_gr
     _check(lib().deva_b200_readout_sparse(_ptr(values), values_ld, values_rows, arr_v, arr_o, n, rows_per_group,
                                           _ptr(idx), _ptr(w), top_k, n_window, q, _ptr(workspace), _ptr(out), ld_out,
                                           _ptr(out_tok), _stream()), 'readout_sparse')
+
+
+def readout_sparse_wide_workspace_bytes(q, n_window, ld_list):
+    return int(lib().deva_b200_readout_sparse_wide_workspace_bytes(q, n_window, ld_list))
+
+
+def readout_sparse_wide(values, values_ld, values_rows, val_row, out_row, rows_per_group, idx, w, ld_list, top_k,
+                        n_window, q, workspace, out, ld_out, out_tok=None):
+    n = len(val_row)
+    arr_v = (c_int32 * n)(*val_row)
+    arr_o = (c_int32 * n)(*out_row)
+    _check(lib().deva_b200_readout_sparse_wide(_ptr(values), values_ld, values_rows, arr_v, arr_o, n, rows_per_group,
+                                               _ptr(idx), _ptr(w), ld_list, top_k, n_window, q, _ptr(workspace),
+                                               _ptr(out), ld_out, _ptr(out_tok), _stream()), 'readout_sparse_wide')
+
+
+def readout_sparse_scatter_wide(values, values_ld, values_rows, val_row, out_row, owner, rows_per_group, idx, w,
+                                ld_list, top_k, n_window, q, workspace, rank_dst_ptrs, ld_out):
+    n = len(val_row)
+    arr_v, arr_o, arr_w = (c_int32 * n)(*val_row), (c_int32 * n)(*out_row), (c_int32 * n)(*owner)
+    ptrs = (c_void_p * len(rank_dst_ptrs))(*rank_dst_ptrs)
+    _check(lib().deva_b200_readout_sparse_scatter_wide(_ptr(values), values_ld, values_rows, arr_v, arr_o, arr_w, n,
+                                                       rows_per_group, _ptr(idx), _ptr(w), ld_list, top_k, n_window, q,
+                                                       _ptr(workspace), ptrs, len(rank_dst_ptrs), ld_out, _stream()),
+           'readout_sparse_scatter_wide')
 
 
 def readout_sparse_scatter(values, values_ld, values_rows, val_row, out_row, owner, rows_per_group, idx, w, top_k,

@@ -3,8 +3,8 @@
 Same class, method names, argument meaning and error behaviour as the reference's ``MemoryManager``;
 the math runs in the sm_90a kernels behind ``deva._native``:
 
-* ``match_memory``  = pack_query -> per bucket [sim_topk (fused similarity / top-k / softmax / usage)
-  -> readout GEMM] writing straight into one [K, CV, h, w] buffer in temporary-id order;
+* ``match_memory``  = pack_query -> per bucket [sim_topk (fused similarity / top-k / softmax / usage; sim_topk_wide
+  for top_k > 32) -> readout GEMM] writing straight into one [K, CV, h, w] buffer in temporary-id order;
 * ``add_memory``    = O(new tokens) append into the preallocated bank (no torch.cat);
 * ``compress_features`` / ``consolidation`` = the same kernels with the full-softmax variant.
 
@@ -132,12 +132,19 @@ class MemoryManager:
             out, out_tok = None, torch.empty(k_total, q, self.CV, dtype=torch.float16, device=dev)
         else:     # fp32 [K*CV, q]: the reference's layout
             out, out_tok = torch.empty(k_total * self.CV, q, dtype=torch.float32, device=dev), None
-        ws = self._buf('topk_ws', (nat.simtopk_workspace_bytes(q), ), torch.uint8, dev)
-        wgt = self._buf('topk_w', (q, nat.LIST_PITCH), torch.float32, dev)
-        thr_ws = self._buf('topk_thr', (q, ), torch.float32, dev)
+        # top_k beyond the 32-entry running lists of sim_topk: exact radix select over a dense similarity row, lists
+        # at a wider pitch, no warm start
+        wide = self.top_k > nat.LIST_PITCH
+        pitch = nat.list_pitch(self.top_k)
+        if wide:
+            wgt = self._buf('topk_w', (q, pitch), torch.float32, dev)
+            wide_idx = self._buf('topk_idx', (q, pitch), torch.int32, dev)
+        else:
+            ws = self._buf('topk_ws', (nat.simtopk_workspace_bytes(q), ), torch.uint8, dev)
+            wgt = self._buf('topk_w', (q, nat.LIST_PITCH), torch.float32, dev)
+            thr_ws = self._buf('topk_thr', (q, ), torch.float32, dev)
         for bank in self._banks.values():
             w0, lead, n_window = bank.window()
-            idx, prev = self._read_slots(bank, q, w0, lead, dev)
             count_work = self.use_long_term
             count_long = self.use_long_term and self.count_long_term_usage and bank.long_size > 0
             # large reads: affinity tiles are generated on chip by the readout kernel; small reads (where its fixed
@@ -147,18 +154,34 @@ class MemoryManager:
             if not fused:
                 ldp = (n_window + 7) // 8 * 8
                 aff = self._buf('affinity', (q, ldp), torch.float16, dev)
-            nat.sim_topk(bank.k_hi[w0:], bank.k_lo[w0:], bank.neg_s[w0:], n_window, lead, q_hi, q_lo, bsq, q,
-                         self.CK, self.top_k, ws, idx, wgt, aff, ldp,
-                         bank.use_cnt[w0:] if count_work else None, bank.life_cnt[w0:] if count_work else None,
-                         bank.base - w0, count_long, count_work, prev_idx=prev, thr_ws=thr_ws)
+            use = bank.use_cnt[w0:] if count_work else None
+            life = bank.life_cnt[w0:] if count_work else None
+            if wide:
+                idx = wide_idx
+                bank.read_key = None  # the next narrow read starts cold
+                ws = self._buf('topk_wide_ws', (nat.sim_topk_wide_workspace_bytes(q, n_window), ), torch.uint8, dev)
+                nat.sim_topk_wide(bank.k_hi[w0:], bank.k_lo[w0:], bank.neg_s[w0:], n_window, lead, q_hi, q_lo, bsq, q,
+                                  self.CK, self.top_k, ws, idx, wgt, pitch, aff, ldp, use, life, bank.base - w0,
+                                  count_long, count_work)
+            else:
+                idx, prev = self._read_slots(bank, q, w0, lead, dev)
+                nat.sim_topk(bank.k_hi[w0:], bank.k_lo[w0:], bank.neg_s[w0:], n_window, lead, q_hi, q_lo, bsq, q,
+                             self.CK, self.top_k, ws, idx, wgt, aff, ldp, use, life,
+                             bank.base - w0, count_long, count_work, prev_idx=prev, thr_ws=thr_ws)
             objs = bank.objects
             if fused:
-                rws = self._buf('readout_ws', (nat.readout_sparse_workspace_bytes(q, n_window), ), torch.uint8, dev)
+                rws_bytes = nat.readout_sparse_wide_workspace_bytes(q, n_window, pitch) if wide else \
+                    nat.readout_sparse_workspace_bytes(q, n_window)
+                rws = self._buf('readout_ws', (rws_bytes, ), torch.uint8, dev)
             for i in range(0, len(objs), nat.MAX_GROUPS):
                 part = objs[i:i + nat.MAX_GROUPS]
                 rows_v = [bank.slot_of[o] * self.CV for o in part]
                 rows_o = [order[o] * self.CV for o in part]
-                if fused:
+                if fused and wide:
+                    nat.readout_sparse_wide(bank.values[:, :, w0:], bank.cap, bank.values.shape[0] * self.CV, rows_v,
+                                            rows_o, self.CV, idx, wgt, pitch, self.top_k, n_window, q, rws, out, q,
+                                            out_tok)
+                elif fused:
                     nat.readout_sparse(bank.values[:, :, w0:], bank.cap, bank.values.shape[0] * self.CV, rows_v, rows_o,
                                        self.CV, idx, wgt, self.top_k, n_window, q, rws, out, q, out_tok)
                 else:

@@ -151,7 +151,9 @@ class ShardedMemoryManager(MemoryManager):
         order = {obj: i for i, obj in enumerate(self._object_order())}
         k_total = len(order)
         per = -(-k_total // self.world)
-        pitch = nat.LIST_PITCH
+        # top_k > 32: every rank keeps up to top_k local candidates in lists of the wider pitch, merged by the wide kernel
+        wide = self.top_k > nat.LIST_PITCH
+        pitch = nat.list_pitch(self.top_k)
         if self._peers is None or tuple(self._peers.local.shape) != (per * self.CV, q):
             if self._peers is not None:
                 self._peers.close()
@@ -172,21 +174,34 @@ class ShardedMemoryManager(MemoryManager):
             stride = 1 << 24
             assert n_window < stride
             k_loc = min(self.top_k, n_loc)
-            l_idx, prev = self._read_slots(bank, q, w0, lead, dev)  # the LOCAL top-k of the previous frame bounds this one's
-            if bank.read_key is not None and getattr(bank, 'read_k', None) != k_loc:
-                prev = None
-            bank.read_k = k_loc
-            if k_loc > 0:
+            if wide:
+                l_idx = self._buf('l_idx_wide', (q, pitch), torch.int32, dev)
+                bank.read_key = None  # the next narrow read starts cold
+            else:
+                l_idx, prev = self._read_slots(bank, q, w0, lead, dev)  # the LOCAL top-k of the previous frame bounds this one's
+                if bank.read_key is not None and getattr(bank, 'read_k', None) != k_loc:
+                    prev = None
+                bank.read_k = k_loc
+            if k_loc > 0 and wide:
+                wws = self._buf('topk_wide_ws', (nat.sim_topk_wide_workspace_bytes(q, n_window), ), torch.uint8, dev)
+                nat.sim_topk_wide(bank.k_hi[w0:], bank.k_lo[w0:], bank.neg_s[w0:], n_window, lead, q_hi, q_lo, bsq, q,
+                                  self.CK, k_loc, wws, l_idx, l_w, pitch, None, 0, None, None, 0, False, False,
+                                  out_sim=l_sim)
+            elif k_loc > 0:
                 nat.sim_topk(bank.k_hi[w0:], bank.k_lo[w0:], bank.neg_s[w0:], n_window, lead, q_hi, q_lo, bsq, q, self.CK,
                              k_loc, ws, l_idx, l_w, None, 0, None, None, 0, False, False, out_sim=l_sim, prev_idx=prev,
                              thr_ws=thr_ws)
+            if k_loc > 0:
                 g_idx = torch.where(col < k_loc, l_idx + self.rank * stride, torch.full_like(l_idx, -1))
             else:
                 l_sim.fill_(float('-inf'))
                 g_idx = torch.full_like(l_idx, -1)
             all_v = self._all_gather(l_sim.t().contiguous())
             all_i = self._all_gather(g_idx.t().contiguous())
-            nat.merge_lists(all_v, all_i, self.world, self.top_k, q, q, g_sel, g_w)
+            if wide:
+                nat.merge_lists_wide(all_v, all_i, self.world, pitch, self.top_k, q, q, g_sel, g_w)
+            else:
+                nat.merge_lists(all_v, all_i, self.world, self.top_k, q, q, g_sel, g_w)
             idx_loc, w_loc = localise(g_sel, g_w, self.rank * stride, self.rank * stride + n_window)
             if self.use_long_term and n_loc > 0:  # usage of MY slots under the global softmax (kv_memory_store.py:118-125)
                 count_long = self.count_long_term_usage and bank.long_size > 0
@@ -196,14 +211,19 @@ class ShardedMemoryManager(MemoryManager):
                 bank.use_cnt.index_add_(0, phys, wv)
                 bank.life_cnt[lo:bank.hi] += 1
             if n_loc > 0:
-                rws = self._buf('readout_ws', (nat.readout_sparse_workspace_bytes(q, n_window), ), torch.uint8, dev)
+                rws_bytes = nat.readout_sparse_wide_workspace_bytes(q, n_window, pitch) if wide else \
+                    nat.readout_sparse_workspace_bytes(q, n_window)
+                rws = self._buf('readout_ws', (rws_bytes, ), torch.uint8, dev)
                 objs = bank.objects
                 for i in range(0, len(objs), nat.MAX_GROUPS):
                     part = objs[i:i + nat.MAX_GROUPS]
-                    nat.readout_sparse_scatter(bank.values[:, :, w0:], bank.cap, bank.values.shape[0] * self.CV,
-                                               [bank.slot_of[o] * self.CV for o in part],
-                                               [(order[o] % per) * self.CV for o in part], [order[o] // per for o in part],
-                                               self.CV, idx_loc, w_loc, pitch, n_window, q, rws, peers.ptrs, q)
+                    args = (bank.values[:, :, w0:], bank.cap, bank.values.shape[0] * self.CV,
+                            [bank.slot_of[o] * self.CV for o in part], [(order[o] % per) * self.CV for o in part],
+                            [order[o] // per for o in part], self.CV, idx_loc, w_loc)
+                    if wide:
+                        nat.readout_sparse_scatter_wide(*args, pitch, pitch, n_window, q, rws, peers.ptrs, q)
+                    else:
+                        nat.readout_sparse_scatter(*args, pitch, n_window, q, rws, peers.ptrs, q)
         if self.world > 1:  # every rank's adds are complete before anyone consumes its buffer
             fence = torch.zeros(1, device=dev)
             dist.all_reduce(fence, group=self.group)

@@ -5,7 +5,8 @@ The reference has no counterpart (its long-video answer is consolidation); the m
 (deva/model/memory_utils.py:6-76, memory_manager.py:64-75) evaluated distributedly:
 
   1. every rank runs the fused similarity/top-k kernel on ITS slots -> local top-k (similarity, slot) per query;
-  2. all-gather of those lists (Q x 32 x 8 B per rank - ~2 MB at 1080p) over NCCL/NVLink;
+  2. all-gather of those lists (Q x 32 x 8 B per rank - ~2 MB at 1080p; Q x pitch x 8 B for top_k > 32, pitch = top_k
+     rounded up to 32) over NCCL/NVLink;
   3. every rank merges the R lists with the same kernel that merges intra-GPU splits -> identical global top-k
      set and softmax weights everywhere (a plain max/sum all-reduce would not do: the softmax is over the
      GLOBAL top-k set);
@@ -133,10 +134,16 @@ class ShardedBankReader:
             self._scratch[name] = cur
         return cur[:need].view(*shape)
 
-    def read(self, qk: torch.Tensor, qe: torch.Tensor, count_usage: bool = True) -> torch.Tensor:
-        """qk/qe fp32 [CK, Q] (replicated on every rank) -> readout fp32 [K*CV, Q] (identical on every rank)."""
-        q = qk.shape[1]
-        pitch = nat.LIST_PITCH
+    def _readout_ws_bytes(self, q: int, pitch: int) -> int:
+        if pitch > nat.LIST_PITCH:
+            return nat.readout_sparse_wide_workspace_bytes(q, self.n, pitch)
+        return nat.readout_sparse_workspace_bytes(q, self.n)
+
+    def _global_topk(self, qk: torch.Tensor, qe: torch.Tensor, q: int):
+        """Steps 1-3 of a read -> (global slot ids [q, pitch], softmax weights [q, pitch], pitch).  top_k > 32 keeps
+        up to top_k local candidates per rank in lists of the wider pitch and merges them with the wide kernel."""
+        wide = self.top_k > nat.LIST_PITCH
+        pitch = nat.list_pitch(self.top_k)
         q_hi = self._buf('q_hi', (q, 2 * self.ck), torch.float16)
         q_lo = self._buf('q_lo', (q, 2 * self.ck), torch.float16)
         bsq = self._buf('bsq', (q, ), torch.float32)
@@ -147,9 +154,14 @@ class ShardedBankReader:
         l_sim = self._buf('l_sim', (q, pitch), torch.float32)
         k_loc = min(self.top_k, self.n)
         if k_loc > 0:
-            ws = self._buf('ws', (nat.simtopk_workspace_bytes(q), ), torch.uint8)
-            nat.sim_topk(self.k_hi, self.k_lo, self.neg_s, self.n, 0, q_hi, q_lo, bsq, q, self.ck, k_loc, ws, l_idx, l_w,
-                         None, 0, None, None, 0, False, False, out_sim=l_sim)
+            if wide:
+                ws = self._buf('ws_wide', (nat.sim_topk_wide_workspace_bytes(q, self.n), ), torch.uint8)
+                nat.sim_topk_wide(self.k_hi, self.k_lo, self.neg_s, self.n, 0, q_hi, q_lo, bsq, q, self.ck, k_loc, ws,
+                                  l_idx, l_w, pitch, None, 0, None, None, 0, False, False, out_sim=l_sim)
+            else:
+                ws = self._buf('ws', (nat.simtopk_workspace_bytes(q), ), torch.uint8)
+                nat.sim_topk(self.k_hi, self.k_lo, self.neg_s, self.n, 0, q_hi, q_lo, bsq, q, self.ck, k_loc, ws, l_idx,
+                             l_w, None, 0, None, None, 0, False, False, out_sim=l_sim)
             valid = torch.arange(pitch, device=self.dev).view(1, -1) < k_loc
             g_idx = torch.where(valid, l_idx + self.offset, torch.full_like(l_idx, -1))
         else:
@@ -165,22 +177,36 @@ class ShardedBankReader:
             dist.all_gather_into_tensor(all_i, mine_i, group=self.group)
         else:
             all_v, all_i = mine_v.unsqueeze(0), mine_i.unsqueeze(0)
-        # 3. global top-k + softmax (same result on every rank)
+        # 3. global top-k + softmax
         g_sel = self._buf('g_sel', (q, pitch), torch.int32)
         g_w = self._buf('g_w', (q, pitch), torch.float32)
-        nat.merge_lists(all_v, all_i, self.world, self.top_k, q, q, g_sel, g_w)
+        if wide:
+            nat.merge_lists_wide(all_v, all_i, self.world, pitch, self.top_k, q, q, g_sel, g_w)
+        else:
+            nat.merge_lists(all_v, all_i, self.world, self.top_k, q, q, g_sel, g_w)
+        return g_sel, g_w, pitch
+
+    def read(self, qk: torch.Tensor, qe: torch.Tensor, count_usage: bool = True) -> torch.Tensor:
+        """qk/qe fp32 [CK, Q] (replicated on every rank) -> readout fp32 [K*CV, Q] (identical on every rank)."""
+        q = qk.shape[1]
+        # 1-3. global top-k + softmax (same result on every rank)
+        g_sel, g_w, pitch = self._global_topk(qk, qe, q)
         # 4. partial readout over the selected slots this rank owns
         idx_loc, w_loc = localise(g_sel, g_w, self.offset, self.offset + self.n)
         if count_usage and self.n > 0:
             self.use_cnt.index_add_(0, idx_loc.reshape(-1).long(), w_loc.reshape(-1))
         out = torch.zeros(self.k * self.cv, q, dtype=torch.float32, device=self.dev)
         if self.n > 0:
-            rws = self._buf('rws', (nat.readout_sparse_workspace_bytes(q, self.n), ), torch.uint8)
+            rws = self._buf('rws', (self._readout_ws_bytes(q, pitch), ), torch.uint8)
             rows = [i * self.cv for i in range(self.k)]
             for i in range(0, self.k, nat.MAX_GROUPS):
                 part = rows[i:i + nat.MAX_GROUPS]
-                nat.readout_sparse(self.values, self.ld, self.k * self.cv, part, part, self.cv, idx_loc, w_loc, pitch,
-                                   self.n, q, rws, out, q)
+                if pitch > nat.LIST_PITCH:
+                    nat.readout_sparse_wide(self.values, self.ld, self.k * self.cv, part, part, self.cv, idx_loc, w_loc,
+                                            pitch, pitch, self.n, q, rws, out, q)
+                else:
+                    nat.readout_sparse(self.values, self.ld, self.k * self.cv, part, part, self.cv, idx_loc, w_loc, pitch,
+                                       self.n, q, rws, out, q)
         # 5. sum of the partial readouts
         if self.world > 1:
             dist.all_reduce(out, op=dist.ReduceOp.SUM, group=self.group)
@@ -196,7 +222,6 @@ class ShardedBankReader:
         """qk/qe fp32 [CK, Q] (replicated) -> fp32 [K_own*CV, Q]: the COMPLETE readout of the objects this rank owns
         (``objects_of(rank)``), summed over every rank's slots inside the readout kernels' epilogues."""
         q = qk.shape[1]
-        pitch = nat.LIST_PITCH
         per = -(-self.k // self.world)
         peers = self._scratch.get('peers')
         if peers is None or peers.local.shape[1] != q:
@@ -206,45 +231,21 @@ class ShardedBankReader:
             peers = PeerBuffers((per * self.cv, q), self.dev, self.group)
             self._scratch['peers'] = peers
         peers.local.zero_()  # ordered before every remote add of this read by the all-gather below
-        q_hi = self._buf('q_hi', (q, 2 * self.ck), torch.float16)
-        q_lo = self._buf('q_lo', (q, 2 * self.ck), torch.float16)
-        bsq = self._buf('bsq', (q, ), torch.float32)
-        nat.pack_query(qk.contiguous(), qe.contiguous(), q, 1, self.ck, q, q_hi, q_lo, bsq)
-        l_idx = self._buf('l_idx', (q, pitch), torch.int32)
-        l_w = self._buf('l_w', (q, pitch), torch.float32)
-        l_sim = self._buf('l_sim', (q, pitch), torch.float32)
-        k_loc = min(self.top_k, self.n)
-        if k_loc > 0:
-            ws = self._buf('ws', (nat.simtopk_workspace_bytes(q), ), torch.uint8)
-            nat.sim_topk(self.k_hi, self.k_lo, self.neg_s, self.n, 0, q_hi, q_lo, bsq, q, self.ck, k_loc, ws, l_idx, l_w,
-                         None, 0, None, None, 0, False, False, out_sim=l_sim)
-            valid = torch.arange(pitch, device=self.dev).view(1, -1) < k_loc
-            g_idx = torch.where(valid, l_idx + self.offset, torch.full_like(l_idx, -1))
-        else:
-            l_sim.fill_(float('-inf'))
-            g_idx = torch.full_like(l_idx, -1)
-        mine_v, mine_i = l_sim.t().contiguous(), g_idx.t().contiguous()
-        if self.world > 1:
-            all_v = torch.empty(self.world, pitch, q, dtype=torch.float32, device=self.dev)
-            all_i = torch.empty(self.world, pitch, q, dtype=torch.int32, device=self.dev)
-            dist.all_gather_into_tensor(all_v, mine_v, group=self.group)
-            dist.all_gather_into_tensor(all_i, mine_i, group=self.group)
-        else:
-            all_v, all_i = mine_v.unsqueeze(0), mine_i.unsqueeze(0)
-        g_sel = self._buf('g_sel', (q, pitch), torch.int32)
-        g_w = self._buf('g_w', (q, pitch), torch.float32)
-        nat.merge_lists(all_v, all_i, self.world, self.top_k, q, q, g_sel, g_w)
+        g_sel, g_w, pitch = self._global_topk(qk, qe, q)
         idx_loc, w_loc = localise(g_sel, g_w, self.offset, self.offset + self.n)
         if count_usage and self.n > 0:
             self.use_cnt.index_add_(0, idx_loc.reshape(-1).long(), w_loc.reshape(-1))
         if self.n > 0:
-            rws = self._buf('rws', (nat.readout_sparse_workspace_bytes(q, self.n), ), torch.uint8)
+            rws = self._buf('rws', (self._readout_ws_bytes(q, pitch), ), torch.uint8)
             objs = list(range(self.k))
             for i in range(0, self.k, nat.MAX_GROUPS):
                 part = objs[i:i + nat.MAX_GROUPS]
-                nat.readout_sparse_scatter(self.values, self.ld, self.k * self.cv, [o * self.cv for o in part],
-                                           [(o % per) * self.cv for o in part], [o // per for o in part], self.cv,
-                                           idx_loc, w_loc, pitch, self.n, q, rws, peers.ptrs, q)
+                args = (self.values, self.ld, self.k * self.cv, [o * self.cv for o in part],
+                        [(o % per) * self.cv for o in part], [o // per for o in part], self.cv, idx_loc, w_loc)
+                if pitch > nat.LIST_PITCH:
+                    nat.readout_sparse_scatter_wide(*args, pitch, pitch, self.n, q, rws, peers.ptrs, q)
+                else:
+                    nat.readout_sparse_scatter(*args, pitch, self.n, q, rws, peers.ptrs, q)
         if self.world > 1:  # every rank's adds have been issued and completed before anyone consumes its buffer
             fence = self._buf('fence', (1, ), torch.float32)
             fence.zero_()
