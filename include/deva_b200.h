@@ -27,7 +27,9 @@
 extern "C" {
 #endif
 
-/* v28: deva_b200_sim_topk_wide(_workspace_bytes), deva_b200_merge_lists_wide, deva_b200_readout_sparse_wide(_workspace_bytes)
+/* v29: deva_b200_sam_mask_stats, deva_b200_sam_mask_compact, deva_b200_sam_nms(_workspace_bytes) and
+ * deva_b200_sam_mask_write (Segment Anything's automatic masks from the low-resolution logits).
+ * v28: deva_b200_sim_topk_wide(_workspace_bytes), deva_b200_merge_lists_wide, deva_b200_readout_sparse_wide(_workspace_bytes)
  * and deva_b200_readout_sparse_scatter_wide (memory reads at any top_k, top-k lists at a caller-given pitch ld_list).
  * v27: deva_b200_conv2d takes flat spatial tiles, th = 0 and tw = 128 (stride 1, no out_pool4): 128 consecutive output
  * pixels of one image in row-major order.
@@ -53,7 +55,7 @@ extern "C" {
  * v12: deva_b200_ingest_rgb8_resize and deva_b200_mask_nearest (frame and first-frame mask resized on the device).
  * v11: deva_b200_cbam / deva_b200_cbam_split take a larger scratch buffer (64 pooling slices) and require c = 8 x a divisor
  * of 256; deva_b200_conv2d requires cout_pad <= 2048 (<= 1024 with a rank-1 input): the layer's bias lives in shared memory. */
-#define DEVA_B200_ABI_VERSION 28
+#define DEVA_B200_ABI_VERSION 29
 #define DEVA_B200_LIST_PITCH 32 /* row pitch of deva_b200_sim_topk's outputs == its max top_k (wider: the _wide calls) */
 #define DEVA_B200_MAX_GROUPS 256 /* objects per deva_b200_readout call */
 #define DEVA_B200_MAX_SEGMENT_CHANNELS 8192 /* channels per deva_b200_prob_to_segments call */
@@ -553,6 +555,36 @@ DEVA_B200_API int deva_b200_jpeg_decode(const uint8_t* scans, const int64_t* des
                                         const int64_t* intervals, int64_t n_intervals, const int64_t* subs,
                                         int64_t n_subs, uint8_t* out, void* workspace, int32_t* status,
                                         deva_stream_t stream);
+
+/* ---- Segment Anything automatic masks (deva/ext/sam_masks.py; DESIGN §7) -------------------------------------------
+ * logits fp32 [n, lh, lw] contiguous: the mask decoder's low-resolution logits.  Every value below is Sam.postprocess_masks'
+ * float32 value at a frame pixel: torch's CUDA bilinear upsample (align_corners=False) of the logits to [grid, grid],
+ * cropped to [in_h, in_w], then the same upsample to [out_h, out_w].  1 <= in_h, in_w <= grid <= 1024, out_h * out_w
+ * < 2^31; n <= 65535.
+ * sam_mask_stats: stats int32 [n, 7] per mask {pixels > thr_hi, > thr_lo, > thr, x0, y0, x1, y1}, the box being the
+ * extent of the pixels > thr (x1 = y1 = -1 when there are none).  With iou (fp32 [n], optional), a mask whose
+ * iou > iou_thresh fails is not evaluated and its counts stay 0.
+ * sam_mask_compact: one CTA.  stability[i] = float(count > thr_hi) / float(count > thr_lo) (nan for 0 / 0); boxes i64
+ * [n, 4] = {x0, y0, x1, y1}, or zeros for a mask with no pixel > thr; kept int32 [n + 1]: kept[0] = the number of masks
+ * with iou > iou_thresh (when iou is given) and stability >= stability_thresh (when stability_thresh > 0), then their
+ * indices in ascending order.
+ * sam_nms: torchvision's CUDA nms of boxes fp32 [n, 4] (x0, y0, x1, y1) by scores fp32 [n]: a stable descending sort of
+ * the scores, IoU = inter / (area_a + area_b - inter) in float32, a box suppressed when its IoU with a kept box of
+ * higher rank is > iou_thresh.  keep i64 [n]: the kept indices in rank order, the first *n_keep valid.  workspace:
+ * deva_b200_sam_nms_workspace_bytes(n) bytes, 16-byte aligned.
+ * sam_mask_write: out bool [n, out_h, out_w]: mask m is the value of logits[sel[m]] > thr (sel i64 [n]). */
+DEVA_B200_API int deva_b200_sam_mask_stats(const float* logits, int n, int lh, int lw, int grid, int in_h, int in_w,
+                                           int out_h, int out_w, const float* iou, float iou_thresh, float thr_hi,
+                                           float thr_lo, float thr, int32_t* stats, deva_stream_t stream);
+DEVA_B200_API int deva_b200_sam_mask_compact(const int32_t* stats, const float* iou, int n, float iou_thresh,
+                                             float stability_thresh, float* stability, int64_t* boxes, int32_t* kept,
+                                             deva_stream_t stream);
+DEVA_B200_API size_t deva_b200_sam_nms_workspace_bytes(int n);
+DEVA_B200_API int deva_b200_sam_nms(const float* boxes, const float* scores, int n, float iou_thresh, void* workspace,
+                                    int64_t* keep, int32_t* n_keep, deva_stream_t stream);
+DEVA_B200_API int deva_b200_sam_mask_write(const float* logits, const int64_t* sel, int n, int lh, int lw, int grid,
+                                           int in_h, int in_w, int out_h, int out_w, float thr, uint8_t* out,
+                                           deva_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'csrc', 'libdeva_b200.so')
-ABI_VERSION = 28
+ABI_VERSION = 29
 LIST_PITCH = 32
 MAX_GROUPS = 256
 MAX_SEGMENT_CHANNELS = 8192
@@ -148,6 +148,15 @@ _SIGNATURES = {
     'deva_b200_jpeg_decode_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int, c_int64]),
     'deva_b200_jpeg_decode': (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p,
                                       c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'deva_b200_sam_mask_stats': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                         ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, c_void_p,
+                                         c_void_p]),
+    'deva_b200_sam_mask_compact': (c_int, [c_void_p, c_void_p, c_int, ctypes.c_float, ctypes.c_float, c_void_p,
+                                           c_void_p, c_void_p, c_void_p]),
+    'deva_b200_sam_nms_workspace_bytes': (c_size_t, [c_int]),
+    'deva_b200_sam_nms': (c_int, [c_void_p, c_void_p, c_int, ctypes.c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
+    'deva_b200_sam_mask_write': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                         ctypes.c_float, c_void_p, c_void_p]),
 }
 EXPORTS = tuple(_SIGNATURES.keys())
 
@@ -700,3 +709,52 @@ def transpose_append(src, dst, ld_dst, n, c):
 
 def head_gather3x3(z, out, bias, b, h, w):
     _check(lib().deva_b200_head_gather3x3(_ptr(z), _ptr(out), float(bias), b, h, w, _stream()), 'head_gather3x3')
+
+
+SAM_STATS = 7  # per mask: > thr + offset, > thr - offset, > thr, x0, y0, x1, y1
+
+
+def _sam_logits(logits):
+    assert logits.dtype == torch.float32 and logits.is_cuda and logits.is_contiguous() and logits.dim() == 3, \
+        (logits.dtype, logits.shape)
+    return logits.shape
+
+
+def sam_mask_stats(logits, grid, in_h, in_w, out_h, out_w, iou, iou_thresh, thr_hi, thr_lo, thr, stats):
+    """logits float32 [n, lh, lw]; iou float32 [n] or None; stats int32 [n, 7] (see include/deva_b200.h)."""
+    n, lh, lw = _sam_logits(logits)
+    assert stats.dtype == torch.int32 and stats.is_contiguous() and stats.shape == (n, SAM_STATS)
+    assert iou is None or (_f32(iou).is_contiguous() and iou.numel() == n)
+    _check(lib().deva_b200_sam_mask_stats(_ptr(logits), n, lh, lw, grid, in_h, in_w, out_h, out_w, _ptr(iou),
+                                          iou_thresh, thr_hi, thr_lo, thr, _ptr(stats), _stream()), 'sam_mask_stats')
+
+
+def sam_mask_compact(stats, iou, iou_thresh, stability_thresh, stability, boxes, kept):
+    """stats int32 [n, 7] -> stability float32 [n], boxes int64 [n, 4], kept int32 [n + 1] (count, then indices)."""
+    n = stats.shape[0]
+    assert stats.dtype == torch.int32 and stats.is_contiguous() and stats.shape == (n, SAM_STATS)
+    assert iou is None or (_f32(iou).is_contiguous() and iou.numel() == n)
+    assert _f32(stability).numel() == n and boxes.dtype == torch.int64 and boxes.shape == (n, 4)
+    assert kept.dtype == torch.int32 and kept.numel() == n + 1
+    _check(lib().deva_b200_sam_mask_compact(_ptr(stats), _ptr(iou), n, iou_thresh, stability_thresh, _ptr(stability),
+                                            _ptr(boxes), _ptr(kept), _stream()), 'sam_mask_compact')
+
+
+def sam_nms(boxes, scores, iou_thresh, keep, n_keep):
+    """boxes float32 [n, 4], scores float32 [n] -> keep int64 [n] (the first n_keep[0] valid), n_keep int32 [1]."""
+    n = scores.numel()
+    assert _f32(boxes).is_contiguous() and boxes.shape == (n, 4) and _f32(scores).is_contiguous()
+    assert keep.dtype == torch.int64 and keep.numel() >= n and n_keep.dtype == torch.int32
+    ws = torch.empty(int(lib().deva_b200_sam_nms_workspace_bytes(n)), dtype=torch.uint8, device=scores.device)
+    _check(lib().deva_b200_sam_nms(_ptr(boxes), _ptr(scores), n, iou_thresh, _ptr(ws), _ptr(keep), _ptr(n_keep),
+                                   _stream()), 'sam_nms')
+
+
+def sam_mask_write(logits, sel, grid, in_h, in_w, out_h, out_w, thr, out):
+    """out bool [n, out_h, out_w]: logits[sel[m]] upsampled twice, > thr; sel int64 [n]."""
+    _, lh, lw = _sam_logits(logits)
+    n = sel.numel()
+    assert sel.dtype == torch.int64 and sel.is_cuda and sel.is_contiguous()
+    assert out.dtype == torch.bool and out.is_contiguous() and out.shape == (n, out_h, out_w)
+    _check(lib().deva_b200_sam_mask_write(_ptr(logits), _ptr(sel), n, lh, lw, grid, in_h, in_w, out_h, out_w, thr,
+                                          _ptr(out), _stream()), 'sam_mask_write')

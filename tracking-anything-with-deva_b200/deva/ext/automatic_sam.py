@@ -3,6 +3,7 @@
 ``segment_anything`` and the ``deva.ext.SAM`` / ``deva.ext.MobileSAM`` modules are imported by ``get_sam_model`` only,
 so importing this module needs neither and does not initialise CUDA.
 """
+import os
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -13,9 +14,16 @@ from deva.ext.detector_masks import host_image, output_size, scored_id_map
 from deva.inference.object_info import ObjectInfo
 
 
-def get_sam_model(config: Dict, device: str):
-    """SAM's automatic mask generator for config['sam_variant'] ('mobile' or 'original')."""
-    from deva.ext.SAM.automatic_mask_generator import SamAutomaticMaskGenerator
+def get_sam_model(config: Dict, device: str, *, mask_generator: Optional[str] = None):
+    """SAM's automatic mask generator for config['sam_variant'] ('mobile' or 'original').
+
+    mask_generator: 'reference' (the reference's SamAutomaticMaskGenerator) or 'device' (deva.ext.sam_masks'
+    DeviceMaskGenerator on the same model: the same masks, with the post-processing on the device); None reads
+    DEVA_B200_SAM_MASK_GENERATOR (default 'reference')."""
+    if mask_generator is None:
+        mask_generator = os.environ.get('DEVA_B200_SAM_MASK_GENERATOR', 'reference')
+    if mask_generator not in ('reference', 'device'):
+        raise ValueError(f"mask_generator must be 'reference' or 'device', not {mask_generator!r}")
     variant = config['sam_variant'].lower()
     if variant == 'mobile':
         from deva.ext.MobileSAM.setup_mobile_sam import setup_model as setup_mobile_sam
@@ -29,10 +37,14 @@ def get_sam_model(config: Dict, device: str):
             device=device)
     else:
         raise ValueError(f'Unknown SAM variant: {config["SAM_VARIANT"]}')
-    return SamAutomaticMaskGenerator(model,
-                                     points_per_side=config['SAM_NUM_POINTS_PER_SIDE'],
-                                     points_per_batch=config['SAM_NUM_POINTS_PER_BATCH'],
-                                     pred_iou_thresh=config['SAM_PRED_IOU_THRESHOLD'])
+    if mask_generator == 'device':
+        from deva.ext.sam_masks import DeviceMaskGenerator as Generator
+    else:
+        from deva.ext.SAM.automatic_mask_generator import SamAutomaticMaskGenerator as Generator
+    return Generator(model,
+                     points_per_side=config['SAM_NUM_POINTS_PER_SIDE'],
+                     points_per_batch=config['SAM_NUM_POINTS_PER_BATCH'],
+                     pred_iou_thresh=config['SAM_PRED_IOU_THRESHOLD'])
 
 
 def _positive_points(config: Dict, forward_mask: torch.Tensor, device) -> np.ndarray:
